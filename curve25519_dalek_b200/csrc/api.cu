@@ -133,20 +133,22 @@ static int run_msm(dalek_b200_ctx *ctx, const void *scalars, const void *points_
                    ge_p3_raw *d_windows, int *bad_out, MsmResult *d_result)
 {
     int rc;
-    const int kind = point_fmt == DALEK_POINTS_COMPRESSED ? PK_NIELS : PK_PNIELS;
-    const size_t psz = kind == PK_NIELS ? sizeof(ge_niels_packed) : sizeof(ge_pniels_packed);
     const size_t pin = point_in_bytes(point_fmt);
     cudaStream_t st = ctx->stream;
-    if ((rc = ws_reserve(ctx, ctx->points, std::max<size_t>(1, n) * psz))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->flags, 64))) return rc;
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->flags.p, 0, 64, st));
     const int c = msm_choose_window_bits(ctx, n_window);
     // the reference's dispatch (edwards.rs:1025-1029): below 190 points vartime Straus -- here three launches
     // (straus_vt.cu) instead of the ~27 of the bucket pipeline; only for whole MSMs (a shard must yield window sums)
     const bool straus = d_result && n == n_window && n < STRAUS_VT_THRESHOLD && ctx->opt_small_straus && ctx->opt_field_f64;
+    // the bucket kernel reads affine Niels; Straus builds its own tables and keeps extended inputs projective, as an
+    // inversion would only lengthen its latency-bound path
+    const int kind = msm_prepared_kind(point_fmt, straus ? PK_PNIELS : PK_NIELS);
+    const size_t psz = kind == PK_NIELS ? sizeof(ge_niels_packed) : sizeof(ge_pniels_packed);
+    if ((rc = ws_reserve(ctx, ctx->points, std::max<size_t>(1, n) * psz))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->flags, 64))) return rc;
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->flags.p, 0, 64, st));
     if (on_device) {
         if (straus) {
-            if ((rc = msm_prepare_points(ctx, points_in, point_fmt, n, ctx->points.p, (int *)ctx->flags.p))) return rc;
+            if ((rc = msm_prepare_points(ctx, points_in, point_fmt, n, ctx->points.p, (int *)ctx->flags.p, kind))) return rc;
             if ((rc = straus_vartime_msm(ctx, (const uint32_t *)scalars, ctx->points.p, kind, n, d_result))) return rc;
         } else {
             // the point conversion (or decompression) runs on the second stream under the digit / sort passes of the main one
@@ -154,7 +156,7 @@ static int run_msm(dalek_b200_ctx *ctx, const void *scalars, const void *points_
             CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->ev_fork, 0));
             if ((rc = msm_prepare_points_on(ctx, ctx->stream2, points_in, point_fmt, n, ctx->points.p, (int *)ctx->flags.p))) return rc;
             CUDA_TRY(ctx, cudaEventRecord(ctx->ev_join, ctx->stream2));
-            if ((rc = msm_accumulate_chunk(ctx, (const uint32_t *)scalars, ctx->points.p, kind, n, c, true, 0, 0, ctx->ev_join))) return rc;
+            if ((rc = msm_accumulate_chunk(ctx, (const uint32_t *)scalars, (const ge_niels_packed *)ctx->points.p, n, c, true, 0, 0, ctx->ev_join))) return rc;
         }
     } else {
         if ((rc = ws_reserve(ctx, ctx->scalars, std::max<size_t>(1, n) * 32))) return rc;
@@ -162,6 +164,7 @@ static int run_msm(dalek_b200_ctx *ctx, const void *scalars, const void *points_
         int K = n >= (1u << 18) ? (int)std::min<long>(8, std::max<long>(1, ctx->opt_host_chunks)) : 1;
         CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, st));
         CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream_copy, ctx->ev_fork, 0));
+        CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->ev_fork, 0));
         // equal pieces: every piece re-runs the per-bucket passes (scans, task lists) and revisits all bucket sums,
         // in exchange for more copy / compute overlap (tools/sweep_msm_options.py times 1, 2, 4 and 8 chunks)
         for (int k = 0; k < K; k++) {
@@ -174,10 +177,17 @@ static int run_msm(dalek_b200_ctx *ctx, const void *scalars, const void *points_
             CUDA_TRY(ctx, cudaEventRecord(ctx->ev_grp[k], ctx->stream_copy));
             CUDA_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_grp[k], 0));
             char *dq = (char *)ctx->points.p + i0 * psz;
-            if ((rc = msm_prepare_points(ctx, dp, point_fmt, cnt, dq, (int *)ctx->flags.p))) return rc;
             if (straus) {                                            // K = 1 for small inputs
+                if ((rc = msm_prepare_points(ctx, dp, point_fmt, cnt, dq, (int *)ctx->flags.p, kind))) return rc;
                 if ((rc = straus_vartime_msm(ctx, (const uint32_t *)ds, dq, kind, cnt, d_result))) return rc;
-            } else if ((rc = msm_accumulate_chunk(ctx, (const uint32_t *)ds, dq, kind, cnt, c, k == 0))) return rc;
+            } else {
+                // as for device inputs: the chunk's points are converted on the second stream while its digit / sort
+                // passes run on the main one (the normalisation's inversions would otherwise sit on the critical path)
+                CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->ev_grp[k], 0));
+                if ((rc = msm_prepare_points_on(ctx, ctx->stream2, dp, point_fmt, cnt, dq, (int *)ctx->flags.p))) return rc;
+                CUDA_TRY(ctx, cudaEventRecord(ctx->ev_join, ctx->stream2));
+                if ((rc = msm_accumulate_chunk(ctx, (const uint32_t *)ds, (const ge_niels_packed *)dq, cnt, c, k == 0, 0, 0, ctx->ev_join))) return rc;
+            }
         }
     }
     if (!straus && (rc = msm_reduce_finish(ctx, c, d_windows, d_result))) return rc;

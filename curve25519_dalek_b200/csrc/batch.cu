@@ -781,13 +781,13 @@ static int verify_equation(dalek_b200_ctx *ctx, const VerifyBufs &b, size_t n, s
     if ((rc = ws_reserve(ctx, ctx->misc0, (size_t)nwin * sizeof(ge_p3_raw)))) return rc;
     if ((rc = ws_reserve(ctx, ctx->result, sizeof(MsmResult)))) return rc;
     if (merged || cnt == n) {
-        if ((rc = msm_accumulate_chunk(ctx, b.scalars, b.points, PK_NIELS, nlong, c, true))) return rc;
+        if ((rc = msm_accumulate_chunk(ctx, b.scalars, b.points, nlong, c, true))) return rc;
     } else {           // one term per signature, sub-range: the basepoint term, then the keys of the range
-        if ((rc = msm_accumulate_chunk(ctx, b.scalars, b.points, PK_NIELS, 1, c, true))) return rc;
-        if (cnt && (rc = msm_accumulate_chunk(ctx, b.scalars + 8 * (1 + lo), b.points + 1 + lo, PK_NIELS, cnt, c, false))) return rc;
+        if ((rc = msm_accumulate_chunk(ctx, b.scalars, b.points, 1, c, true))) return rc;
+        if (cnt && (rc = msm_accumulate_chunk(ctx, b.scalars + 8 * (1 + lo), b.points + 1 + lo, cnt, c, false))) return rc;
     }
     trace_mark(ctx, "key chunk accumulated", st);
-    if (cnt && (rc = msm_accumulate_chunk(ctx, b.scalars + 8 * (1 + n + lo), b.points + 1 + n + lo, PK_NIELS, cnt, c, false, (128 + c) / c))) return rc;
+    if (cnt && (rc = msm_accumulate_chunk(ctx, b.scalars + 8 * (1 + n + lo), b.points + 1 + n + lo, cnt, c, false, (128 + c) / c))) return rc;
     trace_mark(ctx, "R chunk accumulated", st);
     if ((rc = msm_reduce_finish(ctx, c, (ge_p3_raw *)ctx->misc0.p, (MsmResult *)ctx->result.p))) return rc;
     trace_mark(ctx, "reduced and combined", st);

@@ -131,36 +131,40 @@ int ws_reserve(dalek_b200_ctx *ctx, DevBuf &b, size_t bytes);
 int pinned_reserve(dalek_b200_ctx *ctx, size_t bytes);
 
 // ---- point preparation (msm.cu) ----
-// kinds of device point arrays fed to the bucket kernels
+// kinds of prepared device point arrays: the bucket kernel reads PK_NIELS only; the vartime Straus path takes either
 enum { PK_NIELS = 0 /* ge_niels_packed, 96 B */, PK_PNIELS = 1 /* ge_pniels_packed, 128 B */ };
 
 // Convert n input points (device memory, format DALEK_POINTS_*) into packed Niels form.
-// Compressed inputs give PK_NIELS and set *d_bad (device int) nonzero if any fails to decode;
-// extended inputs give PK_PNIELS.
+// Compressed inputs give affine Niels (decompression yields Z = 1) and set *d_bad (device int) nonzero if any fails
+// to decode.  Extended inputs give affine Niels too, normalised to Z = 1 with one inversion per 1024 points; with
+// kind = PK_PNIELS they give projective Niels instead (no inversion, for the latency-bound Straus path).
+// msm_prepared_kind tells which kind a format and a requested kind give.
 int msm_prepare_points(dalek_b200_ctx *ctx, const void *d_in, int point_fmt, size_t n, void *d_out,
-                       int *d_bad);
+                       int *d_bad, int kind = PK_NIELS);
+int msm_prepared_kind(int point_fmt, int kind);
 
 // Window width (bits) the engine uses for an MSM over n pairs.
 int msm_choose_window_bits(const dalek_b200_ctx *ctx, size_t n);
 int msm_window_count_for_bits(int c);
 
 // Bucket MSM over device inputs: writes `nwin` window accumulators (raw p3) to d_windows.
-int msm_window_sums(dalek_b200_ctx *ctx, const uint32_t *d_scalars /* n x 8 words */, const void *d_points,
-                    int point_kind, size_t n, int c, ge_p3_raw *d_windows);
+int msm_window_sums(dalek_b200_ctx *ctx, const uint32_t *d_scalars /* n x 8 words */, const ge_niels_packed *d_points,
+                    size_t n, int c, ge_p3_raw *d_windows);
 // total = sum over ranks of windows, Horner-combined; writes compressed (8 words) + canonical
 // limbs51 (20 u64) + identity flag to d_result (layout: 8 u32 | pad | 20 u64 | u32 flag).
 struct MsmResult { uint32_t compressed[8]; uint64_t limbs[20]; uint32_t is_identity; uint32_t pad; };
 // building blocks: one chunk of pairs into the buckets; then reduction (+ Horner + encode if d_result)
 // points_ready (optional): an event after which d_points may be read -- the digit and sort passes do not wait for it
-int msm_accumulate_chunk(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const void *d_points, int point_kind, size_t n,
+int msm_accumulate_chunk(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const ge_niels_packed *d_points, size_t n,
                          int c, bool first, int active_windows = 0, size_t flat = 0, cudaEvent_t points_ready = nullptr);
-int msm_prepare_points_on(dalek_b200_ctx *ctx, cudaStream_t st, const void *d_in, int point_fmt, size_t n, void *d_out, int *d_bad);
+int msm_prepare_points_on(dalek_b200_ctx *ctx, cudaStream_t st, const void *d_in, int point_fmt, size_t n, void *d_out, int *d_bad,
+                          int kind = PK_NIELS);
 // window width for `n_short` scalars of `short_bits` bits plus `n_long` full-width scalars (verify_batch)
 int msm_choose_window_bits_mixed(const dalek_b200_ctx *ctx, size_t n_short, int short_bits, size_t n_long);
 int msm_reduce_finish(dalek_b200_ctx *ctx, int c, ge_p3_raw *d_windows, MsmResult *d_result, bool flat = false);
 int msm_fill_identity(dalek_b200_ctx *ctx, ge_p3_raw *d_out, uint32_t count);
 // window sums + Horner + encode in one go (single-shard case)
-int msm_full(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const void *d_points, int point_kind, size_t n, int c,
+int msm_full(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const ge_niels_packed *d_points, size_t n, int c,
              ge_p3_raw *d_windows, MsmResult *d_result);
 int msm_combine_windows(dalek_b200_ctx *ctx, const ge_p3_raw *d_windows, int ranks, int nwin, int c,
                         MsmResult *d_result);

@@ -14,15 +14,15 @@
 //                       counting sort of the tasks by length: warps run equal trip counts and the
 //                       grid drains longest-first
 //   k_bucket_accumulate one thread per task: sum of its points with the complete unified mixed
-//                       addition (curve_models.rs:411-494), 7M (affine Niels) or 8M, on the
+//                       addition of an affine Niels point (curve_models.rs:411-494), 7M, on the
 //                       FP64-pipe field (fe64.cuh) with cp.async point prefetch
 //   k_heavy_fixup       sums the task sums of buckets that were cut
 //   k_chunk_reduce, k_plain_sum, k_finish_windows
 //                       sum_k k*B_k per window (pippenger.rs:146-151) in log depth on 4-lane groups
 //   k_combine           total = total*2^c + window (pippenger.rs:159), compress
 //
-// Data layout in HBM: scalars n x 32 B; points packed Niels (96 B) or projective Niels (128 B),
-// canonical 32-byte coordinates, 16-byte aligned for 128-bit loads; digit/rank entries 8 B per
+// Data layout in HBM: scalars n x 32 B; points packed affine Niels (96 B: every input format is normalised
+// to Z = 1 first), canonical 32-byte coordinates, 16-byte aligned for 128-bit loads; digit/rank entries 8 B per
 // (window, scalar); sorted indices 4 B per entry; bucket sums 160 B (10 x u32 limbs x 4).
 #include <algorithm>
 #include <cstdio>
@@ -80,7 +80,131 @@ __global__ void __launch_bounds__(128, 3) k_prep_compressed(const uint4 *__restr
     for (int k = 0; k < 6; k++) o[k] = make_uint4(p.w[4 * k], p.w[4 * k + 1], p.w[4 * k + 2], p.w[4 * k + 3]);
 }
 
-__global__ void k_prep_extended(const uint64_t *__restrict__ in, ge_pniels_packed *__restrict__ out, size_t n)
+// Extended points (X : Y : Z : T) -> affine Niels ((Y+X)/Z, (Y-X)/Z, 2d T/Z): the projective Niels point divided by Z,
+// so every input with Z != 0 stands for the same group element as before, T/Z = xy or not.  The bucket kernel then
+// adds every point with the 7M mixed addition in each of its ~16 windows instead of the 8M projective one, and
+// gathers 96 B per digit instead of 128 B.  The inversions use Montgomery's trick over the PREP_GROUP points of one
+// CTA (1024): a thread multiplies the Z of its PREP_PER_THREAD points, the lanes of a warp scan their products both ways
+// with shuffles, thread 0 inverts the product of the warp products (one inversion per CTA), and every thread then
+// walks its points backwards.  Z = 0 (not a point: bad limbs from the caller) is left out of the products, as
+// FieldElement::invert_batch skips zeros, and gives the identity; the other points of the group are unaffected.
+#define PREP_THREADS 128
+#define PREP_PER_THREAD 8
+#define PREP_GROUP (PREP_THREADS * PREP_PER_THREAD)      // points per inversion
+
+__device__ __forceinline__ void load_coord_f64(fe64 &h, const uint64_t *__restrict__ src)
+{
+    uint64_t l[5];
+#pragma unroll
+    for (int k = 0; k < 5; k++) l[k] = __ldg(src + k);
+    fe t; fe_from_limbs51(t, l);
+    fe64_from_fe_limbs(h, t);
+}
+__device__ __forceinline__ uint32_t fe64_nonzero(const fe64 &f)
+{
+    fe t; fe64_to_fe(t, f);
+    return 1u - (uint32_t)fe_iszero(t);
+}
+__device__ __forceinline__ void fe64_shfl_up(fe64 &o, const fe64 &f, int d)
+{
+#pragma unroll
+    for (int k = 0; k < 5; k++) o.v[k] = __shfl_up_sync(0xffffffffu, f.v[k], d);
+}
+__device__ __forceinline__ void fe64_shfl_down(fe64 &o, const fe64 &f, int d)
+{
+#pragma unroll
+    for (int k = 0; k < 5; k++) o.v[k] = __shfl_down_sync(0xffffffffu, f.v[k], d);
+}
+
+__global__ void __launch_bounds__(PREP_THREADS, 3)
+k_prep_extended(const uint64_t *__restrict__ in, ge_niels_packed *__restrict__ out, size_t n)
+{
+    constexpr int NW = PREP_THREADS / 32;
+    __shared__ fe64 s_warp[NW];                            // warp products, then their inverses
+    __shared__ fe64 s_pre[PREP_PER_THREAD][PREP_THREADS];  // running products, kept out of the registers
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const size_t g0 = (size_t)blockIdx.x * PREP_GROUP + tid;   // point k of this thread: g0 + k * PREP_THREADS
+    // running products pre[k] = Z_0 ... Z_k of this thread's points (zeros and points past n skipped)
+    fe64 acc;
+    uint32_t nz = 0;                                       // bit k: Z_k != 0
+    fe64_1(acc);
+#pragma unroll 1
+    for (int k = 0; k < PREP_PER_THREAD; k++) {
+        const size_t i = g0 + (size_t)k * PREP_THREADS;
+        if (i < n) {
+            fe64 z, t;
+            load_coord_f64(z, in + 20 * i + 10);
+            const uint32_t ok = fe64_nonzero(z);
+            fe64_mul(t, acc, z); fe64_cmov(acc, t, ok);
+            nz |= ok << k;
+        }
+        s_pre[k][tid] = acc;
+    }
+    // products of the lanes below (lo) and above (hi) this one
+    fe64 lo = acc, hi = acc, t;
+#pragma unroll 1
+    for (int d = 1; d < 32; d <<= 1) {
+        fe64_shfl_up(t, lo, d);
+        if (lane >= (uint32_t)d) fe64_mul(lo, lo, t);
+        fe64_shfl_down(t, hi, d);
+        if (lane + d < 32) fe64_mul(hi, hi, t);
+    }
+    if (lane == 31) s_warp[warp] = lo;
+    fe64_shfl_up(t, lo, 1); lo = t; if (lane == 0) fe64_1(lo);
+    fe64_shfl_down(t, hi, 1); hi = t; if (lane == 31) fe64_1(hi);
+    __syncthreads();
+    if (tid == 0) {                                        // Montgomery's trick on the NW warp products (never zero)
+        fe64 run[NW], inv;
+        run[0] = s_warp[0];
+#pragma unroll
+        for (int w = 1; w < NW; w++) fe64_mul(run[w], run[w - 1], s_warp[w]);
+        {   // on the integer field: the temporaries of the FP64 chain (fe64_pow22501) would make the kernel spill
+            fe q; fe64_to_fe(q, run[NW - 1]); fe_invert(q, q); fe64_from_fe_limbs(inv, q);
+        }
+#pragma unroll
+        for (int w = NW - 1; w > 0; w--) {
+            fe64 iw;
+            fe64_mul(iw, inv, run[w - 1]);
+            fe64_mul(inv, inv, s_warp[w]);
+            s_warp[w] = iw;
+        }
+        s_warp[0] = inv;
+    }
+    __syncthreads();
+    fe64 inv;                                              // 1 / pre[PREP_PER_THREAD - 1]
+    fe64_mul(inv, s_warp[warp], lo); fe64_mul(inv, inv, hi);
+#pragma unroll 1
+    for (int k = PREP_PER_THREAD - 1; k >= 0; k--) {       // invariant: inv = 1 / pre[k]
+        const size_t i = g0 + (size_t)k * PREP_THREADS;
+        if (i >= n) continue;
+        const uint32_t ok = (nz >> k) & 1u;
+        const uint64_t *src = in + 20 * i;
+        fe64 X, Y, zi, u, v;
+        load_coord_f64(u, src + 10);
+        if (k > 0) fe64_mul(zi, inv, s_pre[k - 1][tid]); else zi = inv;   // 1 / Z_k
+        fe64_mul(v, inv, u); fe64_cmov(inv, v, ok);
+        // each coordinate goes to its canonical bytes as soon as it is made (fewer live registers)
+        ge_niels_packed pk;
+        fe f;
+        load_coord_f64(X, src); load_coord_f64(Y, src + 5);
+        fe64_add(u, Y, X); fe64_mul(v, u, zi);                         // 2 x 1
+        fe64_to_fe(f, v); fe_tobytes_words(pk.w, f);
+        fe64_sub(u, Y, X); fe64_mul(v, u, zi);
+        fe64_to_fe(f, v); fe_tobytes_words(pk.w + 8, f);
+        load_coord_f64(u, src + 15);
+        fe64_mul(v, u, zi); fe64_const_2d(u); fe64_mul(v, v, u);
+        fe64_to_fe(f, v); fe_tobytes_words(pk.w + 16, f);
+#pragma unroll
+        for (int q = 0; q < 24; q++) pk.w[q] = ok ? pk.w[q] : (q == 0 || q == 8 ? 1u : 0u);   // Z = 0: the identity (1, 1, 0)
+        uint4 *o = reinterpret_cast<uint4 *>(out + i);
+#pragma unroll
+        for (int q = 0; q < 6; q++) o[q] = make_uint4(pk.w[4 * q], pk.w[4 * q + 1], pk.w[4 * q + 2], pk.w[4 * q + 3]);
+    }
+}
+
+// Extended points -> projective Niels (Y+X, Y-X, Z, 2dT), no inversion: for the latency-bound vartime Straus path,
+// which builds its own tables from the point
+__global__ void k_prep_extended_pniels(const uint64_t *__restrict__ in, ge_pniels_packed *__restrict__ out, size_t n)
 {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -97,23 +221,31 @@ __global__ void k_prep_extended(const uint64_t *__restrict__ in, ge_pniels_packe
     for (int k = 0; k < 8; k++) o[k] = make_uint4(pk.w[4 * k], pk.w[4 * k + 1], pk.w[4 * k + 2], pk.w[4 * k + 3]);
 }
 
-int msm_prepare_points_on(dalek_b200_ctx *ctx, cudaStream_t st, const void *d_in, int point_fmt, size_t n, void *d_out, int *d_bad)
+int msm_prepared_kind(int point_fmt, int kind)
+{
+    return point_fmt == DALEK_POINTS_EXTENDED ? kind : PK_NIELS;
+}
+
+int msm_prepare_points_on(dalek_b200_ctx *ctx, cudaStream_t st, const void *d_in, int point_fmt, size_t n, void *d_out, int *d_bad,
+                          int kind)
 {
     if (n == 0) return 0;
     if (point_fmt == DALEK_POINTS_COMPRESSED) {
         if (ctx->opt_decompress_f64) k_prep_compressed<1><<<cdiv(n, 128), 128, 0, st>>>((const uint4 *)d_in, (ge_niels_packed *)d_out, n, d_bad);
         else k_prep_compressed<0><<<cdiv(n, 128), 128, 0, st>>>((const uint4 *)d_in, (ge_niels_packed *)d_out, n, d_bad);
+    } else if (kind == PK_PNIELS) {
+        k_prep_extended_pniels<<<cdiv(n, 128), 128, 0, st>>>((const uint64_t *)d_in, (ge_pniels_packed *)d_out, n);
     } else {
-        k_prep_extended<<<cdiv(n, 128), 128, 0, st>>>((const uint64_t *)d_in, (ge_pniels_packed *)d_out, n);
+        k_prep_extended<<<cdiv(n, PREP_GROUP), PREP_THREADS, 0, st>>>((const uint64_t *)d_in, (ge_niels_packed *)d_out, n);
     }
     ctx->launches++;
     CUDA_TRY(ctx, cudaGetLastError());
     return 0;
 }
 
-int msm_prepare_points(dalek_b200_ctx *ctx, const void *d_in, int point_fmt, size_t n, void *d_out, int *d_bad)
+int msm_prepare_points(dalek_b200_ctx *ctx, const void *d_in, int point_fmt, size_t n, void *d_out, int *d_bad, int kind)
 {
-    return msm_prepare_points_on(ctx, ctx->stream, d_in, point_fmt, n, d_out, d_bad);
+    return msm_prepare_points_on(ctx, ctx->stream, d_in, point_fmt, n, d_out, d_bad, kind);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -385,19 +517,19 @@ __device__ __forceinline__ void load_p3(ge_p3 &p, const ge_p3_raw *src)
 }
 
 // TMA = 1: the gather of the next point is ONE bulk copy of the TMA unit (cp.async.bulk.shared.global, completion
-// on a per-thread mbarrier) instead of 6-8 16-byte cp.async (LDGSTS); tools/ab_tma.py is the A/B measurement.
-template <int KIND, int F64, int TMA>
+// on a per-thread mbarrier) instead of 6 16-byte cp.async (LDGSTS); tools/ab_tma.py is the A/B measurement.
+template <int F64, int TMA>
 __global__ void __launch_bounds__(128, ACC_MIN_BLOCKS)
-k_bucket_accumulate(const void *__restrict__ points, const uint32_t *__restrict__ sorted,
+k_bucket_accumulate(const ge_niels_packed *__restrict__ points, const uint32_t *__restrict__ sorted,
                     const uint32_t *__restrict__ counts, const uint32_t *__restrict__ offsets,
                     const uint32_t *__restrict__ ntasks, const uint2 *__restrict__ tasks, const uint32_t *__restrict__ order,
                     const uint32_t *__restrict__ win_base, int w0, int w1, size_t n, uint32_t nbuckets, uint32_t task_len,
                     ge_p3_raw *__restrict__ buckets, ge_p3_raw *__restrict__ task_sums, int first)
 {
-    constexpr int NQ = KIND == PK_NIELS ? 6 : 8;              // 16-byte pieces per point
+    constexpr int NQ = sizeof(ge_niels_packed) / 16;          // 16-byte pieces per point
     constexpr int TSTRIDE = NQ * 16 + 16;                     // bulk copies land contiguously: pad the per-thread slot so
                                                               // that the 16-byte reads of 8 consecutive threads hit 8 different bank groups
-    __shared__ uint4 s_pts[(F64 && !TMA) ? 2 : 1][(F64 && !TMA) ? 8 : 1][(F64 && !TMA) ? 128 : 1];   // cp.async slots, [buffer][piece][thread]: conflict-free
+    __shared__ uint4 s_pts[(F64 && !TMA) ? 2 : 1][(F64 && !TMA) ? NQ : 1][(F64 && !TMA) ? 128 : 1];   // cp.async slots, [buffer][piece][thread]: conflict-free
     __shared__ __align__(16) unsigned char s_bulk[(F64 && TMA) ? 2 : 1][(F64 && TMA) ? 128 : 1][(F64 && TMA) ? TSTRIDE : 16];
     __shared__ __align__(8) unsigned long long s_bar[(F64 && TMA) ? 2 : 1][(F64 && TMA) ? 128 : 1];
     const uint32_t total_tasks = win_base[w1];            // this launch covers the tasks of windows [w0, w1)
@@ -477,19 +609,11 @@ k_bucket_accumulate(const void *__restrict__ points, const uint32_t *__restrict_
 #pragma unroll
                 for (int q = 0; q < NQ; q++) { uint4 v = s_pts[buf][q][threadIdx.x]; words[4 * q] = v.x; words[4 * q + 1] = v.y; words[4 * q + 2] = v.z; words[4 * q + 3] = v.w; }
             }
-            if constexpr (KIND == PK_NIELS) {
-                ge_niels_packed pk;
+            ge_niels_packed pk;
 #pragma unroll
-                for (int q = 0; q < 24; q++) pk.w[q] = words[q];
-                ge64_niels nl; ge64_niels_unpack(nl, pk);
-                ge64_madd(acc64, acc64, nl, neg);
-            } else {
-                ge_pniels_packed pk;
-#pragma unroll
-                for (int q = 0; q < 32; q++) pk.w[q] = words[q];
-                ge64_pniels pn; ge64_pniels_unpack(pn, pk);
-                ge64_padd(acc64, acc64, pn, neg);
-            }
+            for (int q = 0; q < 24; q++) pk.w[q] = words[q];
+            ge64_niels nl; ge64_niels_unpack(nl, pk);
+            ge64_madd(acc64, acc64, nl, neg);
         }
         ge64_to_p3(acc, acc64);
     } else {
@@ -497,21 +621,12 @@ k_bucket_accumulate(const void *__restrict__ points, const uint32_t *__restrict_
     for (uint32_t k = 0; k < len; k++) {
         uint32_t e = idx[k];
         uint32_t neg = e >> 31, pi = e & 0x7fffffffu;
-        if (KIND == PK_NIELS) {
-            const uint4 *src = reinterpret_cast<const uint4 *>(reinterpret_cast<const ge_niels_packed *>(points) + pi);
-            ge_niels_packed pk;
+        const uint4 *src = reinterpret_cast<const uint4 *>(reinterpret_cast<const ge_niels_packed *>(points) + pi);
+        ge_niels_packed pk;
 #pragma unroll
-            for (int q = 0; q < 6; q++) { uint4 v = __ldg(src + q); pk.w[4 * q] = v.x; pk.w[4 * q + 1] = v.y; pk.w[4 * q + 2] = v.z; pk.w[4 * q + 3] = v.w; }
-            ge_niels nl; ge_niels_unpack(nl, pk);
-            ge_madd(acc, acc, nl, neg);
-        } else {
-            const uint4 *src = reinterpret_cast<const uint4 *>(reinterpret_cast<const ge_pniels_packed *>(points) + pi);
-            ge_pniels_packed pk;
-#pragma unroll
-            for (int q = 0; q < 8; q++) { uint4 v = __ldg(src + q); pk.w[4 * q] = v.x; pk.w[4 * q + 1] = v.y; pk.w[4 * q + 2] = v.z; pk.w[4 * q + 3] = v.w; }
-            ge_pniels pn; ge_pniels_unpack(pn, pk);
-            ge_padd(acc, acc, pn, neg);
-        }
+        for (int q = 0; q < 6; q++) { uint4 v = __ldg(src + q); pk.w[4 * q] = v.x; pk.w[4 * q + 1] = v.y; pk.w[4 * q + 2] = v.z; pk.w[4 * q + 3] = v.w; }
+        ge_niels nl; ge_niels_unpack(nl, pk);
+        ge_madd(acc, acc, nl, neg);
     }
     }
     ge_p3_raw r; ge_p3_store_raw(r, acc);
@@ -716,7 +831,7 @@ k_combine(const ge_p3_raw *__restrict__ windows, int ranks, int nwin, int c, Msm
 // `flat` (a table stride): d_points holds nwin tables of `flat` points, table w = 2^(cw) P_i (precomp.cu); every digit then goes into ONE
 // bucket window, so the reduction handles 2^(c-1) buckets instead of nwin times as many and no doubling is left
 // (pair with msm_reduce_finish(..., flat = true)).
-int msm_accumulate_chunk(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const void *d_points, int point_kind, size_t n,
+int msm_accumulate_chunk(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const ge_niels_packed *d_points, size_t n,
                          int c, bool first, int active_windows, size_t flat, cudaEvent_t points_ready)
 {
     const int nwin_d = msm_window_count_for_bits(c);               // digit windows
@@ -786,10 +901,9 @@ int msm_accumulate_chunk(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const v
     {
         const unsigned grid = cdiv(max_tasks, 128);
         const int f = first ? 1 : 0;
-#define LAUNCH_ACC(KIND_, F64_, TMA_) k_bucket_accumulate<KIND_, F64_, TMA_><<<grid, 128, 0, st>>>(d_points, sorted, counts, offsets, ntasks, tasks, order, win_base, 0, nwin, n, nb, task_len, buckets, task_sums, f)
+#define LAUNCH_ACC(F64_, TMA_) k_bucket_accumulate<F64_, TMA_><<<grid, 128, 0, st>>>(d_points, sorted, counts, offsets, ntasks, tasks, order, win_base, 0, nwin, n, nb, task_len, buckets, task_sums, f)
         const bool tma = ctx->opt_field_f64 && ctx->opt_acc_tma;
-        if (point_kind == PK_NIELS) { if (tma) LAUNCH_ACC(PK_NIELS, 1, 1); else if (ctx->opt_field_f64) LAUNCH_ACC(PK_NIELS, 1, 0); else LAUNCH_ACC(PK_NIELS, 0, 0); }
-        else { if (tma) LAUNCH_ACC(PK_PNIELS, 1, 1); else if (ctx->opt_field_f64) LAUNCH_ACC(PK_PNIELS, 1, 0); else LAUNCH_ACC(PK_PNIELS, 0, 0); }
+        if (tma) LAUNCH_ACC(1, 1); else if (ctx->opt_field_f64) LAUNCH_ACC(1, 0); else LAUNCH_ACC(0, 0);
 #undef LAUNCH_ACC
         k_heavy_fixup<<<ctx->sm_count * 4, 128, 0, st>>>(heavy, ntasks, task_off, win_base, nb, 0u, (uint32_t)nwin, task_sums, buckets, f);
         ctx->launches += 2;
@@ -896,19 +1010,19 @@ int msm_fill_identity(dalek_b200_ctx *ctx, ge_p3_raw *d_out, uint32_t count)
     return 0;
 }
 
-int msm_window_sums(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const void *d_points, int point_kind, size_t n,
+int msm_window_sums(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const ge_niels_packed *d_points, size_t n,
                     int c, ge_p3_raw *d_windows)
 {
     int rc;
-    if ((rc = msm_accumulate_chunk(ctx, d_scalars, d_points, point_kind, n, c, true))) return rc;
+    if ((rc = msm_accumulate_chunk(ctx, d_scalars, d_points, n, c, true))) return rc;
     return msm_reduce_finish(ctx, c, d_windows, nullptr);
 }
 
-int msm_full(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const void *d_points, int point_kind, size_t n, int c,
+int msm_full(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const ge_niels_packed *d_points, size_t n, int c,
              ge_p3_raw *d_windows, MsmResult *d_result)
 {
     int rc;
-    if ((rc = msm_accumulate_chunk(ctx, d_scalars, d_points, point_kind, n, c, true))) return rc;
+    if ((rc = msm_accumulate_chunk(ctx, d_scalars, d_points, n, c, true))) return rc;
     return msm_reduce_finish(ctx, c, d_windows, d_result);
 }
 

@@ -4,12 +4,11 @@
 //
 // The reference precomputes width-8 NAF tables of the static points so that repeated calls skip that work.
 // Here the precomputation is what the bucket MSM can reuse between calls, RESIDENT in HBM:
-//   * the static points decoded and converted to packed (projective) Niels form, and
+//   * the static points decoded and converted to packed affine Niels form (96 B each, what the bucket kernel reads), and
 //   * with the option "precomp_tables" and >= 4096 points, the tables 2^(c w) P_i for every window w of the width c
 //     chosen at construction, as affine Niels points (96 B each, 1.7 GB for 2^20 points at c = 16).  With them a
 //     digit of window w selects from table w and ALL windows share one set of 2^(c-1) buckets: the reduction shrinks
-//     by the window count, the final Horner (256 sequential doublings) disappears, and the additions are mixed (7M
-//     instead of 8M).  But the bucket kernel then gathers from 1.7 GB at random instead of from the 128 MB point
+//     by the window count and the final Horner (256 sequential doublings) disappears.  But the bucket kernel then gathers from 1.7 GB at random instead of from the 128 MB point
 //     array, and that costs it most of what the tail saves (tools/sweep_precomp.py times both).  Hence off by default.
 // A call moves only scalars (32 B per static point instead of 192 B).  Dynamic terms go through the ordinary
 // multi-window path and the two partial results are added.  The result is the same group element as the
@@ -24,42 +23,34 @@
 
 struct dalek_b200_precomp {
     dalek_b200_ctx *ctx;
-    void *d_points;        // n packed points, device
-    int kind;              // PK_NIELS / PK_PNIELS
+    ge_niels_packed *d_points;  // n packed affine Niels points, device
     int ristretto;         // 1: inputs/outputs are Ristretto encodings
     size_t n;
     ge_niels_packed *d_table;   // nwin slabs of n affine Niels points: slab w holds 2^(c w) P_i; null if not built
     int c, nwin;
 };
 
-// P_i from the packed form (Y+X, Y-X, Z, 2dT): X = ((Y+X) - (Y-X)) / 2, Y = ((Y+X) + (Y-X)) / 2, T = X Y / Z
-__device__ __forceinline__ void point_from_packed(ge_p3 &p, const void *packed, int kind, size_t i)
+// P_i from the packed affine Niels form (y+x, y-x, 2dxy): x = ((y+x) - (y-x)) / 2, y = ((y+x) + (y-x)) / 2
+__device__ __forceinline__ void point_from_packed(ge_p3 &p, const ge_niels_packed *packed, size_t i)
 {
     fe ypx, ymx, half, t;
-    if (kind == PK_NIELS) {
-        ge_niels_packed q = reinterpret_cast<const ge_niels_packed *>(packed)[i];
-        fe_frombytes_words(ypx, q.w); fe_frombytes_words(ymx, q.w + 8);
-        fe_1(p.Z);
-    } else {
-        ge_pniels_packed q = reinterpret_cast<const ge_pniels_packed *>(packed)[i];
-        fe_frombytes_words(ypx, q.w); fe_frombytes_words(ymx, q.w + 8); fe_frombytes_words(p.Z, q.w + 16);
-    }
+    ge_niels_packed q = packed[i];
+    fe_frombytes_words(ypx, q.w); fe_frombytes_words(ymx, q.w + 8);
     const uint32_t half_words[8] = {0xfffffff7u, 0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu, 0x3fffffffu};
     fe_frombytes_words(half, half_words);                 // (p + 1) / 2 = 2^254 - 9
     fe_sub(t, ypx, ymx); fe_mul(p.X, t, half);
     fe_add(t, ypx, ymx); fe_mul(p.Y, t, half);
-    // extended coordinates with this Z: (X Z : Y Z : Z^2 : X Y) is the same point with T consistent
-    fe x = p.X, y = p.Y, z = p.Z;
-    fe_mul(p.X, x, z); fe_mul(p.Y, y, z); fe_mul(p.T, x, y); fe_sq(p.Z, z);
+    fe_1(p.Z);
+    fe_mul(p.T, p.X, p.Y);
 }
 
 __global__ void __launch_bounds__(128, 2)
-k_precomp_table(const void *__restrict__ packed, int kind, size_t n, int c, int nwin, ge_niels_packed *__restrict__ table)
+k_precomp_table(const ge_niels_packed *__restrict__ packed, size_t n, int c, int nwin, ge_niels_packed *__restrict__ table)
 {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     ge_p3 P;
-    point_from_packed(P, packed, kind, i);
+    point_from_packed(P, packed, i);
     ge64_p3 Q; ge64_from_p3(Q, P);
 #pragma unroll 1
     for (int w = 0; w < nwin; w++) {
@@ -94,11 +85,9 @@ __global__ void k_add_results(const MsmResult *__restrict__ a, const MsmResult *
 }
 
 static size_t in_bytes(int fmt) { return fmt == DALEK_POINTS_EXTENDED ? 160 : 32; }
-static int kind_of(int fmt) { return fmt == DALEK_POINTS_COMPRESSED ? PK_NIELS : PK_PNIELS; }
-static size_t packed_bytes(int kind) { return kind == PK_NIELS ? sizeof(ge_niels_packed) : sizeof(ge_pniels_packed); }
 
-// device input in format `fmt` -> packed points at d_out
-static int prepare(dalek_b200_ctx *ctx, const void *d_in, int fmt, size_t n, void *d_out, int *d_bad)
+// device input in format `fmt` -> packed affine Niels points at d_out
+static int prepare(dalek_b200_ctx *ctx, const void *d_in, int fmt, size_t n, ge_niels_packed *d_out, int *d_bad)
 {
     if (fmt == DALEK_POINTS_RISTRETTO) return ristretto_prepare_points(ctx, d_in, n, d_out, d_bad);
     return msm_prepare_points(ctx, d_in, fmt, n, d_out, d_bad);
@@ -116,9 +105,9 @@ int dalek_b200_precomp_new(dalek_b200_ctx *ctx, const void *static_points, int p
     cudaStream_t st = ctx->stream;
     dalek_b200_precomp *pre = new (std::nothrow) dalek_b200_precomp();
     if (!pre) return DALEK_E_NOMEM;
-    pre->ctx = ctx; pre->n = n; pre->kind = kind_of(point_fmt); pre->ristretto = point_fmt == DALEK_POINTS_RISTRETTO;
+    pre->ctx = ctx; pre->n = n; pre->ristretto = point_fmt == DALEK_POINTS_RISTRETTO;
     pre->d_points = nullptr;
-    if (cudaMalloc(&pre->d_points, std::max<size_t>(1, n) * packed_bytes(pre->kind)) != cudaSuccess) {
+    if (cudaMalloc((void **)&pre->d_points, std::max<size_t>(1, n) * sizeof(ge_niels_packed)) != cudaSuccess) {
         ctx->last_error = "cudaMalloc failed for the static point table";
         delete pre;
         return DALEK_E_NOMEM;
@@ -144,7 +133,7 @@ int dalek_b200_precomp_new(dalek_b200_ctx *ctx, const void *static_points, int p
         size_t free_b = 0, total_b = 0;
         if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && bytes < free_b / 2 && (size_t)pre->nwin * n < (1ull << 31) &&
             cudaMalloc((void **)&pre->d_table, bytes) == cudaSuccess) {
-            k_precomp_table<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(pre->d_points, pre->kind, n, pre->c, pre->nwin, pre->d_table);
+            k_precomp_table<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(pre->d_points, n, pre->c, pre->nwin, pre->d_table);
             ctx->launches++;
             if (cudaStreamSynchronize(st) != cudaSuccess) { cudaFree(pre->d_table); return fail(DALEK_E_CUDA); }
         } else {
@@ -184,7 +173,6 @@ int dalek_b200_precomp_mixed_msm(dalek_b200_ctx *ctx, const dalek_b200_precomp *
     CallTimer timer(ctx);
     int rc;
     cudaStream_t st = ctx->stream;
-    const int dkind = kind_of(dynamic_fmt);
     const size_t din = in_bytes(dynamic_fmt);
     const bool use_table = pre->d_table != nullptr && n_static > 0;
     // window widths: the table fixes the static width; the dynamic part picks its own
@@ -193,7 +181,8 @@ int dalek_b200_precomp_mixed_msm(dalek_b200_ctx *ctx, const dalek_b200_precomp *
     const int nwin = std::max(msm_window_count_for_bits(c), msm_window_count_for_bits(c_dyn));
     if ((rc = ws_reserve(ctx, ctx->scalars, std::max<size_t>(1, n_static + n_dynamic) * 32))) return rc;
     if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n_dynamic) * din))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points, std::max<size_t>(1, n_dynamic) * packed_bytes(dkind)))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->points, std::max<size_t>(1, n_dynamic) * sizeof(ge_niels_packed)))) return rc;
+    ge_niels_packed *d_dpts = (ge_niels_packed *)ctx->points.p;
     if ((rc = ws_reserve(ctx, ctx->flags, 64))) return rc;
     if ((rc = ws_reserve(ctx, ctx->misc0, (size_t)nwin * sizeof(ge_p3_raw)))) return rc;
     if ((rc = ws_reserve(ctx, ctx->result, 3 * sizeof(MsmResult) + 64))) return rc;
@@ -220,26 +209,25 @@ int dalek_b200_precomp_mixed_msm(dalek_b200_ctx *ctx, const dalek_b200_precomp *
         CUDA_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_grp[k], 0));
         if (use_table) {
             // one bucket window: the digit of window w of scalar i selects table[w * n + i]
-            if ((rc = msm_accumulate_chunk(ctx, d_ss + 8 * i0, pre->d_table + i0, PK_NIELS, i1 - i0, c, k == 0, 0, pre->n))) return rc;
+            if ((rc = msm_accumulate_chunk(ctx, d_ss + 8 * i0, pre->d_table + i0, i1 - i0, c, k == 0, 0, pre->n))) return rc;
         } else {
-            const char *pts = (const char *)pre->d_points + i0 * packed_bytes(pre->kind);
-            if ((rc = msm_accumulate_chunk(ctx, d_ss + 8 * i0, pts, pre->kind, i1 - i0, c, k == 0))) return rc;
+            if ((rc = msm_accumulate_chunk(ctx, d_ss + 8 * i0, pre->d_points + i0, i1 - i0, c, k == 0))) return rc;
         }
     }
     CUDA_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_grp[K], 0));
     if (use_table) {
         if ((rc = msm_reduce_finish(ctx, c, (ge_p3_raw *)ctx->misc0.p, n_dynamic ? d_r1 : d_res, true))) return rc;
         if (n_dynamic) {
-            if ((rc = prepare(ctx, ctx->points_in.p, dynamic_fmt, n_dynamic, ctx->points.p, (int *)ctx->flags.p))) return rc;
-            if ((rc = msm_accumulate_chunk(ctx, d_ds, ctx->points.p, dkind, n_dynamic, c_dyn, true))) return rc;
+            if ((rc = prepare(ctx, ctx->points_in.p, dynamic_fmt, n_dynamic, d_dpts, (int *)ctx->flags.p))) return rc;
+            if ((rc = msm_accumulate_chunk(ctx, d_ds, d_dpts, n_dynamic, c_dyn, true))) return rc;
             if ((rc = msm_reduce_finish(ctx, c_dyn, (ge_p3_raw *)ctx->misc0.p, d_r2))) return rc;
             k_add_results<<<1, 1, 0, st>>>(d_r1, d_r2, d_res);
             ctx->launches++;
         }
     } else {
         if (n_dynamic) {
-            if ((rc = prepare(ctx, ctx->points_in.p, dynamic_fmt, n_dynamic, ctx->points.p, (int *)ctx->flags.p))) return rc;
-            if ((rc = msm_accumulate_chunk(ctx, d_ds, ctx->points.p, dkind, n_dynamic, c, false))) return rc;
+            if ((rc = prepare(ctx, ctx->points_in.p, dynamic_fmt, n_dynamic, d_dpts, (int *)ctx->flags.p))) return rc;
+            if ((rc = msm_accumulate_chunk(ctx, d_ds, d_dpts, n_dynamic, c, false))) return rc;
         }
         if ((rc = msm_reduce_finish(ctx, c, (ge_p3_raw *)ctx->misc0.p, d_res))) return rc;
     }

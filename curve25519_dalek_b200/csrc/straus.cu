@@ -385,8 +385,9 @@ int ristretto_double_base(dalek_b200_ctx *ctx, const uint8_t *d_a, const uint8_t
 // ------------------------------------------------------------------------------------------
 // Ristretto vartime MSM: decode with the Ristretto rules, then the Edwards bucket MSM; encode the
 // result with RistrettoPoint::compress (ristretto.rs:980-994).
+// The decoded point is affine (Z = 1), so it goes straight to the affine Niels form of the bucket kernel.
 template <int F64>
-__global__ void k_prep_ristretto(const uint32_t *__restrict__ in, ge_pniels_packed *__restrict__ out, size_t n, int *__restrict__ bad)
+__global__ void k_prep_ristretto(const uint32_t *__restrict__ in, ge_niels_packed *__restrict__ out, size_t n, int *__restrict__ bad)
 {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -395,8 +396,8 @@ __global__ void k_prep_ristretto(const uint32_t *__restrict__ in, ge_pniels_pack
     for (int k = 0; k < 8; k++) enc[k] = in[8 * i + k];
     ge_p3 P;
     if (!ristretto_decompress<F64>(P, enc)) { atomicOr(bad, 1); ge_p3_identity(P); }
-    ge_pniels pn; ge_p3_to_pniels(pn, P);
-    ge_pniels_packed pk; ge_pniels_pack(pk, pn);
+    ge_niels nl; ge_affine_to_niels(nl, P.X, P.Y);
+    ge_niels_packed pk; ge_niels_pack(pk, nl);
     out[i] = pk;
 }
 
@@ -410,12 +411,12 @@ __global__ void k_ristretto_encode_result(const MsmResult *__restrict__ res, uin
     for (int k = 0; k < 8; k++) out[k] = enc[k];
 }
 
-// CompressedRistretto (device, n x 32 B) -> packed projective Niels; *d_bad set if one does not decode
+// CompressedRistretto (device, n x 32 B) -> packed affine Niels; *d_bad set if one does not decode
 int ristretto_prepare_points(dalek_b200_ctx *ctx, const void *d_in, size_t n, void *d_out, int *d_bad)
 {
     if (!n) return 0;
-    if (ctx->opt_decompress_f64) k_prep_ristretto<1><<<cdiv(n, 128), 128, 0, ctx->stream>>>((const uint32_t *)d_in, (ge_pniels_packed *)d_out, n, d_bad);
-    else k_prep_ristretto<0><<<cdiv(n, 128), 128, 0, ctx->stream>>>((const uint32_t *)d_in, (ge_pniels_packed *)d_out, n, d_bad);
+    if (ctx->opt_decompress_f64) k_prep_ristretto<1><<<cdiv(n, 128), 128, 0, ctx->stream>>>((const uint32_t *)d_in, (ge_niels_packed *)d_out, n, d_bad);
+    else k_prep_ristretto<0><<<cdiv(n, 128), 128, 0, ctx->stream>>>((const uint32_t *)d_in, (ge_niels_packed *)d_out, n, d_bad);
     ctx->launches++;
     CUDA_TRY(ctx, cudaGetLastError());
     return 0;
@@ -460,7 +461,7 @@ int dalek_b200_edwards_ct_msm(dalek_b200_ctx *ctx, const uint8_t *scalars, const
         if ((rc = msm_prepare_points(ctx, ctx->points_in.p, point_fmt, n, ctx->misc1.p, (int *)ctx->flags.p))) return rc;
         launch_niels_to_pniels(ctx, ctx->misc1.p, ctx->points.p, n);
     } else {
-        if ((rc = msm_prepare_points(ctx, ctx->points_in.p, point_fmt, n, ctx->points.p, (int *)ctx->flags.p))) return rc;
+        if ((rc = msm_prepare_points(ctx, ctx->points_in.p, point_fmt, n, ctx->points.p, (int *)ctx->flags.p, PK_PNIELS))) return rc;
     }
     if ((rc = straus_ct_msm(ctx, (const uint32_t *)ctx->scalars.p, d_pn, n, (MsmResult *)ctx->result.p))) return rc;
     if ((rc = pinned_reserve(ctx, sizeof(MsmResult) + 64))) return rc;
@@ -531,21 +532,21 @@ int dalek_b200_ristretto_vartime_msm(dalek_b200_ctx *ctx, const uint8_t *scalars
     cudaStream_t st = ctx->stream;
     if ((rc = ws_reserve(ctx, ctx->scalars, std::max<size_t>(1, n) * 32))) return rc;
     if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * 32))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points, std::max<size_t>(1, n) * sizeof(ge_pniels_packed)))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->points, std::max<size_t>(1, n) * sizeof(ge_niels_packed)))) return rc;
     if ((rc = ws_reserve(ctx, ctx->flags, 64))) return rc;
     if ((rc = ws_reserve(ctx, ctx->result, sizeof(MsmResult) + 64))) return rc;
     CUDA_TRY(ctx, cudaMemsetAsync(ctx->flags.p, 0, 64, st));
     if (n) {
         CUDA_TRY(ctx, cudaMemcpyAsync(ctx->scalars.p, scalars, n * 32, cudaMemcpyHostToDevice, st));
         CUDA_TRY(ctx, cudaMemcpyAsync(ctx->points_in.p, points, n * 32, cudaMemcpyHostToDevice, st));
-        if (ctx->opt_decompress_f64) k_prep_ristretto<1><<<cdiv(n, 128), 128, 0, st>>>((const uint32_t *)ctx->points_in.p, (ge_pniels_packed *)ctx->points.p, n, (int *)ctx->flags.p);
-        else k_prep_ristretto<0><<<cdiv(n, 128), 128, 0, st>>>((const uint32_t *)ctx->points_in.p, (ge_pniels_packed *)ctx->points.p, n, (int *)ctx->flags.p);
+        if (ctx->opt_decompress_f64) k_prep_ristretto<1><<<cdiv(n, 128), 128, 0, st>>>((const uint32_t *)ctx->points_in.p, (ge_niels_packed *)ctx->points.p, n, (int *)ctx->flags.p);
+        else k_prep_ristretto<0><<<cdiv(n, 128), 128, 0, st>>>((const uint32_t *)ctx->points_in.p, (ge_niels_packed *)ctx->points.p, n, (int *)ctx->flags.p);
         ctx->launches++;
     }
     int c = msm_choose_window_bits(ctx, n);
     int nwin = msm_window_count_for_bits(c);
     if ((rc = ws_reserve(ctx, ctx->misc0, (size_t)nwin * sizeof(ge_p3_raw)))) return rc;
-    if ((rc = msm_full(ctx, (const uint32_t *)ctx->scalars.p, ctx->points.p, PK_PNIELS, n, c, (ge_p3_raw *)ctx->misc0.p, (MsmResult *)ctx->result.p))) return rc;
+    if ((rc = msm_full(ctx, (const uint32_t *)ctx->scalars.p, (const ge_niels_packed *)ctx->points.p, n, c, (ge_p3_raw *)ctx->misc0.p, (MsmResult *)ctx->result.p))) return rc;
     uint32_t *d_enc = (uint32_t *)((char *)ctx->result.p + sizeof(MsmResult));
     k_ristretto_encode_result<<<1, 1, 0, st>>>((const MsmResult *)ctx->result.p, d_enc);
     ctx->launches++;
