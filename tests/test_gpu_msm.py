@@ -258,7 +258,7 @@ def test_msm_host_chunked_streaming(eng, oracle, fmt):
         try:
             rc, got, _ = eng.edwards_vartime_msm(sb, pb, n, point_fmt=fmt)
         finally:
-            eng.set_option("host_chunks", 2)
+            eng.set_option("host_chunks", 8)                # the engine's default
         assert rc == 0 and got == want, chunks
 
 
