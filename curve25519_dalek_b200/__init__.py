@@ -8,11 +8,15 @@ touches the CPU checker used by the tests.  Names follow the reference:
   RistrettoPoint.multiscalar_mul / vartime_multiscalar_mul (src/ristretto.rs:964-994)
   VartimeEdwardsPrecomputation / VartimeRistrettoPrecomputation (traits.rs:290-406, edwards.rs:1038-1076)
   verify_batch (ed25519-dalek/src/batch.rs:146-251) and its SignatureError values.
+  x25519 / x25519_public_keys / X25519_BASEPOINT_BYTES (x25519-dalek/src/x25519.rs:105-110, :385-392)
+  EdwardsPoint.to_montgomery_batch (src/edwards.rs:592-612)
 """
 from .engine import (Engine, MultiEngine, EngineError, EdwardsPoint, RistrettoPoint, SignatureError, verify_batch, default_engine,
                      library_path, load_library, POINTS_COMPRESSED, POINTS_EXTENDED, POINTS_RISTRETTO,
-                     VartimeEdwardsPrecomputation, VartimeRistrettoPrecomputation)
+                     VartimeEdwardsPrecomputation, VartimeRistrettoPrecomputation, x25519, x25519_public_keys,
+                     X25519_BASEPOINT_BYTES)
 
 __all__ = ["Engine", "MultiEngine", "EngineError", "EdwardsPoint", "RistrettoPoint", "SignatureError", "verify_batch", "default_engine",
            "library_path", "load_library", "POINTS_COMPRESSED", "POINTS_EXTENDED", "POINTS_RISTRETTO",
-           "VartimeEdwardsPrecomputation", "VartimeRistrettoPrecomputation"]
+           "VartimeEdwardsPrecomputation", "VartimeRistrettoPrecomputation", "x25519", "x25519_public_keys",
+           "X25519_BASEPOINT_BYTES"]

@@ -3,7 +3,8 @@
 //   EdwardsPoint::compress_batch              C/edwards.rs:619-647        k_compress_batch
 //   CompressedRistretto::decompress           C/ristretto.rs:266-345      k_ristretto_decompress_batch
 //   RistrettoPoint::double_and_compress_batch C/ristretto.rs:564-646      k_ristretto_double_and_compress_batch
-// The two compressors use Montgomery's simultaneous inversion exactly like the reference
+//   EdwardsPoint::to_montgomery_batch         C/edwards.rs:592-612        k_to_montgomery_batch
+// The two compressors and the Montgomery map use Montgomery's simultaneous inversion exactly like the reference
 // (FieldElement::invert_batch, C/field.rs:239-274, zeros skipped): a thread owns CODEC_K consecutive points, so one
 // 254-squaring inversion (on the FP64 field) is shared by CODEC_K points.
 // Points travel as the reference's in-memory EdwardsPoint: 20 u64 limbs X | Y | Z | T in radix 2^51.
@@ -12,6 +13,7 @@
 
 #include "../../include/dalek_b200.h"
 #include "engine.h"
+#include "pieces.h"
 
 static inline unsigned cdiv(size_t a, unsigned b) { return (unsigned)((a + b - 1) / b); }
 
@@ -112,6 +114,37 @@ k_compress_batch(const uint64_t *__restrict__ in, size_t n, uint32_t *__restrict
     }
 }
 
+// Montgomery u = (Z + Y) / (Z - Y) (C/edwards.rs:592-612), one shared inversion per CODEC_K points; the identity
+// (Z = Y) has a zero denominator, skipped by invert_batch, and gives u = 0 like the reference's to_montgomery
+__global__ void __launch_bounds__(128)
+k_to_montgomery_batch(const uint64_t *__restrict__ in, size_t n, uint32_t *__restrict__ out)
+{
+    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x, i0 = t * CODEC_K;
+    if (i0 >= n) return;
+    fe den[CODEC_K];
+#pragma unroll
+    for (int k = 0; k < CODEC_K; k++) {
+        if (i0 + k < n) {
+            fe Y, Z, d;
+            load_limbs(Y, in + 20 * (i0 + k) + 5); load_limbs(Z, in + 20 * (i0 + k) + 10);
+            fe_sub(d, Z, Y); fe_carry(den[k], d);
+        } else fe_1(den[k]);
+    }
+    invert_batch(den);
+#pragma unroll 1
+    for (int k = 0; k < CODEC_K; k++) {
+        if (i0 + k >= n) break;
+        fe Y, Z, s, u;
+        load_limbs(Y, in + 20 * (i0 + k) + 5); load_limbs(Z, in + 20 * (i0 + k) + 10);
+        fe_add(s, Z, Y);
+        fe_mul(u, s, den[k]);
+        uint32_t w[8];
+        fe_tobytes_words(w, u);
+#pragma unroll
+        for (int q = 0; q < 8; q++) out[8 * (i0 + k) + q] = w[q];
+    }
+}
+
 // the per-point state of C/ristretto.rs:584-601
 struct dbl_state { fe e, f, g, h, eg, fh; };
 __device__ __forceinline__ void dbl_state_from(dbl_state &s, const uint64_t *__restrict__ pt)
@@ -174,42 +207,6 @@ k_ristretto_double_and_compress_batch(const uint64_t *__restrict__ in, size_t n,
     }
 }
 
-// ------------------------------------------------------------------------------------------
-// host buffers in and out, streamed in pieces over two streams (copy-in -> kernel -> copy-out)
-template <typename Launch>
-static int run_pieces(dalek_b200_ctx *ctx, const uint8_t *in, size_t in_sz, uint8_t *out, size_t out_sz, uint8_t *out2, size_t out2_sz,
-                      size_t n, Launch launch)
-{
-    int rc;
-    if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * in_sz))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points, std::max<size_t>(1, n) * (out_sz + out2_sz)))) return rc;
-    uint8_t *d_in = (uint8_t *)ctx->points_in.p, *d_out = (uint8_t *)ctx->points.p, *d_out2 = d_out + n * out_sz;
-    cudaStream_t ss[2] = {ctx->stream, ctx->stream2};
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, ctx->stream));
-    CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->ev_fork, 0));
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, ctx->stream));
-    const size_t piece = n >= (1u << 17) ? (size_t)1 << 16 : std::max<size_t>(1, n);   // a multiple of 128 * CODEC_K
-    size_t k = 0;
-    for (size_t lo = 0; lo < n; lo += piece, k++) {
-        const size_t m = std::min(piece, n - lo);
-        cudaStream_t st = ss[k & 1];
-        CUDA_TRY(ctx, cudaMemcpyAsync(d_in + lo * in_sz, in + lo * in_sz, m * in_sz, cudaMemcpyHostToDevice, st));
-        launch(d_in + lo * in_sz, m, d_out + lo * out_sz, d_out2 + lo * out2_sz, st);
-        ctx->launches++;
-        CUDA_TRY(ctx, cudaGetLastError());
-        CUDA_TRY(ctx, cudaMemcpyAsync(out + lo * out_sz, d_out + lo * out_sz, m * out_sz, cudaMemcpyDeviceToHost, st));
-        if (out2_sz) CUDA_TRY(ctx, cudaMemcpyAsync(out2 + lo * out2_sz, d_out2 + lo * out2_sz, m * out2_sz, cudaMemcpyDeviceToHost, st));
-    }
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_join, ctx->stream2));
-    CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, ctx->stream));
-    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    float ms = 0.f;
-    if ((ms = elapsed_ms(ctx->ev_a, ctx->ev_b)) >= 0.f) ctx->last_kernel_ms = ms;
-    ctx->last_kernel_launches = (int)k;
-    return 0;
-}
-
 extern "C" {
 
 int dalek_b200_edwards_decompress_batch(dalek_b200_ctx *ctx, const uint8_t *in, size_t n, uint64_t *out_limbs, uint8_t *ok)
@@ -217,7 +214,7 @@ int dalek_b200_edwards_decompress_batch(dalek_b200_ctx *ctx, const uint8_t *in, 
     if (!ctx || (n && (!in || !out_limbs || !ok))) return DALEK_E_INVALID_ARG;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     const bool f64 = ctx->opt_decompress_f64 != 0;
-    int rc = run_pieces(ctx, in, 32, (uint8_t *)out_limbs, 160, ok, 1, n, [&](const uint8_t *di, size_t m, uint8_t *d_o, uint8_t *d_ok, cudaStream_t st) {
+    int rc = run_pieces(ctx, in, 32, nullptr, 0, (uint8_t *)out_limbs, 160, ok, 1, n, [&](const uint8_t *di, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *d_ok, cudaStream_t st) {
         if (f64) k_decompress_batch<1><<<cdiv(m, 128), 128, 0, st>>>((const uint32_t *)di, m, (uint64_t *)d_o, d_ok);
         else k_decompress_batch<0><<<cdiv(m, 128), 128, 0, st>>>((const uint32_t *)di, m, (uint64_t *)d_o, d_ok);
     });
@@ -232,7 +229,7 @@ int dalek_b200_ristretto_decompress_batch(dalek_b200_ctx *ctx, const uint8_t *in
     if (!ctx || (n && (!in || !out_limbs || !ok))) return DALEK_E_INVALID_ARG;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     const bool f64 = ctx->opt_decompress_f64 != 0;
-    int rc = run_pieces(ctx, in, 32, (uint8_t *)out_limbs, 160, ok, 1, n, [&](const uint8_t *di, size_t m, uint8_t *d_o, uint8_t *d_ok, cudaStream_t st) {
+    int rc = run_pieces(ctx, in, 32, nullptr, 0, (uint8_t *)out_limbs, 160, ok, 1, n, [&](const uint8_t *di, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *d_ok, cudaStream_t st) {
         if (f64) k_ristretto_decompress_batch<1><<<cdiv(m, 128), 128, 0, st>>>((const uint32_t *)di, m, (uint64_t *)d_o, d_ok);
         else k_ristretto_decompress_batch<0><<<cdiv(m, 128), 128, 0, st>>>((const uint32_t *)di, m, (uint64_t *)d_o, d_ok);
     });
@@ -246,7 +243,7 @@ int dalek_b200_edwards_compress_batch(dalek_b200_ctx *ctx, const uint64_t *limbs
 {
     if (!ctx || (n && (!limbs || !out))) return DALEK_E_INVALID_ARG;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    return run_pieces(ctx, (const uint8_t *)limbs, 160, out, 32, nullptr, 0, n, [&](const uint8_t *di, size_t m, uint8_t *d_o, uint8_t *, cudaStream_t st) {
+    return run_pieces(ctx, (const uint8_t *)limbs, 160, nullptr, 0, out, 32, nullptr, 0, n, [&](const uint8_t *di, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *, cudaStream_t st) {
         k_compress_batch<<<cdiv(cdiv(m, CODEC_K), 128), 128, 0, st>>>((const uint64_t *)di, m, (uint32_t *)d_o);
     });
 }
@@ -255,8 +252,19 @@ int dalek_b200_ristretto_double_and_compress_batch(dalek_b200_ctx *ctx, const ui
 {
     if (!ctx || (n && (!limbs || !out))) return DALEK_E_INVALID_ARG;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    return run_pieces(ctx, (const uint8_t *)limbs, 160, out, 32, nullptr, 0, n, [&](const uint8_t *di, size_t m, uint8_t *d_o, uint8_t *, cudaStream_t st) {
+    return run_pieces(ctx, (const uint8_t *)limbs, 160, nullptr, 0, out, 32, nullptr, 0, n, [&](const uint8_t *di, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *, cudaStream_t st) {
         k_ristretto_double_and_compress_batch<<<cdiv(cdiv(m, CODEC_K), 128), 128, 0, st>>>((const uint64_t *)di, m, (uint32_t *)d_o);
+    });
+}
+
+int dalek_b200_edwards_to_montgomery_batch(dalek_b200_ctx *ctx, const uint64_t *limbs, size_t n, uint8_t *out)
+{
+    if (!ctx || (n && (!limbs || !out))) return DALEK_E_INVALID_ARG;
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    if (!n) return DALEK_OK;
+    CallTimer timer(ctx);
+    return run_pieces(ctx, (const uint8_t *)limbs, 160, nullptr, 0, out, 32, nullptr, 0, n, [&](const uint8_t *di, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *, cudaStream_t st) {
+        k_to_montgomery_batch<<<cdiv(cdiv(m, CODEC_K), 128), 128, 0, st>>>((const uint64_t *)di, m, (uint32_t *)d_o);
     });
 }
 

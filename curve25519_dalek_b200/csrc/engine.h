@@ -64,6 +64,8 @@ struct dalek_b200_ctx {
     bool base_table_ready = false;
     bool each_attr_set = false;     // the same for k_verify_each_comb
     bool comb_attr_set = false;     // cudaFuncAttributeMaxDynamicSharedMemorySize set for the comb kernel on this device
+    DevBuf x25519_table;            // comb table of the Ed25519 basepoint for X25519 public keys (x25519.cu), built once
+    bool x25519_table_ready = false;
     // pinned host staging
     void *h_pinned = nullptr;
     size_t h_pinned_cap = 0;

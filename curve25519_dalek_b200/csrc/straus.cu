@@ -14,6 +14,7 @@
 #include <cstring>
 
 #include "../../include/dalek_b200.h"
+#include "comb.cuh"
 #include "engine.h"
 #include "ge64.cuh"
 
@@ -222,9 +223,8 @@ k_double_base(const uint32_t *__restrict__ a, const uint32_t *__restrict__ b, co
 // doublings + 128 additions for Straus.  The contract of MultiscalarMul is kept: the 2 x 64 x 8 table
 // entries (j+1) 16^i {G,H} sit in shared memory as balanced FP64 limbs (15 doubles each, 120 KiB), every
 // lookup scans all 8 entries of a row at warp-uniform addresses with arithmetic masks (window.rs:54-76),
-// and the digit's sign is applied by masked swap / negate inside the addition.
+// and the digit's sign is applied by masked swap / negate inside the addition (comb.cuh).
 #define COMB_ROWS 128          // 2 bases x 64 digit positions
-#define COMB_ENTRY 15          // doubles per affine Niels entry
 
 __global__ void __launch_bounds__(128)
 k_comb_tables(const uint32_t *__restrict__ GH, double *__restrict__ table, int *__restrict__ status)
@@ -235,43 +235,9 @@ k_comb_tables(const uint32_t *__restrict__ GH, double *__restrict__ table, int *
     uint32_t enc[8];
 #pragma unroll
     for (int k = 0; k < 8; k++) enc[k] = GH[8 * b + k];
-    ge_p3 base, P;
+    ge_p3 base;
     if (!ristretto_decompress(base, enc)) { atomicOr(status, 1); ge_p3_identity(base); }
-    ge_pniels nb; ge_p3_to_pniels(nb, base);
-    P = base;
-    for (int k = 0; k < j; k++) ge_padd(P, P, nb, 0);            // (j+1) * base
-    if (i) ge_mul_by_pow_2(P, P, 4 * i);                         // * 16^i
-    fe zi, x, y;
-    fe_invert(zi, P.Z);
-    fe_mul(x, P.X, zi); fe_mul(y, P.Y, zi);
-    ge_niels n; ge_affine_to_niels(n, x, y);
-    fe64 e[3];
-    fe64_from_fe(e[0], n.ypx); fe64_from_fe(e[1], n.ymx); fe64_from_fe(e[2], n.xy2d);
-    double *dst = table + (size_t)t * COMB_ENTRY;
-#pragma unroll
-    for (int c = 0; c < 3; c++)
-#pragma unroll
-        for (int k = 0; k < 5; k++) dst[5 * c + k] = e[c].v[k];
-}
-
-// constant-time: select |digit| * 16^i * base from the 8 entries of one table row (digit 0 -> identity)
-__device__ __forceinline__ void comb_select(ge64_niels &q, const double *__restrict__ row, uint32_t xabs)
-{
-    long long w[COMB_ENTRY];
-#pragma unroll
-    for (int k = 0; k < COMB_ENTRY; k++) w[k] = 0;
-#pragma unroll 1
-    for (uint32_t j = 1; j <= 8; j++) {
-        const long long m = 0LL - (long long)(xabs == j);
-#pragma unroll
-        for (int k = 0; k < COMB_ENTRY; k++) w[k] |= __double_as_longlong(row[(j - 1) * COMB_ENTRY + k]) & m;
-    }
-    const long long one = 0x3ff0000000000000LL & (0LL - (long long)(xabs == 0));      // 1.0 for the identity (1, 1, 0)
-    w[0] |= one; w[5] |= one;
-#pragma unroll
-    for (int k = 0; k < 5; k++) {
-        q.ypx.v[k] = __longlong_as_double(w[k]); q.ymx.v[k] = __longlong_as_double(w[5 + k]); q.xy2d.v[k] = __longlong_as_double(w[10 + k]);
-    }
+    comb_entry(table + (size_t)t * COMB_ENTRY, base, i, j);
 }
 
 template <int THREADS>

@@ -1,0 +1,173 @@
+// x25519.cu -- X25519 key agreement and public-key derivation in bulk (x25519-dalek, RFC 7748).
+//   x25519(k, u)             x25519.rs:390-392 -> C/montgomery.rs:150-211   k_x25519       one thread per pair, the ladder
+//                                                                                         of x25519.cuh on the FP64 field
+//   PublicKey::from(&secret) x25519.rs:105-110 -> C/montgomery.rs:164-174   k_x25519_base  mul_base_clamped(k).to_montgomery()
+//                            -> C/edwards.rs:580-590                                       as a constant-time fixed-base comb
+// Both are constant time in k and u: no branch, loop bound or address depends on them (x25519.cuh; comb.cuh scans
+// every entry of a table row).  The comb table of the Ed25519 basepoint B (64 x 8 entries (j+1) 16^i B, 60 KiB) is
+// built once per context.  Unlike base.cu's mul_base, which indexes its table by the digit, the comb never reads a
+// secret-dependent address.
+// The device workspaces that held scalars or shared secrets are cleared before a host-buffer call returns, as the
+// reference zeroizes its secrets on drop (x25519.rs:112-117).
+#include <algorithm>
+#include <cstring>
+
+#include "../../include/dalek_b200.h"
+#include "comb.cuh"
+#include "engine.h"
+#include "pieces.h"
+#include "x25519.cuh"
+
+static inline unsigned cdiv(size_t a, unsigned b) { return (unsigned)((a + b - 1) / b); }
+
+#define X25519_THREADS 128
+#define X25519_COMB_THREADS 384
+#define X25519_COMB_DOUBLES (64 * 8 * COMB_ENTRY)
+
+__global__ void __launch_bounds__(X25519_THREADS)
+k_x25519(const uint32_t *__restrict__ scalars, const uint32_t *__restrict__ us, size_t n, uint32_t *__restrict__ out,
+         uint8_t *__restrict__ contributory)
+{
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t k[8], u[8], r[8];
+#pragma unroll
+    for (int j = 0; j < 8; j++) { k[j] = scalars[8 * i + j]; u[j] = us[8 * i + j]; }
+    x25519_ladder(r, k, u);
+#pragma unroll
+    for (int j = 0; j < 8; j++) out[8 * i + j] = r[j];
+    if (contributory) contributory[i] = (uint8_t)x25519_contributory(r);
+}
+
+__global__ void __launch_bounds__(128) k_x25519_base_table(double *__restrict__ table)
+{
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= 64 * 8) return;
+    ge_p3 B; ge_p3_basepoint(B);
+    comb_entry(table + (size_t)t * COMB_ENTRY, B, t >> 3, t & 7);
+}
+
+// u(clamp(k) B): 64 mixed additions over the radix-16 signed digits of the clamped, unreduced k (< 2^255, so the
+// recoding of scalar.rs:1019-1051 holds), then u = (Z + Y) / (Z - Y) (C/edwards.rs:580-590).
+__global__ void __launch_bounds__(X25519_COMB_THREADS, 1)
+k_x25519_base(const uint32_t *__restrict__ scalars, const double *__restrict__ table, size_t n, uint32_t *__restrict__ out)
+{
+    extern __shared__ double s_tab[];                             // X25519_COMB_DOUBLES
+    for (int k = threadIdx.x; k < X25519_COMB_DOUBLES; k += blockDim.x) s_tab[k] = table[k];
+    __syncthreads();
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    ge64_p3 acc; ge64_identity(acc);
+    int carry = 0;
+    uint32_t w = 0;
+#pragma unroll 1
+    for (int pos = 0; pos < 64; pos++) {
+        if ((pos & 7) == 0) {                                     // one scalar word per 8 digits, clamped as it is read
+            w = scalars[8 * i + (pos >> 3)];
+            w &= pos == 0 ? 0xfffffff8u : 0xffffffffu;
+            w = pos == 56 ? ((w & 0x7fffffffu) | 0x40000000u) : w;
+        }
+        int d = (int)(w & 15) + carry; w >>= 4;
+        if (pos < 63) { carry = (d + 8) >> 4; d -= carry << 4; }
+        const int m = d >> 31;
+        ge64_niels q;
+        comb_select(q, s_tab + (size_t)pos * 8 * COMB_ENTRY, (uint32_t)((d + m) ^ m));
+        ge64_madd(acc, acc, q, (uint32_t)(d < 0));
+    }
+    fe64 num, den, inv, u;
+    fe64_add(num, acc.Z, acc.Y);                                  // 2
+    fe64_sub(den, acc.Z, acc.Y); fe64_carry(den, den);            // 1
+    x25519_invert(inv, den);
+    fe64_mul(u, num, inv);                                        // 2 x 1
+    uint32_t r[8];
+    x25519_encode(r, u);
+#pragma unroll
+    for (int j = 0; j < 8; j++) out[8 * i + j] = r[j];
+}
+
+static int x25519_table_ensure(dalek_b200_ctx *ctx)
+{
+    if (ctx->x25519_table_ready) return 0;
+    int rc;
+    if ((rc = ws_reserve(ctx, ctx->x25519_table, X25519_COMB_DOUBLES * sizeof(double)))) return rc;
+    CUDA_TRY(ctx, cudaFuncSetAttribute(k_x25519_base, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)(X25519_COMB_DOUBLES * sizeof(double))));
+    k_x25519_base_table<<<4, 128, 0, ctx->stream>>>((double *)ctx->x25519_table.p);
+    ctx->launches++;
+    CUDA_TRY(ctx, cudaGetLastError());
+    ctx->x25519_table_ready = true;
+    return 0;
+}
+
+static void launch_x25519(const void *d_k, const void *d_u, size_t m, void *d_out, void *d_contrib, cudaStream_t st)
+{
+    k_x25519<<<cdiv(m, X25519_THREADS), X25519_THREADS, 0, st>>>((const uint32_t *)d_k, (const uint32_t *)d_u, m,
+                                                               (uint32_t *)d_out, (uint8_t *)d_contrib);
+}
+
+// clear the staged scalars / points and the staged results (zeroize on drop), then wait for the stream
+static int wipe_staging(dalek_b200_ctx *ctx, size_t in_bytes, size_t out_bytes)
+{
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->points_in.p, 0, in_bytes, ctx->stream));
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->points.p, 0, out_bytes, ctx->stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+extern "C" {
+
+int dalek_b200_x25519_batch(dalek_b200_ctx *ctx, const uint8_t *scalars, const uint8_t *us, size_t n, uint8_t *out,
+                            uint8_t *contributory)
+{
+    if (!ctx || (n && (!scalars || !us || !out))) return DALEK_E_INVALID_ARG;
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    if (!n) return DALEK_OK;
+    CallTimer timer(ctx);
+    const size_t c_sz = contributory ? 1 : 0;
+    int rc = run_pieces(ctx, scalars, 32, us, 32, out, 32, contributory, c_sz, n,
+                        [&](const uint8_t *dk, const uint8_t *du, size_t m, uint8_t *d_o, uint8_t *d_c, cudaStream_t st) {
+                            launch_x25519(dk, du, m, d_o, c_sz ? d_c : nullptr, st);
+                        });
+    if (rc) return rc;
+    return wipe_staging(ctx, n * 64, n * (32 + c_sz));
+}
+
+int dalek_b200_x25519_batch_dev(dalek_b200_ctx *ctx, const void *d_scalars, const void *d_us, size_t n, void *d_out,
+                                void *d_contributory)
+{
+    if (!ctx || (n && (!d_scalars || !d_us || !d_out))) return DALEK_E_INVALID_ARG;
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    if (!n) return DALEK_OK;
+    CallTimer timer(ctx);
+    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, ctx->stream));
+    launch_x25519(d_scalars, d_us, n, d_out, d_contributory, ctx->stream);
+    ctx->launches++;
+    CUDA_TRY(ctx, cudaGetLastError());
+    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, ctx->stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    float ms = 0.f;
+    if ((ms = elapsed_ms(ctx->ev_a, ctx->ev_b)) >= 0.f) ctx->last_kernel_ms = ms;
+    ctx->last_kernel_launches = 1;
+    return DALEK_OK;
+}
+
+int dalek_b200_x25519_public_keys(dalek_b200_ctx *ctx, const uint8_t *scalars, size_t n, uint8_t *out)
+{
+    if (!ctx || (n && (!scalars || !out))) return DALEK_E_INVALID_ARG;
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    if (!n) return DALEK_OK;
+    CallTimer timer(ctx);
+    int rc;
+    if ((rc = x25519_table_ensure(ctx))) return rc;
+    const double *table = (const double *)ctx->x25519_table.p;
+    const size_t smem = X25519_COMB_DOUBLES * sizeof(double);
+    rc = run_pieces(ctx, scalars, 32, nullptr, 0, out, 32, nullptr, 0, n,
+                    [&](const uint8_t *dk, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *, cudaStream_t st) {
+                        k_x25519_base<<<cdiv(m, X25519_COMB_THREADS), X25519_COMB_THREADS, smem, st>>>((const uint32_t *)dk, table, m,
+                                                                                                    (uint32_t *)d_o);
+                    });
+    if (rc) return rc;
+    return wipe_staging(ctx, n * 32, n * 32);
+}
+
+}  // extern "C"

@@ -87,6 +87,10 @@ def load_library():
     lib.ed25519_b200_last_zs.argtypes = [vp, vp, sz]
     lib.dalek_b200_edwards_mul_base_batch.argtypes = [vp, vp, sz, vp, vp]
     lib.ed25519_b200_sign_batch_flat.argtypes = [vp, vp, vp, vp, sz, vp, vp]
+    lib.dalek_b200_edwards_to_montgomery_batch.argtypes = [vp, vp, sz, vp]
+    lib.dalek_b200_x25519_batch.argtypes = [vp, vp, vp, sz, vp, vp]
+    lib.dalek_b200_x25519_batch_dev.argtypes = [vp, vp, vp, sz, vp, vp]
+    lib.dalek_b200_x25519_public_keys.argtypes = [vp, vp, sz, vp]
     _lib = lib
     return lib
 
@@ -288,6 +292,41 @@ class Engine:
         self._check(self.lib.dalek_b200_ristretto_double_and_compress_batch(self.h, _ptr(limbs), n, C.addressof(out)))
         return bytes(out)[:32 * n]
 
+    def edwards_to_montgomery_batch(self, limbs, n):
+        """EdwardsPoint::to_montgomery_batch for n points given as 20 u64 limbs each -> n x 32 B (the identity gives 0)."""
+        out = (C.c_uint8 * (32 * max(n, 1)))()
+        self._check(self.lib.dalek_b200_edwards_to_montgomery_batch(self.h, _ptr(limbs), n, C.addressof(out)))
+        return bytes(out)[:32 * n]
+
+    # ---- X25519 ----
+    def x25519_batch(self, scalars, us, n, device_ptrs=False, want_contributory=False, out=None, contributory=None):
+        """x25519(k_i, u_i) for n pairs of 32-byte secrets and u coordinates: (out, contributory or None).
+        Host buffers give bytes.  With device_ptrs the inputs are device buffers (torch CUDA tensors or addresses); the
+        results go to `out` / `contributory` if given (device buffers of 32 n and n bytes), else to new uint8 tensors on
+        the engine's device, which are returned."""
+        if device_ptrs:
+            if out is None or (want_contributory and contributory is None):
+                import torch
+                dev = torch.device("cuda", self.device)
+                if out is None:
+                    out = torch.empty(32 * max(n, 1), dtype=torch.uint8, device=dev)
+                if want_contributory and contributory is None:
+                    contributory = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+            self._check(self.lib.dalek_b200_x25519_batch_dev(self.h, _ptr(scalars), _ptr(us), n, _ptr(out),
+                                                             _ptr(contributory) if want_contributory else None))
+            return out, (contributory if want_contributory else None)
+        res = (C.c_uint8 * (32 * max(n, 1)))()
+        flags = (C.c_uint8 * max(n, 1))() if want_contributory else None
+        self._check(self.lib.dalek_b200_x25519_batch(self.h, _ptr(scalars), _ptr(us), n, C.addressof(res),
+                                                     C.addressof(flags) if want_contributory else None))
+        return bytes(res)[:32 * n], (bytes(flags)[:n] if want_contributory else None)
+
+    def x25519_public_keys(self, scalars, n):
+        """PublicKey::from(&StaticSecret) for n 32-byte secrets -> n x 32 B (constant-time fixed-base comb)."""
+        out = (C.c_uint8 * (32 * max(n, 1)))()
+        self._check(self.lib.dalek_b200_x25519_public_keys(self.h, _ptr(scalars), n, C.addressof(out)))
+        return bytes(out)[:32 * n]
+
     # ---- ed25519 ----
     def verify_batch_raw(self, messages, sigs, pubkeys):
         """messages: list of bytes; sigs: n*64 bytes; pubkeys: n*32 bytes.  Returns the C return code."""
@@ -449,6 +488,49 @@ class EdwardsPoint:
         eng = engine or default_engine()
         rc, comp, _ = eng.edwards_ct_msm(b"".join(scalars), b"".join(points), len(scalars))
         return comp
+
+    @staticmethod
+    def to_montgomery_batch(limbs, n=None, engine=None):
+        """EdwardsPoint::to_montgomery_batch (edwards.rs:592-612): `limbs` holds n points as 20 u64 radix-2^51 limbs
+        each (X | Y | Z | T, e.g. what Engine.mul_base_batch returns); returns the n 32-byte Montgomery u coordinates."""
+        n = len(limbs) // 20 if n is None else n
+        eng = engine or default_engine()
+        raw = eng.edwards_to_montgomery_batch(limbs, n)
+        return [raw[32 * i:32 * i + 32] for i in range(n)]
+
+
+X25519_BASEPOINT_BYTES = bytes([9]) + bytes(31)      # x25519-dalek x25519.rs:385, u = 9
+
+
+def _x25519_items(xs):
+    single = isinstance(xs, (bytes, bytearray))
+    items = [bytes(xs)] if single else [bytes(x) for x in xs]
+    if any(len(x) != 32 for x in items):
+        raise ValueError("X25519 secrets and u coordinates are 32 bytes each")
+    return single, items
+
+
+def x25519(scalars, us, engine=None):
+    """x25519-dalek's x25519(k, u) (x25519.rs:390-392).  One 32-byte secret and u coordinate give 32 bytes; lists of
+    them give the list of shared secrets, computed in one batch."""
+    single, ks = _x25519_items(scalars)
+    _, vs = _x25519_items(us)
+    if len(ks) != len(vs):
+        raise ValueError("scalars and us must have the same length")
+    eng = engine or default_engine()
+    raw, _ = eng.x25519_batch(b"".join(ks), b"".join(vs), len(ks))
+    outs = [raw[32 * i:32 * i + 32] for i in range(len(ks))]
+    return outs[0] if single else outs
+
+
+def x25519_public_keys(secrets, engine=None):
+    """PublicKey::from(&StaticSecret) (x25519.rs:105-110) for each 32-byte secret: one secret gives its 32-byte public
+    key, a list gives the list."""
+    single, ks = _x25519_items(secrets)
+    eng = engine or default_engine()
+    raw = eng.x25519_public_keys(b"".join(ks), len(ks))
+    outs = [raw[32 * i:32 * i + 32] for i in range(len(ks))]
+    return outs[0] if single else outs
 
 
 class _Precomputation:

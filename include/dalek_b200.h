@@ -84,7 +84,7 @@ int dalek_b200_last_kernel_ms(const dalek_b200_ctx *ctx, float *ms, int *launche
  * verify_batch call, the largest kernel of that path; summed over the pieces of a host-streamed call). */
 int dalek_b200_last_stage_ms(const dalek_b200_ctx *ctx, const char *stage, float *ms);
 /* Milliseconds between CUDA events recorded on the context's stream at entry of the last MSM / verify_batch /
- * precomputed-MSM call and after the last work it enqueued (all of the call's streams joined): the device time
+ * precomputed-MSM / X25519 / to_montgomery_batch call and after the last work it enqueued (all of the call's streams joined): the device time
  * of that call, copies of host-buffer calls included. */
 int dalek_b200_last_call_ms(const dalek_b200_ctx *ctx, float *ms);
 
@@ -221,6 +221,25 @@ int dalek_b200_ristretto_decompress_batch(dalek_b200_ctx *ctx, const uint8_t *in
 /* RistrettoPoint::double_and_compress_batch (C/ristretto.rs:564-646): out[i] = compress(2 P_i). */
 int dalek_b200_ristretto_double_and_compress_batch(dalek_b200_ctx *ctx, const uint64_t *limbs, size_t n,
                                                    uint8_t *out);
+/* EdwardsPoint::to_montgomery_batch (C/edwards.rs:592-612): n x 20 u64 limbs -> n x 32 B Montgomery u = (Z+Y)/(Z-Y),
+ * one shared inversion per 8 points; the identity (Z = Y) gives u = 0. */
+int dalek_b200_edwards_to_montgomery_batch(dalek_b200_ctx *ctx, const uint64_t *limbs, size_t n, uint8_t *out);
+
+/* -------- X25519 (x25519-dalek, RFC 7748) ------------------------------------------------------
+ * Scalars are 32-byte secrets, clamped inside the call (clamp_integer, C/scalar.rs:1407-1412) and not reduced; u
+ * coordinates are read like FieldElement::from_bytes (bit 255 ignored, values in [p, 2^255) accepted).  Both calls are
+ * constant time in the secrets: uniform control flow, XOR-mask swaps, full-row table scans.  Host-buffer calls stream
+ * the batch in pieces like the codecs and clear the device copies of the secrets and results before returning.
+ * n = 0 is a successful no-op; a NULL buffer with n > 0 is DALEK_E_INVALID_ARG.  The option "field_f64" has no effect.
+ *
+ * x25519(k_i, u_i) (x25519-dalek x25519.rs:390-392); out: n x 32 B; contributory: n bytes or NULL. Never fails on input values. */
+int dalek_b200_x25519_batch(dalek_b200_ctx *ctx, const uint8_t *scalars, const uint8_t *us, size_t n,
+                            uint8_t *out, uint8_t *contributory);
+/* same, every buffer a device pointer; blocks until done */
+int dalek_b200_x25519_batch_dev(dalek_b200_ctx *ctx, const void *d_scalars, const void *d_us, size_t n,
+                                void *d_out, void *d_contributory);
+/* PublicKey::from(&StaticSecret) = mul_base_clamped(k).to_montgomery(); out: n x 32 B */
+int dalek_b200_x25519_public_keys(dalek_b200_ctx *ctx, const uint8_t *scalars, size_t n, uint8_t *out);
 
 /* -------- scalar batch helpers (SURVEY 8f rank 4) ---------------------------------------------
  * Scalar::from_bytes_mod_order_wide (C/scalar.rs:248-250) for n 64-byte strings -> n canonical 32-byte scalars. */
