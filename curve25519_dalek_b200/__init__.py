@@ -10,6 +10,8 @@ touches the CPU checker used by the tests.  Names follow the reference:
   verify_batch (ed25519-dalek/src/batch.rs:146-251) and its SignatureError values.
   x25519 / x25519_public_keys / X25519_BASEPOINT_BYTES (x25519-dalek/src/x25519.rs:105-110, :385-392)
   EdwardsPoint.to_montgomery_batch (src/edwards.rs:592-612)
+  RistrettoPoint.from_uniform_bytes_batch / hash_from_bytes_batch (src/ristretto.rs:736-790)
+  EdwardsPoint.hash_to_curve_batch / encode_to_curve_batch (src/edwards.rs:710-750, RFC 9380)
 """
 from .engine import (Engine, MultiEngine, EngineError, EdwardsPoint, RistrettoPoint, SignatureError, verify_batch, default_engine,
                      library_path, load_library, POINTS_COMPRESSED, POINTS_EXTENDED, POINTS_RISTRETTO,

@@ -91,6 +91,10 @@ def load_library():
     lib.dalek_b200_x25519_batch.argtypes = [vp, vp, vp, sz, vp, vp]
     lib.dalek_b200_x25519_batch_dev.argtypes = [vp, vp, vp, sz, vp, vp]
     lib.dalek_b200_x25519_public_keys.argtypes = [vp, vp, sz, vp]
+    lib.dalek_b200_ristretto_from_uniform_bytes_batch.argtypes = [vp, vp, sz, vp]
+    lib.dalek_b200_ristretto_hash_from_bytes_batch.argtypes = [vp, vp, vp, sz, vp]
+    lib.dalek_b200_edwards_hash_to_curve_batch.argtypes = [vp, vp, vp, sz, vp, sz, vp]
+    lib.dalek_b200_edwards_encode_to_curve_batch.argtypes = [vp, vp, vp, sz, vp, sz, vp]
     _lib = lib
     return lib
 
@@ -327,6 +331,35 @@ class Engine:
         self._check(self.lib.dalek_b200_x25519_public_keys(self.h, _ptr(scalars), n, C.addressof(out)))
         return bytes(out)[:32 * n]
 
+    # ---- hash to group ----
+    def ristretto_from_uniform_bytes_batch(self, data, n):
+        """RistrettoPoint::from_uniform_bytes for n x 64 B -> n x 32 B CompressedRistretto."""
+        out = (C.c_uint8 * (32 * max(n, 1)))()
+        self._check(self.lib.dalek_b200_ristretto_from_uniform_bytes_batch(self.h, _ptr(data), n, C.addressof(out)))
+        return bytes(out)[:32 * n]
+
+    def ristretto_hash_from_bytes_batch(self, msgs_flat, offsets, n):
+        """RistrettoPoint::hash_from_bytes::<Sha512> for n flat messages (message i = msgs_flat[offsets[i]:offsets[i+1]],
+        n + 1 u64 offsets) -> n x 32 B CompressedRistretto."""
+        out = (C.c_uint8 * (32 * max(n, 1)))()
+        self._check(self.lib.dalek_b200_ristretto_hash_from_bytes_batch(self.h, _ptr(msgs_flat), _ptr(offsets), n, C.addressof(out)))
+        return bytes(out)[:32 * n]
+
+    def _edwards_h2c(self, fn, msgs_flat, offsets, n, dst):
+        out = (C.c_uint8 * (32 * max(n, 1)))()
+        dst = bytes(dst)
+        self._check(fn(self.h, _ptr(msgs_flat), _ptr(offsets), n, _ptr(dst) if dst else None, len(dst), C.addressof(out)))
+        return bytes(out)[:32 * n]
+
+    def edwards_hash_to_curve_batch(self, msgs_flat, offsets, n, dst):
+        """EdwardsPoint::hash_to_curve::<Sha512> (RFC 9380 ..._RO_) for n flat messages and one DST of 1..255 bytes
+        -> n x 32 B CompressedEdwardsY."""
+        return self._edwards_h2c(self.lib.dalek_b200_edwards_hash_to_curve_batch, msgs_flat, offsets, n, dst)
+
+    def edwards_encode_to_curve_batch(self, msgs_flat, offsets, n, dst):
+        """EdwardsPoint::encode_to_curve::<Sha512> (RFC 9380 ..._NU_), same layout as edwards_hash_to_curve_batch."""
+        return self._edwards_h2c(self.lib.dalek_b200_edwards_encode_to_curve_batch, msgs_flat, offsets, n, dst)
+
     # ---- ed25519 ----
     def verify_batch_raw(self, messages, sigs, pubkeys):
         """messages: list of bytes; sigs: n*64 bytes; pubkeys: n*32 bytes.  Returns the C return code."""
@@ -498,6 +531,37 @@ class EdwardsPoint:
         raw = eng.edwards_to_montgomery_batch(limbs, n)
         return [raw[32 * i:32 * i + 32] for i in range(n)]
 
+    @staticmethod
+    def hash_to_curve_batch(messages, dst, engine=None):
+        """EdwardsPoint::hash_to_curve::<Sha512> (edwards.rs:736-750, RFC 9380 edwards25519_XMD:SHA-512_ELL2_RO_) for each
+        message, with one domain separation tag of 1..255 bytes: the list of 32-byte CompressedEdwardsY encodings."""
+        eng = engine or default_engine()
+        flat, offs, n = _flat_messages(messages)
+        raw = eng.edwards_hash_to_curve_batch(flat, offs, n, dst)
+        return [raw[32 * i:32 * i + 32] for i in range(n)]
+
+    @staticmethod
+    def encode_to_curve_batch(messages, dst, engine=None):
+        """EdwardsPoint::encode_to_curve::<Sha512> (edwards.rs:710-721, ..._ELL2_NU_), like hash_to_curve_batch."""
+        eng = engine or default_engine()
+        flat, offs, n = _flat_messages(messages)
+        raw = eng.edwards_encode_to_curve_batch(flat, offs, n, dst)
+        return [raw[32 * i:32 * i + 32] for i in range(n)]
+
+
+def _flat_messages(messages):
+    """Messages back to back with n + 1 u64 offsets (the layout of verify_batch_flat); the buffer is never empty."""
+    msgs = [bytes(m) for m in messages]
+    n = len(msgs)
+    offs = (C.c_uint64 * (n + 1))()
+    acc = 0
+    for i, m in enumerate(msgs):
+        offs[i] = acc
+        acc += len(m)
+    offs[n] = acc
+    flat = b"".join(msgs) + b"\0"
+    return flat, offs, n
+
 
 X25519_BASEPOINT_BYTES = bytes([9]) + bytes(31)      # x25519-dalek x25519.rs:385, u = 9
 
@@ -627,6 +691,26 @@ class RistrettoPoint:
         if rc == 1:
             raise ValueError("G or H is not a valid Ristretto encoding")
         return out
+
+    @staticmethod
+    def from_uniform_bytes_batch(data, engine=None):
+        """RistrettoPoint::from_uniform_bytes (ristretto.rs:774-790) for each 64-byte string: the list of 32-byte
+        CompressedRistretto encodings."""
+        items = [bytes(x) for x in data]
+        if any(len(x) != 64 for x in items):
+            raise ValueError("from_uniform_bytes takes 64 bytes per item")
+        eng = engine or default_engine()
+        raw = eng.ristretto_from_uniform_bytes_batch(b"".join(items), len(items))
+        return [raw[32 * i:32 * i + 32] for i in range(len(items))]
+
+    @staticmethod
+    def hash_from_bytes_batch(messages, engine=None):
+        """RistrettoPoint::hash_from_bytes::<Sha512> (ristretto.rs:736-761) for each message: the list of 32-byte
+        CompressedRistretto encodings."""
+        eng = engine or default_engine()
+        flat, offs, n = _flat_messages(messages)
+        raw = eng.ristretto_hash_from_bytes_batch(flat, offs, n)
+        return [raw[32 * i:32 * i + 32] for i in range(n)]
 
 
 def verify_batch(messages, signatures, verifying_keys, engine=None):

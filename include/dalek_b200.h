@@ -84,7 +84,7 @@ int dalek_b200_last_kernel_ms(const dalek_b200_ctx *ctx, float *ms, int *launche
  * verify_batch call, the largest kernel of that path; summed over the pieces of a host-streamed call). */
 int dalek_b200_last_stage_ms(const dalek_b200_ctx *ctx, const char *stage, float *ms);
 /* Milliseconds between CUDA events recorded on the context's stream at entry of the last MSM / verify_batch /
- * precomputed-MSM / X25519 / to_montgomery_batch call and after the last work it enqueued (all of the call's streams joined): the device time
+ * precomputed-MSM / X25519 / to_montgomery_batch / hash-to-group call and after the last work it enqueued (all of the call's streams joined): the device time
  * of that call, copies of host-buffer calls included. */
 int dalek_b200_last_call_ms(const dalek_b200_ctx *ctx, float *ms);
 
@@ -240,6 +240,27 @@ int dalek_b200_x25519_batch_dev(dalek_b200_ctx *ctx, const void *d_scalars, cons
                                 void *d_out, void *d_contributory);
 /* PublicKey::from(&StaticSecret) = mul_base_clamped(k).to_montgomery(); out: n x 32 B */
 int dalek_b200_x25519_public_keys(dalek_b200_ctx *ctx, const uint8_t *scalars, size_t n, uint8_t *out);
+
+/* -------- hash to group ------------------------------------------------------------------------
+ * Host buffers; each call blocks and streams the batch in pieces like the codecs.  The maps are total: these calls never
+ * return DALEK_NONE.  n = 0 is a successful no-op; a NULL buffer with n > 0 is DALEK_E_INVALID_ARG.  Messages are laid out
+ * back to back as in ed25519_b200_verify_each_flat: message i = msgs_flat[msg_offsets[i] .. msg_offsets[i+1]) (n + 1
+ * offsets), msg_offsets[0] must be 0 and the offsets must not decrease, else DALEK_E_INVALID_ARG.  Constant time in the
+ * message bytes (only the lengths of the messages and of the DST shape the work).  No option affects these calls.
+ *
+ * RistrettoPoint::from_uniform_bytes (C/ristretto.rs:774-790): in n x 64 B -> out n x 32 B CompressedRistretto */
+int dalek_b200_ristretto_from_uniform_bytes_batch(dalek_b200_ctx *ctx, const uint8_t *in, size_t n, uint8_t *out);
+/* RistrettoPoint::hash_from_bytes::<Sha512> (C/ristretto.rs:736-761): out n x 32 B CompressedRistretto */
+int dalek_b200_ristretto_hash_from_bytes_batch(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets,
+                                               size_t n, uint8_t *out);
+/* EdwardsPoint::hash_to_curve::<Sha512> (C/edwards.rs:736-750, RFC 9380 edwards25519_XMD:SHA-512_ELL2_RO_) and
+ * EdwardsPoint::encode_to_curve::<Sha512> (C/edwards.rs:710-721, ..._ELL2_NU_): one DST of 1..255 bytes for the whole batch
+ * (dst_len 0 or > 255 is DALEK_E_INVALID_ARG, where the reference panics, C/field.rs:457-462); out n x 32 B
+ * CompressedEdwardsY */
+int dalek_b200_edwards_hash_to_curve_batch(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets,
+                                           size_t n, const uint8_t *dst, size_t dst_len, uint8_t *out);
+int dalek_b200_edwards_encode_to_curve_batch(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets,
+                                             size_t n, const uint8_t *dst, size_t dst_len, uint8_t *out);
 
 /* -------- scalar batch helpers (SURVEY 8f rank 4) ---------------------------------------------
  * Scalar::from_bytes_mod_order_wide (C/scalar.rs:248-250) for n 64-byte strings -> n canonical 32-byte scalars. */
