@@ -156,13 +156,12 @@ int dalek_b200_edwards_mul_base_batch(dalek_b200_ctx *ctx, const uint8_t *scalar
 int ed25519_b200_sign_batch_flat(dalek_b200_ctx *ctx, const uint8_t *seeds, const uint8_t *msgs_flat,
                                  const uint64_t *msg_offsets, size_t n, uint8_t *pubkeys_out, uint8_t *sigs_out)
 {
-    if (!ctx || (n && (!seeds || !msg_offsets || !pubkeys_out || !sigs_out))) return DALEK_E_INVALID_ARG;
+    if (!ctx || (n && (!seeds || !pubkeys_out || !sigs_out)) || !flat_messages_ok(msgs_flat, msg_offsets, n)) return DALEK_E_INVALID_ARG;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     int rc;
     cudaStream_t st = ctx->stream;
     if ((rc = base_table_ensure(ctx))) return rc;
     if (!n) return 0;
-    for (size_t i = 0; i < n; i++) if (msg_offsets[i] > msg_offsets[i + 1]) return DALEK_E_INVALID_ARG;   // offsets must not decrease
     size_t mbytes = (size_t)msg_offsets[n];
     if ((rc = ws_reserve(ctx, ctx->scalars, n * 32))) return rc;
     if ((rc = ws_reserve(ctx, ctx->misc1, mbytes + 16))) return rc;

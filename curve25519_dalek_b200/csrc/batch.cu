@@ -1003,7 +1003,7 @@ int ed25519_b200_verify_batch_flat_points_dev(dalek_b200_ctx *ctx, const void *d
 int ed25519_b200_verify_batch_flat_points(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets,
                                           const uint8_t *sigs, const uint8_t *pubkeys, const uint64_t *key_points, size_t n)
 {
-    if (!ctx || (n && (!msg_offsets || !sigs || !pubkeys || !key_points))) return DALEK_E_INVALID_ARG;
+    if (!ctx || (n && (!sigs || !pubkeys || !key_points))) return DALEK_E_INVALID_ARG;
     return verify_host(ctx, msgs_flat, msg_offsets, sigs, pubkeys, n, 0, nullptr, key_points);
 }
 
@@ -1020,7 +1020,7 @@ int ed25519_b200_verify_batches_flat_dev(dalek_b200_ctx *ctx, const void *d_msgs
 int ed25519_b200_verify_batches_flat(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets,
                                      const uint8_t *sigs, const uint8_t *pubkeys, size_t n, size_t batch_size, int32_t *verdicts)
 {
-    if (!ctx || !batch_size || batch_size > (1u << 20) || (n && (!msg_offsets || !sigs || !pubkeys || !verdicts))) return DALEK_E_INVALID_ARG;
+    if (!ctx || !batch_size || batch_size > (1u << 20) || (n && (!sigs || !pubkeys || !verdicts))) return DALEK_E_INVALID_ARG;
     ChunkOverride guard(ctx, batch_size);
     return verify_host(ctx, msgs_flat, msg_offsets, sigs, pubkeys, n, batch_size, verdicts);
 }
@@ -1040,7 +1040,7 @@ int ed25519_b200_verify_batches_flat_points_dev(dalek_b200_ctx *ctx, const void 
 int ed25519_b200_verify_batches_flat_points(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets, const uint8_t *sigs,
                                             const uint8_t *pubkeys, const uint64_t *key_points, size_t n, size_t batch_size, int32_t *verdicts)
 {
-    if (!ctx || !batch_size || batch_size > (1u << 20) || (n && (!msg_offsets || !sigs || !pubkeys || !key_points || !verdicts)))
+    if (!ctx || !batch_size || batch_size > (1u << 20) || (n && (!sigs || !pubkeys || !key_points || !verdicts)))
         return DALEK_E_INVALID_ARG;
     ChunkOverride guard(ctx, batch_size);
     return verify_host(ctx, msgs_flat, msg_offsets, sigs, pubkeys, n, batch_size, verdicts, key_points);
@@ -1049,7 +1049,7 @@ int ed25519_b200_verify_batches_flat_points(dalek_b200_ctx *ctx, const uint8_t *
 int ed25519_b200_verify_batch_flat(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets,
                                    const uint8_t *sigs, const uint8_t *pubkeys, size_t n)
 {
-    if (!ctx || (n && (!msg_offsets || !sigs || !pubkeys))) return DALEK_E_INVALID_ARG;
+    if (!ctx || (n && (!sigs || !pubkeys))) return DALEK_E_INVALID_ARG;
     return verify_host(ctx, msgs_flat, msg_offsets, sigs, pubkeys, n, 0, nullptr);
 }
 
@@ -1058,12 +1058,11 @@ int ed25519_b200_verify_batch_flat(dalek_b200_ctx *ctx, const uint8_t *msgs_flat
 static int verify_host(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets, const uint8_t *sigs,
                        const uint8_t *pubkeys, size_t n, size_t batch, int32_t *verdicts, const uint64_t *key_points)
 {
+    if (!flat_messages_ok(msgs_flat, msg_offsets, n)) return DALEK_E_INVALID_ARG;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     CallTimer timer(ctx);
     int rc;
     size_t mbytes = n ? (size_t)msg_offsets[n] : 0;
-    if (n && msg_offsets[0] != 0) return DALEK_E_INVALID_ARG;
-    for (size_t i = 0; i < n; i++) if (msg_offsets[i] > msg_offsets[i + 1]) return DALEK_E_INVALID_ARG;   // a negative length would read outside the staging buffer
     if ((rc = ws_reserve(ctx, ctx->misc1, mbytes + 16))) return rc;
     if ((rc = ws_reserve(ctx, ctx->msg_offs, (n + 1) * 8))) return rc;
     if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * 96))) return rc;   // sigs + keys

@@ -213,10 +213,14 @@ int dalek_b200_edwards_decompress_batch(dalek_b200_ctx *ctx, const uint8_t *in, 
 {
     if (!ctx || (n && (!in || !out_limbs || !ok))) return DALEK_E_INVALID_ARG;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    CallTimer timer(ctx);
     const bool f64 = ctx->opt_decompress_f64 != 0;
-    int rc = run_pieces(ctx, in, 32, nullptr, 0, (uint8_t *)out_limbs, 160, ok, 1, n, [&](const uint8_t *di, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *d_ok, cudaStream_t st) {
+    int rc = run_pieces(ctx, nullptr, nullptr, in, 32, nullptr, 0, (uint8_t *)out_limbs, 160, ok, 1, n,
+                        [&](const uint8_t *, const uint64_t *, const uint8_t *di, const uint8_t *, size_t m, uint8_t *d_o,
+                            uint8_t *d_ok, cudaStream_t st) {
         if (f64) k_decompress_batch<1><<<cdiv(m, 128), 128, 0, st>>>((const uint32_t *)di, m, (uint64_t *)d_o, d_ok);
         else k_decompress_batch<0><<<cdiv(m, 128), 128, 0, st>>>((const uint32_t *)di, m, (uint64_t *)d_o, d_ok);
+        return 0;
     });
     if (rc) return rc;
     uint8_t all = 1;
@@ -228,10 +232,14 @@ int dalek_b200_ristretto_decompress_batch(dalek_b200_ctx *ctx, const uint8_t *in
 {
     if (!ctx || (n && (!in || !out_limbs || !ok))) return DALEK_E_INVALID_ARG;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    CallTimer timer(ctx);
     const bool f64 = ctx->opt_decompress_f64 != 0;
-    int rc = run_pieces(ctx, in, 32, nullptr, 0, (uint8_t *)out_limbs, 160, ok, 1, n, [&](const uint8_t *di, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *d_ok, cudaStream_t st) {
+    int rc = run_pieces(ctx, nullptr, nullptr, in, 32, nullptr, 0, (uint8_t *)out_limbs, 160, ok, 1, n,
+                        [&](const uint8_t *, const uint64_t *, const uint8_t *di, const uint8_t *, size_t m, uint8_t *d_o,
+                            uint8_t *d_ok, cudaStream_t st) {
         if (f64) k_ristretto_decompress_batch<1><<<cdiv(m, 128), 128, 0, st>>>((const uint32_t *)di, m, (uint64_t *)d_o, d_ok);
         else k_ristretto_decompress_batch<0><<<cdiv(m, 128), 128, 0, st>>>((const uint32_t *)di, m, (uint64_t *)d_o, d_ok);
+        return 0;
     });
     if (rc) return rc;
     uint8_t all = 1;
@@ -243,8 +251,12 @@ int dalek_b200_edwards_compress_batch(dalek_b200_ctx *ctx, const uint64_t *limbs
 {
     if (!ctx || (n && (!limbs || !out))) return DALEK_E_INVALID_ARG;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    return run_pieces(ctx, (const uint8_t *)limbs, 160, nullptr, 0, out, 32, nullptr, 0, n, [&](const uint8_t *di, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *, cudaStream_t st) {
+    CallTimer timer(ctx);
+    return run_pieces(ctx, nullptr, nullptr, (const uint8_t *)limbs, 160, nullptr, 0, out, 32, nullptr, 0, n,
+                      [&](const uint8_t *, const uint64_t *, const uint8_t *di, const uint8_t *, size_t m, uint8_t *d_o,
+                          uint8_t *, cudaStream_t st) {
         k_compress_batch<<<cdiv(cdiv(m, CODEC_K), 128), 128, 0, st>>>((const uint64_t *)di, m, (uint32_t *)d_o);
+        return 0;
     });
 }
 
@@ -252,8 +264,12 @@ int dalek_b200_ristretto_double_and_compress_batch(dalek_b200_ctx *ctx, const ui
 {
     if (!ctx || (n && (!limbs || !out))) return DALEK_E_INVALID_ARG;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    return run_pieces(ctx, (const uint8_t *)limbs, 160, nullptr, 0, out, 32, nullptr, 0, n, [&](const uint8_t *di, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *, cudaStream_t st) {
+    CallTimer timer(ctx);
+    return run_pieces(ctx, nullptr, nullptr, (const uint8_t *)limbs, 160, nullptr, 0, out, 32, nullptr, 0, n,
+                      [&](const uint8_t *, const uint64_t *, const uint8_t *di, const uint8_t *, size_t m, uint8_t *d_o,
+                          uint8_t *, cudaStream_t st) {
         k_ristretto_double_and_compress_batch<<<cdiv(cdiv(m, CODEC_K), 128), 128, 0, st>>>((const uint64_t *)di, m, (uint32_t *)d_o);
+        return 0;
     });
 }
 
@@ -263,8 +279,11 @@ int dalek_b200_edwards_to_montgomery_batch(dalek_b200_ctx *ctx, const uint64_t *
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     if (!n) return DALEK_OK;
     CallTimer timer(ctx);
-    return run_pieces(ctx, (const uint8_t *)limbs, 160, nullptr, 0, out, 32, nullptr, 0, n, [&](const uint8_t *di, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *, cudaStream_t st) {
+    return run_pieces(ctx, nullptr, nullptr, (const uint8_t *)limbs, 160, nullptr, 0, out, 32, nullptr, 0, n,
+                      [&](const uint8_t *, const uint64_t *, const uint8_t *di, const uint8_t *, size_t m, uint8_t *d_o,
+                          uint8_t *, cudaStream_t st) {
         k_to_montgomery_batch<<<cdiv(cdiv(m, CODEC_K), 128), 128, 0, st>>>((const uint64_t *)di, m, (uint32_t *)d_o);
+        return 0;
     });
 }
 

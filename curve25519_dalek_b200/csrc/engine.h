@@ -129,6 +129,18 @@ inline void trace_dump(dalek_b200_ctx *ctx)
     ctx->trace.clear();
 }
 
+// The rule for flat messages of the host-buffer calls (include/dalek_b200.h, hash to group): for n > 0 the n + 1 offsets
+// start at 0 and do not decrease, and msgs_flat may be NULL only when every message is empty.  A negative length would
+// read outside the staging buffer.
+inline bool flat_messages_ok(const uint8_t *msgs_flat, const uint64_t *offsets, size_t n)
+{
+    if (!n) return true;
+    if (!offsets || offsets[0] != 0) return false;
+    for (size_t i = 0; i < n; i++)
+        if (offsets[i] > offsets[i + 1]) return false;
+    return msgs_flat || offsets[n] == 0;
+}
+
 int ws_reserve(dalek_b200_ctx *ctx, DevBuf &b, size_t bytes);
 int pinned_reserve(dalek_b200_ctx *ctx, size_t bytes);
 
@@ -198,5 +210,3 @@ int base_table_ensure(dalek_b200_ctx *ctx);
 
 int ristretto_prepare_points(dalek_b200_ctx *ctx, const void *d_in, size_t n, void *d_out, int *d_bad);
 int ristretto_encode_result(dalek_b200_ctx *ctx, const MsmResult *d_res, uint32_t *d_enc);
-int ristretto_double_base(dalek_b200_ctx *ctx, const uint8_t *d_a, const uint8_t *d_b, const uint8_t G[32],
-                          const uint8_t H[32], size_t n, uint8_t *d_out, int *h_status);

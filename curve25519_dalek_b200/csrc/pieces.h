@@ -1,36 +1,52 @@
 // pieces.h -- host buffers in and out, streamed in pieces over the context's two streams (copy-in -> kernel ->
 // copy-out), for batch calls whose items are independent: the PCIe traffic of one piece hides under the arithmetic
-// of its neighbours.  Used by the codecs (codecs.cu) and the X25519 batches (x25519.cu).
+// of its neighbours.  Used by the codecs, X25519, hash-to-group, the plain path of verify_each and the double-base batch.
 #pragma once
 #include <algorithm>
 
 #include "engine.h"
 
-// Per item: in_sz bytes of `in`, optionally in2_sz bytes of a second input `in2` (in2_sz = 0: none), out_sz bytes of
-// `out` and optionally out2_sz bytes of a second output `out2`.  The inputs are staged in ctx->points_in (first all of
-// `in`, then all of `in2`), the outputs in ctx->points.  launch(d_in, d_in2, m, d_out, d_out2, stream) enqueues the
-// kernel of one piece of m items.  Sets last_kernel_ms to the device span of the whole batch, copies included.
+// Per item: optionally a message of the flat layout (msgs + n + 1 offsets, include/dalek_b200.h; offs = NULL: none),
+// in_sz bytes of `in` (0: none), optionally in2_sz bytes of a second input `in2`, out_sz bytes of `out` and optionally
+// out2_sz bytes of a second output `out2`.  The messages are staged in ctx->misc1 at their own offsets and the offsets in
+// ctx->msg_offs, the fixed-width inputs in ctx->points_in (first all of `in`, then all of `in2`), the outputs in
+// ctx->points.  launch(d_msgs, d_offs, d_in, d_in2, m, d_out, d_out2, stream) enqueues the kernel of one piece of m items
+// and returns an engine code; d_offs points at the piece's m + 1 offsets, which stay absolute (d_msgs is the base of the
+// whole staged buffer).  Pieces hold `piece` items (0: 2^16 from 2^17 items up, else one piece).  Sets last_kernel_ms
+// to the device span of the whole batch, copies included, and last_kernel_launches to the number of pieces.
 template <typename Launch>
-static int run_pieces(dalek_b200_ctx *ctx, const uint8_t *in, size_t in_sz, const uint8_t *in2, size_t in2_sz, uint8_t *out,
-                      size_t out_sz, uint8_t *out2, size_t out2_sz, size_t n, Launch launch)
+static int run_pieces(dalek_b200_ctx *ctx, const uint8_t *msgs, const uint64_t *offs, const uint8_t *in, size_t in_sz,
+                      const uint8_t *in2, size_t in2_sz, uint8_t *out, size_t out_sz, uint8_t *out2, size_t out2_sz, size_t n,
+                      Launch launch, size_t piece = 0)
 {
     int rc;
+    if (offs) {
+        if ((rc = ws_reserve(ctx, ctx->misc1, (n ? (size_t)offs[n] : 0) + 16))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->msg_offs, (n + 1) * 8))) return rc;
+    }
     if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * (in_sz + in2_sz)))) return rc;
     if ((rc = ws_reserve(ctx, ctx->points, std::max<size_t>(1, n) * (out_sz + out2_sz)))) return rc;
-    uint8_t *d_in = (uint8_t *)ctx->points_in.p, *d_in2 = d_in + n * in_sz;
+    uint8_t *d_msgs = (uint8_t *)ctx->misc1.p, *d_in = (uint8_t *)ctx->points_in.p, *d_in2 = d_in + n * in_sz;
     uint8_t *d_out = (uint8_t *)ctx->points.p, *d_out2 = d_out + n * out_sz;
+    uint64_t *d_offs = (uint64_t *)ctx->msg_offs.p;
     cudaStream_t ss[2] = {ctx->stream, ctx->stream2};
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, ctx->stream));
     CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->ev_fork, 0));
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, ctx->stream));
-    const size_t piece = n >= (1u << 17) ? (size_t)1 << 16 : std::max<size_t>(1, n);   // a multiple of 128 * 8
+    if (!piece) piece = n >= (1u << 17) ? (size_t)1 << 16 : std::max<size_t>(1, n);   // a multiple of 128 * 8
     size_t k = 0;
     for (size_t lo = 0; lo < n; lo += piece, k++) {
         const size_t m = std::min(piece, n - lo);
         cudaStream_t st = ss[k & 1];
-        CUDA_TRY(ctx, cudaMemcpyAsync(d_in + lo * in_sz, in + lo * in_sz, m * in_sz, cudaMemcpyHostToDevice, st));
+        if (offs) {
+            const size_t m0 = (size_t)offs[lo], m1 = (size_t)offs[lo + m];
+            if (m1 > m0) CUDA_TRY(ctx, cudaMemcpyAsync(d_msgs + m0, msgs + m0, m1 - m0, cudaMemcpyHostToDevice, st));
+            CUDA_TRY(ctx, cudaMemcpyAsync(d_offs + lo, offs + lo, (m + 1) * 8, cudaMemcpyHostToDevice, st));
+        }
+        if (in_sz) CUDA_TRY(ctx, cudaMemcpyAsync(d_in + lo * in_sz, in + lo * in_sz, m * in_sz, cudaMemcpyHostToDevice, st));
         if (in2_sz) CUDA_TRY(ctx, cudaMemcpyAsync(d_in2 + lo * in2_sz, in2 + lo * in2_sz, m * in2_sz, cudaMemcpyHostToDevice, st));
-        launch(d_in + lo * in_sz, d_in2 + lo * in2_sz, m, d_out + lo * out_sz, d_out2 + lo * out2_sz, st);
+        if ((rc = launch(d_msgs, d_offs + lo, d_in + lo * in_sz, d_in2 + lo * in2_sz, m, d_out + lo * out_sz, d_out2 + lo * out2_sz, st)))
+            return rc;
         ctx->launches++;
         CUDA_TRY(ctx, cudaGetLastError());
         CUDA_TRY(ctx, cudaMemcpyAsync(out + lo * out_sz, d_out + lo * out_sz, m * out_sz, cudaMemcpyDeviceToHost, st));

@@ -21,6 +21,7 @@
 #include "engine.h"
 #include "ge64.cuh"
 #include "hash.cuh"
+#include "pieces.h"
 #include "sc.cuh"
 
 static inline unsigned cdiv(size_t a, unsigned b) { return (unsigned)((a + b - 1) / b); }
@@ -407,23 +408,21 @@ int ed25519_b200_verify_each_flat_dev(dalek_b200_ctx *ctx, const void *d_msgs_fl
 int ed25519_b200_verify_each_flat(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets, const uint8_t *sigs,
                                   const uint8_t *pubkeys, size_t n, int strict, uint8_t *results)
 {
-    if (!ctx || (n && (!msg_offsets || !sigs || !pubkeys || !results))) return DALEK_E_INVALID_ARG;
-    if (n && msg_offsets[0] != 0) return DALEK_E_INVALID_ARG;
-    for (size_t i = 0; i < n; i++) if (msg_offsets[i] > msg_offsets[i + 1]) return DALEK_E_INVALID_ARG;   // offsets must not decrease
+    if (!ctx || (n && (!sigs || !pubkeys || !results)) || !flat_messages_ok(msgs_flat, msg_offsets, n)) return DALEK_E_INVALID_ARG;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     CallTimer timer(ctx);
     int rc;
-    const size_t mbytes = n ? (size_t)msg_offsets[n] : 0;
     if ((rc = base_table_ensure(ctx))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->misc1, mbytes + 16))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->msg_offs, (n + 1) * 8))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * 96))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->misc6, std::max<size_t>(1, n)))) return rc;
-    uint8_t *d_msgs = (uint8_t *)ctx->misc1.p, *d_sigs = (uint8_t *)ctx->points_in.p, *d_keys = d_sigs + n * 64, *d_out = (uint8_t *)ctx->misc6.p;
-    uint64_t *d_offs = (uint64_t *)ctx->msg_offs.p;
     if (ctx->opt_each_comb && ctx->opt_field_f64 && n) {
         // keys may repeat: everything crosses PCIe first (the key tables need every key), then either the comb path or,
         // when the keys turn out not to repeat, the plain kernel on the resident copies
+        const size_t mbytes = (size_t)msg_offsets[n];
+        if ((rc = ws_reserve(ctx, ctx->misc1, mbytes + 16))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->msg_offs, (n + 1) * 8))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->points_in, n * 96))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->misc6, n))) return rc;
+        uint8_t *d_msgs = (uint8_t *)ctx->misc1.p, *d_sigs = (uint8_t *)ctx->points_in.p, *d_keys = d_sigs + n * 64, *d_out = (uint8_t *)ctx->misc6.p;
+        uint64_t *d_offs = (uint64_t *)ctx->msg_offs.p;
         cudaStream_t st = ctx->stream;
         if (mbytes) CUDA_TRY(ctx, cudaMemcpyAsync(d_msgs, msgs_flat, mbytes, cudaMemcpyHostToDevice, st));
         CUDA_TRY(ctx, cudaMemcpyAsync(d_offs, msg_offsets, (n + 1) * 8, cudaMemcpyHostToDevice, st));
@@ -434,32 +433,18 @@ int ed25519_b200_verify_each_flat(dalek_b200_ctx *ctx, const uint8_t *msgs_flat,
         if (!comb && (rc = verify_each_dev(ctx, d_msgs, d_offs, (const uint32_t *)d_sigs, (const uint32_t *)d_keys, n, strict, d_out, st))) return rc;
         CUDA_TRY(ctx, cudaMemcpyAsync(results, d_out, n, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(ctx, cudaStreamSynchronize(st));
-        uint8_t any = 0;
-        for (size_t i = 0; i < n; i++) any |= results[i];
-        return any ? ED25519_ERR_VERIFY : DALEK_OK;
+    } else {
+        // independent per signature: pieces alternate between two streams (copy-in -> kernel -> copy-out)
+        const ge_niels_packed *base = (const ge_niels_packed *)ctx->base_table.p;
+        rc = run_pieces(ctx, msgs_flat, msg_offsets, sigs, 64, pubkeys, 32, results, 1, nullptr, 0, n,
+                        [&](const uint8_t *d_msgs, const uint64_t *d_offs, const uint8_t *d_sigs, const uint8_t *d_keys, size_t m,
+                            uint8_t *d_out, uint8_t *, cudaStream_t st) {
+                            k_verify_each<<<cdiv(m, 128), 128, 0, st>>>(d_msgs, d_offs, (const uint32_t *)d_sigs, (const uint32_t *)d_keys,
+                                                                        m, strict, base, d_out);
+                            return 0;
+                        });
+        if (rc) return rc;
     }
-    // independent per signature: pieces alternate between two streams (copy-in -> kernel -> copy-out)
-    cudaStream_t ss[2] = {ctx->stream, ctx->stream2};
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, ctx->stream));
-    CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->ev_fork, 0));
-    const size_t piece = n >= (1u << 17) ? (size_t)1 << 16 : std::max<size_t>(1, n);
-    size_t k = 0;
-    for (size_t lo = 0; lo < n; lo += piece, k++) {
-        const size_t m = std::min(piece, n - lo);
-        cudaStream_t st = ss[k & 1];
-        const size_t m0 = (size_t)msg_offsets[lo], m1 = (size_t)msg_offsets[lo + m];
-        if (m1 > m0) CUDA_TRY(ctx, cudaMemcpyAsync(d_msgs + m0, msgs_flat + m0, m1 - m0, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(ctx, cudaMemcpyAsync(d_offs + lo, msg_offsets + lo, (m + 1) * 8, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(ctx, cudaMemcpyAsync(d_sigs + lo * 64, sigs + lo * 64, m * 64, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(ctx, cudaMemcpyAsync(d_keys + lo * 32, pubkeys + lo * 32, m * 32, cudaMemcpyHostToDevice, st));
-        // offsets are absolute: the kernel indexes msgs by them, so pass the bases shifted by the piece start
-        if ((rc = verify_each_dev(ctx, d_msgs, d_offs + lo, (const uint32_t *)(d_sigs + lo * 64), (const uint32_t *)(d_keys + lo * 32), m, strict,
-                                  d_out + lo, st))) return rc;
-        CUDA_TRY(ctx, cudaMemcpyAsync(results + lo, d_out + lo, m, cudaMemcpyDeviceToHost, st));
-    }
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_join, ctx->stream2));
-    CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
-    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     uint8_t any = 0;
     for (size_t i = 0; i < n; i++) any |= results[i];
     return any ? ED25519_ERR_VERIFY : DALEK_OK;

@@ -17,6 +17,7 @@
 #include "comb.cuh"
 #include "engine.h"
 #include "ge64.cuh"
+#include "pieces.h"
 
 static inline unsigned cdiv(size_t a, unsigned b) { return (unsigned)((a + b - 1) / b); }
 void launch_niels_to_pniels(dalek_b200_ctx *ctx, const void *in, void *out, size_t n);
@@ -309,17 +310,14 @@ static int double_base_setup(dalek_b200_ctx *ctx, const uint8_t G[32], const uin
     return 0;
 }
 
-static int double_base_launch(dalek_b200_ctx *ctx, const DoubleBasePlan &plan, const uint8_t *d_a, const uint8_t *d_b, size_t n,
-                              uint8_t *d_out, cudaStream_t st)
+// enqueues the kernel of n >= 1 pairs
+static void double_base_launch(const DoubleBasePlan &plan, const uint8_t *d_a, const uint8_t *d_b, size_t n, uint8_t *d_out,
+                               cudaStream_t st)
 {
-    if (!n) return 0;
     const uint32_t *a = (const uint32_t *)d_a, *b = (const uint32_t *)d_b;
     // 384 threads x 168 registers fill the register file with the 120 KiB table resident (512 x 128 spills; measured slower)
     if (plan.variant == 1) k_double_base_comb<384><<<cdiv(n, 384), 384, plan.smem, st>>>(a, b, (const double *)plan.table, n, (uint32_t *)d_out);
     else k_double_base<<<cdiv(n, 128), 128, 0, st>>>(a, b, (const uint32_t *)plan.table, n, (uint32_t *)d_out);
-    ctx->launches++;
-    CUDA_TRY(ctx, cudaGetLastError());
-    return 0;
 }
 
 static int double_base_status(dalek_b200_ctx *ctx, const DoubleBasePlan &plan, int *h_status)
@@ -328,24 +326,8 @@ static int double_base_status(dalek_b200_ctx *ctx, const DoubleBasePlan &plan, i
     int *hs = (int *)((char *)ctx->h_pinned + 128);
     CUDA_TRY(ctx, cudaMemcpyAsync(hs, plan.d_status, 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(ctx, cudaStreamSynchronize(st));
-    float ms = 0.f;
-    if ((ms = elapsed_ms(ctx->ev_a, ctx->ev_b)) >= 0.f) ctx->last_kernel_ms = ms;
-    ctx->last_kernel_launches = 1;
     *h_status = *hs;
     return 0;
-}
-
-// device-resident scalars in, device-resident encodings out
-int ristretto_double_base(dalek_b200_ctx *ctx, const uint8_t *d_a, const uint8_t *d_b, const uint8_t G[32], const uint8_t H[32],
-                          size_t n, uint8_t *d_out, int *h_status)
-{
-    int rc;
-    DoubleBasePlan plan;
-    if ((rc = double_base_setup(ctx, G, H, n, plan))) return rc;
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, ctx->stream));
-    if ((rc = double_base_launch(ctx, plan, d_a, d_b, n, d_out, ctx->stream))) return rc;
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, ctx->stream));
-    return double_base_status(ctx, plan, h_status);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -454,35 +436,24 @@ int dalek_b200_ristretto_double_base_batch(dalek_b200_ctx *ctx, const uint8_t *a
         for (size_t i = 0; i < n; i++) top |= a[32 * i + 31] | b[32 * i + 31];
         if (top & 0x80) { ctx->last_error = "scalar with bit 255 set (Scalar invariant #1)"; return DALEK_E_INVALID_ARG; }
     }
+    CallTimer timer(ctx);
     int rc;
-    if ((rc = ws_reserve(ctx, ctx->scalars, std::max<size_t>(1, n) * 64))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * 32))) return rc;
-    uint8_t *d_a = (uint8_t *)ctx->scalars.p, *d_b = d_a + n * 32, *d_out = (uint8_t *)ctx->points_in.p;
     DoubleBasePlan plan;
     if ((rc = double_base_setup(ctx, G, H, n, plan))) return rc;
-    // The batch is independent per pair: pieces alternate between two streams, each doing copy-in -> kernel ->
-    // copy-out, so that the PCIe traffic of one piece (both directions) hides under the arithmetic of its
-    // neighbours.  (With pageable caller memory the copies are staged by the driver and overlap less.)
-    cudaStream_t ss[2] = {ctx->stream, ctx->stream2};
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, ctx->stream));
-    CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->ev_fork, 0));
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, ctx->stream));
-    // piece size: two full waves of the comb kernel (one 384-thread CTA per SM), so that no piece ends in a
-    // partly filled wave; the per-pair Straus kernel has small CTAs and simply gets 8 pieces
+    // The batch is independent per pair: the PCIe traffic of one piece (both directions) hides under the arithmetic of
+    // its neighbours.  (With pageable caller memory the copies are staged by the driver and overlap less.)  Pieces of a
+    // large batch: two full waves of the comb kernel (one 384-thread CTA per SM), so that no piece ends in a partly
+    // filled wave; the per-pair Straus kernel has small CTAs and simply gets 8 pieces.
     size_t piece = n;
     if (n >= (1u << 16)) piece = plan.variant == 1 ? (size_t)2 * ctx->sm_count * 384 : (n + 7) / 8;
-    size_t k = 0;
-    for (size_t lo = 0; lo < n; lo += piece, k++) {
-        const size_t m = std::min(piece, n - lo);
-        cudaStream_t st = ss[k & 1];
-        CUDA_TRY(ctx, cudaMemcpyAsync(d_a + 32 * lo, a + 32 * lo, 32 * m, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(ctx, cudaMemcpyAsync(d_b + 32 * lo, b + 32 * lo, 32 * m, cudaMemcpyHostToDevice, st));
-        if ((rc = double_base_launch(ctx, plan, d_a + 32 * lo, d_b + 32 * lo, m, d_out + 32 * lo, st))) return rc;
-        CUDA_TRY(ctx, cudaMemcpyAsync(out + 32 * lo, d_out + 32 * lo, 32 * m, cudaMemcpyDeviceToHost, st));
-    }
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_join, ctx->stream2));
-    CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, ctx->stream));          // ev_a .. ev_b: device span of the whole batch, copies included
+    rc = run_pieces(ctx, nullptr, nullptr, a, 32, b, 32, out, 32, nullptr, 0, n,
+                    [&](const uint8_t *, const uint64_t *, const uint8_t *d_a, const uint8_t *d_b, size_t m, uint8_t *d_out, uint8_t *,
+                        cudaStream_t st) {
+                        double_base_launch(plan, d_a, d_b, m, d_out, st);
+                        return 0;
+                    },
+                    piece);
+    if (rc) return rc;
     int status = 0;
     if ((rc = double_base_status(ctx, plan, &status))) return rc;
     if (status) return DALEK_NONE;                                   // G or H does not decode; `out` is unspecified

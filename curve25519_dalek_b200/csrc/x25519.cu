@@ -124,9 +124,11 @@ int dalek_b200_x25519_batch(dalek_b200_ctx *ctx, const uint8_t *scalars, const u
     if (!n) return DALEK_OK;
     CallTimer timer(ctx);
     const size_t c_sz = contributory ? 1 : 0;
-    int rc = run_pieces(ctx, scalars, 32, us, 32, out, 32, contributory, c_sz, n,
-                        [&](const uint8_t *dk, const uint8_t *du, size_t m, uint8_t *d_o, uint8_t *d_c, cudaStream_t st) {
+    int rc = run_pieces(ctx, nullptr, nullptr, scalars, 32, us, 32, out, 32, contributory, c_sz, n,
+                        [&](const uint8_t *, const uint64_t *, const uint8_t *dk, const uint8_t *du, size_t m, uint8_t *d_o,
+                            uint8_t *d_c, cudaStream_t st) {
                             launch_x25519(dk, du, m, d_o, c_sz ? d_c : nullptr, st);
+                            return 0;
                         });
     if (rc) return rc;
     return wipe_staging(ctx, n * 64, n * (32 + c_sz));
@@ -161,10 +163,12 @@ int dalek_b200_x25519_public_keys(dalek_b200_ctx *ctx, const uint8_t *scalars, s
     if ((rc = x25519_table_ensure(ctx))) return rc;
     const double *table = (const double *)ctx->x25519_table.p;
     const size_t smem = X25519_COMB_DOUBLES * sizeof(double);
-    rc = run_pieces(ctx, scalars, 32, nullptr, 0, out, 32, nullptr, 0, n,
-                    [&](const uint8_t *dk, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *, cudaStream_t st) {
+    rc = run_pieces(ctx, nullptr, nullptr, scalars, 32, nullptr, 0, out, 32, nullptr, 0, n,
+                    [&](const uint8_t *, const uint64_t *, const uint8_t *dk, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *,
+                        cudaStream_t st) {
                         k_x25519_base<<<cdiv(m, X25519_COMB_THREADS), X25519_COMB_THREADS, smem, st>>>((const uint32_t *)dk, table, m,
                                                                                                     (uint32_t *)d_o);
+                        return 0;
                     });
     if (rc) return rc;
     return wipe_staging(ctx, n * 32, n * 32);

@@ -243,10 +243,12 @@ int dalek_b200_x25519_public_keys(dalek_b200_ctx *ctx, const uint8_t *scalars, s
 
 /* -------- hash to group ------------------------------------------------------------------------
  * Host buffers; each call blocks and streams the batch in pieces like the codecs.  The maps are total: these calls never
- * return DALEK_NONE.  n = 0 is a successful no-op; a NULL buffer with n > 0 is DALEK_E_INVALID_ARG.  Messages are laid out
- * back to back as in ed25519_b200_verify_each_flat: message i = msgs_flat[msg_offsets[i] .. msg_offsets[i+1]) (n + 1
- * offsets), msg_offsets[0] must be 0 and the offsets must not decrease, else DALEK_E_INVALID_ARG.  Constant time in the
- * message bytes (only the lengths of the messages and of the DST shape the work).  No option affects these calls.
+ * return DALEK_NONE.  n = 0 is a successful no-op; with n > 0 a NULL buffer other than msgs_flat is DALEK_E_INVALID_ARG.
+ * Flat messages, the layout of every host-buffer call that takes msgs_flat and msg_offsets: message i =
+ * msgs_flat[msg_offsets[i] .. msg_offsets[i+1]) (n + 1 offsets).  For n > 0, msg_offsets must not be NULL,
+ * msg_offsets[0] must be 0, the offsets must not decrease, and msgs_flat may be NULL only when every message is empty
+ * (msg_offsets[n] = 0); otherwise the call returns DALEK_E_INVALID_ARG.  Constant time in the message bytes (only the
+ * lengths of the messages and of the DST shape the work).  No option affects these calls.
  *
  * RistrettoPoint::from_uniform_bytes (C/ristretto.rs:774-790): in n x 64 B -> out n x 32 B CompressedRistretto */
 int dalek_b200_ristretto_from_uniform_bytes_batch(dalek_b200_ctx *ctx, const uint8_t *in, size_t n, uint8_t *out);
@@ -312,7 +314,8 @@ int dalek_b200_ristretto_vartime_msm(dalek_b200_ctx *ctx, const uint8_t *scalars
 int ed25519_b200_verify_batch(dalek_b200_ctx *ctx, const uint8_t *const *msgs, const size_t *msg_lens,
                               const uint8_t *sigs, const uint8_t *pubkeys, size_t n);
 /* Same with the messages laid out back to back: message i = msgs_flat[msg_offsets[i] ..
- * msg_offsets[i+1]) (n+1 offsets).  Avoids the host-side gather of the pointer form. */
+ * msg_offsets[i+1]) (n+1 offsets; the flat-message rule of the hash-to-group block applies to every host-buffer
+ * ..._flat call).  Avoids the host-side gather of the pointer form. */
 int ed25519_b200_verify_batch_flat(dalek_b200_ctx *ctx, const uint8_t *msgs_flat,
                                    const uint64_t *msg_offsets, const uint8_t *sigs,
                                    const uint8_t *pubkeys, size_t n);
@@ -364,7 +367,8 @@ int ed25519_b200_verify_batches_flat_points_dev(dalek_b200_ctx *ctx, const void 
  * When the batch holds few distinct keys (every key signing at least eight signatures on average; option "each_comb") the
  * 64 x 8 multiples (j+1) 16^i A of every distinct key are tabulated once per call and each signature costs 128 mixed
  * additions and no doubling; otherwise every signature pays its own 252 doublings.  Same results either way.
- * Returns 0 if every result is 0, 1 otherwise; negative on engine errors.  results: n bytes (host). */
+ * Returns 0 if every result is 0, 1 otherwise; negative on engine errors.  results: n bytes (host).  Flat messages as in
+ * the hash-to-group block. */
 int ed25519_b200_verify_each_flat(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets,
                                   const uint8_t *sigs, const uint8_t *pubkeys, size_t n, int strict,
                                   uint8_t *results);
@@ -379,7 +383,7 @@ int ed25519_b200_last_zs(dalek_b200_ctx *ctx, uint8_t *zs_out, size_t n);
 int dalek_b200_edwards_mul_base_batch(dalek_b200_ctx *ctx, const uint8_t *scalars, size_t n,
                                       uint64_t *out_limbs /* n x 20 */, uint8_t *out_compressed /* n x 32, nullable */);
 /* Deterministic Ed25519 keygen + sign on the GPU: seeds n x 32 B -> pubkeys n x 32 B, sigs n x 64 B
- * (E/signing.rs, hazmat.rs:40-99); message layout as in verify_batch_flat. */
+ * (E/signing.rs, hazmat.rs:40-99); message layout and checks as in verify_batch_flat. */
 int ed25519_b200_sign_batch_flat(dalek_b200_ctx *ctx, const uint8_t *seeds, const uint8_t *msgs_flat,
                                  const uint64_t *msg_offsets, size_t n, uint8_t *pubkeys_out,
                                  uint8_t *sigs_out);
