@@ -12,13 +12,17 @@ touches the CPU checker used by the tests.  Names follow the reference:
   EdwardsPoint.to_montgomery_batch (src/edwards.rs:592-612)
   RistrettoPoint.from_uniform_bytes_batch / hash_from_bytes_batch (src/ristretto.rs:736-790)
   EdwardsPoint.hash_to_curve_batch / encode_to_curve_batch (src/edwards.rs:710-750, RFC 9380)
+  ed25519_verifying_keys / ed25519_sign / ed25519_sign_prehashed / ed25519_verify_prehashed
+      (ed25519-dalek/src/signing.rs:106-171, :312, :566-571; src/verifying.rs:230-257, :424-459)
 """
 from .engine import (Engine, MultiEngine, EngineError, EdwardsPoint, RistrettoPoint, SignatureError, verify_batch, default_engine,
                      library_path, load_library, POINTS_COMPRESSED, POINTS_EXTENDED, POINTS_RISTRETTO,
                      VartimeEdwardsPrecomputation, VartimeRistrettoPrecomputation, x25519, x25519_public_keys,
-                     X25519_BASEPOINT_BYTES)
+                     X25519_BASEPOINT_BYTES, ed25519_verifying_keys, ed25519_sign, ed25519_sign_prehashed,
+                     ed25519_verify_prehashed)
 
 __all__ = ["Engine", "MultiEngine", "EngineError", "EdwardsPoint", "RistrettoPoint", "SignatureError", "verify_batch", "default_engine",
            "library_path", "load_library", "POINTS_COMPRESSED", "POINTS_EXTENDED", "POINTS_RISTRETTO",
            "VartimeEdwardsPrecomputation", "VartimeRistrettoPrecomputation", "x25519", "x25519_public_keys",
-           "X25519_BASEPOINT_BYTES"]
+           "X25519_BASEPOINT_BYTES", "ed25519_verifying_keys", "ed25519_sign", "ed25519_sign_prehashed",
+           "ed25519_verify_prehashed"]

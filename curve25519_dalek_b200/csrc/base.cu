@@ -1,9 +1,6 @@
-// base.cu -- fixed-base multiples of the Ed25519 basepoint and RFC 8032 signing on the GPU.
-// These exist to synthesise benchmark / test inputs on the device (2^20..2^24 points, 2^22
-// signatures would take minutes on the host): EdwardsPoint::mul_base
-// (curve25519-dalek/src/edwards.rs:918-928) and the signing half of ed25519-dalek
-// (src/signing.rs, src/hazmat.rs:40-99).  Variable-time table indexing: do not use with
-// production secrets.
+// base.cu -- fixed-base multiples of the Ed25519 basepoint for PUBLIC scalars: EdwardsPoint::mul_base
+// (curve25519-dalek/src/edwards.rs:918-928), e.g. to synthesise benchmark / test points on the device, and the table of B
+// that the verifiers read.  Variable-time table indexing: secrets go through the comb of comb.cuh (sign.cu, x25519.cu).
 //
 // Table: T[i][j] = (j+1) * 16^i * B as packed affine Niels points, i < 64, j < 8 (48 KiB), so that
 // s*B = sum_i digit_i * 16^i * B needs 64 mixed additions and no doublings.
@@ -12,7 +9,6 @@
 
 #include "../../include/dalek_b200.h"
 #include "engine.h"
-#include "hash.cuh"
 #include "sc.cuh"
 
 static inline unsigned cdiv(size_t a, unsigned b) { return (unsigned)((a + b - 1) / b); }
@@ -82,40 +78,6 @@ k_mul_base(const uint32_t *__restrict__ scalars, size_t n, const ge_niels_packed
     }
 }
 
-// RFC 8032 5.1.5 / 5.1.6 (ed25519-dalek src/hazmat.rs:40-99, src/signing.rs): one thread per message
-__global__ void __launch_bounds__(128)
-k_sign(const uint32_t *__restrict__ seeds, const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ offs, size_t n,
-       const ge_niels_packed *__restrict__ table, uint32_t *__restrict__ pks, uint32_t *__restrict__ sigs)
-{
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    uint32_t seed[8], hd[16], a[8], prefix[8];
-#pragma unroll
-    for (int k = 0; k < 8; k++) seed[k] = seeds[8 * i + k];
-    sha512_state st;
-    sha512_init(st); sha512_update_words(st, seed); sha512_final_words(st, hd);
-#pragma unroll
-    for (int k = 0; k < 8; k++) { a[k] = hd[k]; prefix[k] = hd[8 + k]; }
-    a[0] &= 0xfffffff8u; a[7] &= 0x3fffffffu; a[7] |= 0x40000000u;          // clamp
-    ge_p3 P;
-    mul_base(P, a, table);
-    uint32_t A[8]; ge_compress(A, P);
-    const uint8_t *m = msgs + offs[i];
-    size_t len = (size_t)(offs[i + 1] - offs[i]);
-    sha512_init(st); sha512_update_words(st, prefix); sha512_update(st, m, len); sha512_final_words(st, hd);
-    uint32_t r[8]; sc_reduce512(r, hd);
-    mul_base(P, r, table);
-    uint32_t R[8]; ge_compress(R, P);
-    sha512_init(st); sha512_update_words(st, R); sha512_update_words(st, A); sha512_update(st, m, len); sha512_final_words(st, hd);
-    uint32_t k_[8], ka[8], ar[8], S[8];
-    sc_reduce512(k_, hd);
-    sc_reduce256(ar, a);
-    sc_mul(ka, k_, ar);
-    sc_add(S, ka, r);
-#pragma unroll
-    for (int k = 0; k < 8; k++) { pks[8 * i + k] = A[k]; sigs[16 * i + k] = R[k]; sigs[16 * i + 8 + k] = S[k]; }
-}
-
 int base_table_ensure(dalek_b200_ctx *ctx)
 {
     if (ctx->base_table_ready) return 0;
@@ -149,33 +111,6 @@ int dalek_b200_edwards_mul_base_batch(dalek_b200_ctx *ctx, const uint8_t *scalar
     ctx->launches++;
     if (out_limbs) CUDA_TRY(ctx, cudaMemcpyAsync(out_limbs, ctx->points_in.p, n * 160, cudaMemcpyDeviceToHost, st));
     if (out_compressed) CUDA_TRY(ctx, cudaMemcpyAsync(out_compressed, ctx->misc1.p, n * 32, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(ctx, cudaStreamSynchronize(st));
-    return 0;
-}
-
-int ed25519_b200_sign_batch_flat(dalek_b200_ctx *ctx, const uint8_t *seeds, const uint8_t *msgs_flat,
-                                 const uint64_t *msg_offsets, size_t n, uint8_t *pubkeys_out, uint8_t *sigs_out)
-{
-    if (!ctx || (n && (!seeds || !pubkeys_out || !sigs_out)) || !flat_messages_ok(msgs_flat, msg_offsets, n)) return DALEK_E_INVALID_ARG;
-    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    int rc;
-    cudaStream_t st = ctx->stream;
-    if ((rc = base_table_ensure(ctx))) return rc;
-    if (!n) return 0;
-    size_t mbytes = (size_t)msg_offsets[n];
-    if ((rc = ws_reserve(ctx, ctx->scalars, n * 32))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->misc1, mbytes + 16))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->misc2, (n + 1) * 8))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points_in, n * 96))) return rc;
-    uint32_t *d_pk = (uint32_t *)ctx->points_in.p, *d_sig = d_pk + n * 8;
-    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->scalars.p, seeds, n * 32, cudaMemcpyHostToDevice, st));
-    if (mbytes) CUDA_TRY(ctx, cudaMemcpyAsync(ctx->misc1.p, msgs_flat, mbytes, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->misc2.p, msg_offsets, (n + 1) * 8, cudaMemcpyHostToDevice, st));
-    k_sign<<<cdiv(n, 128), 128, 0, st>>>((const uint32_t *)ctx->scalars.p, (const uint8_t *)ctx->misc1.p,
-                                         (const uint64_t *)ctx->misc2.p, n, (const ge_niels_packed *)ctx->base_table.p, d_pk, d_sig);
-    ctx->launches++;
-    CUDA_TRY(ctx, cudaMemcpyAsync(pubkeys_out, d_pk, n * 32, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(ctx, cudaMemcpyAsync(sigs_out, d_sig, n * 64, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(ctx, cudaStreamSynchronize(st));
     return 0;
 }

@@ -53,6 +53,28 @@ k_hram(const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ offs, cons
     if (!sc_is_canonical(s)) { atomicOr(&flags[FLAG_BAD_S], 1); bad_s[i] = 1; }
 }
 
+// k_hram for Ed25519ph (verifying.rs:530-535): SHA-512(dom2(1, C) || R || A || PH) with PH the fixed 64-byte prehash
+__global__ void __launch_bounds__(128)
+k_hram_ph(const uint8_t *__restrict__ phs, const __grid_constant__ Sha512Prefix dom, const uint32_t *__restrict__ sigs,
+          const uint32_t *__restrict__ keys, size_t n, uint32_t *__restrict__ hrams, uint32_t *__restrict__ hs,
+          int *__restrict__ flags, uint8_t *__restrict__ bad_s)
+{
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t R[8], A[8], s[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) { R[k] = sigs[16 * i + k]; s[k] = sigs[16 * i + 8 + k]; A[k] = keys[8 * i + k]; }
+    uint32_t dig[16];
+    sha512_pxm<2, 1>(dig, dom.b, dom.len, R, A, phs + 64 * i, 64);
+#pragma unroll
+    for (int k = 0; k < 16; k++) hrams[16 * i + k] = dig[k];
+    uint32_t h[8];
+    sc_reduce512(h, dig);
+#pragma unroll
+    for (int k = 0; k < 8; k++) hs[8 * i + k] = h[k];
+    if (!sc_is_canonical(s)) { atomicOr(&flags[FLAG_BAD_S], 1); bad_s[i] = 1; }
+}
+
 __global__ void __launch_bounds__(64)
 k_transcript(const uint32_t *__restrict__ hrams, const uint32_t *__restrict__ sigs, size_t n, uint32_t chunk,
              uint32_t *__restrict__ zs)
@@ -918,11 +940,11 @@ static int verify_batches_tail(dalek_b200_ctx *ctx, const VerifyBufs &b, size_t 
     return any ? ED25519_ERR_VERIFY : DALEK_OK;
 }
 
-// Front end shared with the per-signature verifier (single.cu): SHA-512(R || A || M) mod l and the canonical-s marks of
-// every signature, public keys de-duplicated (rep / dense / uniq as in verify_batch).  Synchronises to return the number
+// Front end shared with the per-signature verifier (single.cu): SHA-512(R || A || M) mod l (with ph_dom: SHA-512(dom2 ||
+// R || A || PH), d_msgs then holding n 64-byte prehashes and d_offs unused) and the canonical-s marks of every signature, public keys de-duplicated (rep / dense / uniq as in verify_batch).  Synchronises to return the number
 // of distinct keys.  All arrays live in the context's workspaces until the next verify call.
 int verify_each_front(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const uint64_t *d_offs, const uint32_t *d_sigs, const uint32_t *d_keys,
-                      size_t n, EachFront *out)
+                      size_t n, EachFront *out, const Sha512Prefix *ph_dom)
 {
     int rc;
     VerifyBufs b;
@@ -933,7 +955,8 @@ int verify_each_front(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const uint64_t
         CUDA_TRY(ctx, cudaMemsetAsync(b.table, 0xff, ((size_t)b.tmask + 1) * 4, st));
         CUDA_TRY(ctx, cudaMemsetAsync(b.counters, 0, 64, st));
     }
-    k_hram<<<cdiv(n, 128), 128, 0, st>>>(d_msgs, d_offs, d_sigs, d_keys, n, b.hrams, b.hs, b.flags, b.bad_s);
+    if (ph_dom) k_hram_ph<<<cdiv(n, 128), 128, 0, st>>>(d_msgs, *ph_dom, d_sigs, d_keys, n, b.hrams, b.hs, b.flags, b.bad_s);
+    else k_hram<<<cdiv(n, 128), 128, 0, st>>>(d_msgs, d_offs, d_sigs, d_keys, n, b.hrams, b.hs, b.flags, b.bad_s);
     k_key_dedupe<<<cdiv(n, 256), 256, 0, st>>>(d_keys, 0, n, b.table, b.tmask, b.rep, b.uniq, b.dense, b.counters,
                                                make_uint4(ctx->hash_seed[0], ctx->hash_seed[1], ctx->hash_seed[2], ctx->hash_seed[3]));
     ctx->launches += 2;

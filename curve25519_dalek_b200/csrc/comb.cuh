@@ -1,5 +1,5 @@
-// comb.cuh -- the pieces of a constant-time fixed-base comb shared by the Ristretto double-base batch (straus.cu)
-// and the X25519 public keys (x25519.cu).
+// comb.cuh -- the pieces of a constant-time fixed-base comb shared by the Ristretto double-base batch (straus.cu),
+// the X25519 public keys (x25519.cu) and the Ed25519 signer (sign.cu).
 //
 // A base P is tabulated as 64 rows of 8 entries, entry j of row i = (j+1) 16^i P as balanced FP64 affine Niels
 // (15 doubles: y+x | y-x | 2dxy).  s P is then the sum over the 64 radix-16 signed digits d_i of s
@@ -48,4 +48,37 @@ __device__ __forceinline__ void comb_select(ge64_niels &q, const double *__restr
     for (int k = 0; k < 5; k++) {
         q.ypx.v[k] = __longlong_as_double(w[k]); q.ymx.v[k] = __longlong_as_double(w[5 + k]); q.xy2d.v[k] = __longlong_as_double(w[10 + k]);
     }
+}
+
+// acc = s B from the table of B in shared memory (64 rows of 8 entries, COMB_ENTRY doubles each), for a secret s < 2^255
+// (clamped scalars, reduced scalars): radix-16 signed digits (scalar.rs:1019-1051; s < 2^255 keeps the last digit in range),
+// every row scanned in full and the sign applied by the masked negate of ge64_madd, so no branch or address depends on s.
+// nibble(pos) returns bits 4 pos .. 4 pos + 3 of s, for pos = 0..63 in order.
+template <class Nibble>
+__device__ __forceinline__ void comb_mul_base_nibbles(ge64_p3 &acc, const double *__restrict__ s_tab, Nibble nibble)
+{
+    ge64_identity(acc);
+    int carry = 0;
+#pragma unroll 1
+    for (int pos = 0; pos < 64; pos++) {
+        int d = (int)nibble(pos) + carry;
+        if (pos < 63) { carry = (d + 8) >> 4; d -= carry << 4; }
+        const int m = d >> 31;
+        ge64_niels q;
+        comb_select(q, s_tab + (size_t)pos * 8 * COMB_ENTRY, (uint32_t)((d + m) ^ m));
+        ge64_madd(acc, acc, q, (uint32_t)(d < 0));
+    }
+}
+
+// the same for s held in registers (consumed: shifted down by one digit per row with funnel shifts, so that no register
+// array is indexed at run time)
+__device__ __forceinline__ void comb_mul_base(ge64_p3 &acc, uint32_t s[8], const double *__restrict__ s_tab)
+{
+    comb_mul_base_nibbles(acc, s_tab, [&](int) {
+        const uint32_t v = s[0] & 15;
+#pragma unroll
+        for (int k = 0; k < 7; k++) s[k] = __funnelshift_r(s[k], s[k + 1], 4);
+        s[7] >>= 4;
+        return v;
+    });
 }

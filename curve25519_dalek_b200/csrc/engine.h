@@ -64,8 +64,8 @@ struct dalek_b200_ctx {
     bool base_table_ready = false;
     bool each_attr_set = false;     // the same for k_verify_each_comb
     bool comb_attr_set = false;     // cudaFuncAttributeMaxDynamicSharedMemorySize set for the comb kernel on this device
-    DevBuf x25519_table;            // comb table of the Ed25519 basepoint for X25519 public keys (x25519.cu), built once
-    bool x25519_table_ready = false;
+    DevBuf comb_base_table;         // comb table of the Ed25519 basepoint (comb.cuh) for X25519 public keys and signing, built once
+    bool comb_base_table_ready = false;
     // pinned host staging
     void *h_pinned = nullptr;
     size_t h_pinned_cap = 0;
@@ -194,8 +194,9 @@ int msm_combine_records(dalek_b200_ctx *ctx, const void *records, bool on_device
 
 // ---- front end of verify_batch reused by the per-signature verifier (batch.cu -> single.cu) ----
 struct EachFront { const uint32_t *hs; const uint8_t *bad_s; const uint32_t *rep, *dense, *uniq; size_t nkeys; };
+struct Sha512Prefix;   // hash.cuh: the dom2 prefix of Ed25519ph
 int verify_each_front(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const uint64_t *d_offs, const uint32_t *d_sigs, const uint32_t *d_keys,
-                      size_t n, EachFront *out);
+                      size_t n, EachFront *out, const Sha512Prefix *ph_dom = nullptr);
 
 // ---- variable-time Straus for small inputs (straus_vt.cu): the reference's path below 190 points ----
 #define STRAUS_VT_THRESHOLD 190            // edwards.rs:1025-1029
@@ -207,6 +208,10 @@ int straus_ct_msm(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const void *d_
                   MsmResult *d_result);
 // ---- fixed-base table (base.cu): 64 x 8 affine Niels entries (j+1) 16^i B, built once per context ----
 int base_table_ensure(dalek_b200_ctx *ctx);
+// ---- constant-time comb table of B (x25519.cu): 64 x 8 x COMB_ENTRY balanced FP64 doubles (comb.cuh), built once per
+// context and shared by the X25519 public keys and the Ed25519 signer (sign.cu) ----
+#define COMB_BASE_DOUBLES (64 * 8 * 15)
+int comb_base_table_ensure(dalek_b200_ctx *ctx);
 
 int ristretto_prepare_points(dalek_b200_ctx *ctx, const void *d_in, size_t n, void *d_out, int *d_bad);
 int ristretto_encode_result(dalek_b200_ctx *ctx, const MsmResult *d_res, uint32_t *d_enc);

@@ -116,9 +116,7 @@ __device__ __forceinline__ void sha512_final_words(sha512_state &s, uint32_t out
     }
 }
 
-// SHA-512(R || A || M) with the blocks assembled in registers (static word indices, no staging buffer in local
-// memory): the hash of batch.rs:179-191 / verifying.rs:515-523, one call per signature.  R, A: eight little-endian
-// words each (their bytes in order); M: `len` bytes at `msg` (any alignment).  dig: 16 LE words.
+// One SHA-512 compression with the block in registers (static word indices, no staging buffer in local memory).
 __device__ __forceinline__ void sha512_compress_regs(uint64_t h[8], uint64_t w[16])
 {
     uint64_t a = h[0], b = h[1], c = h[2], d = h[3], e = h[4], f = h[5], g = h[6], hh = h[7];
@@ -144,43 +142,126 @@ __device__ __forceinline__ void sha512_compress_regs(uint64_t h[8], uint64_t w[1
     h[0] += a; h[1] += b; h[2] += c; h[3] += d; h[4] += e; h[5] += f; h[6] += g; h[7] += hh;
 }
 
-__device__ __forceinline__ void sha512_ram(uint32_t dig[16], const uint32_t R[8], const uint32_t A[8], const uint8_t *__restrict__ msg,
-                                           size_t len)
+// A public prefix hashed before the register strings: Ed25519ph's dom2(1, C) = "SigEd25519 no Ed25519 collisions" || 1 ||
+// |C| || C (RFC 8032 5.1; ed25519-dalek signing.rs:945-951, verifying.rs:530-535), at most 34 + 255 bytes.  Travels as a
+// __grid_constant__ kernel parameter, like the DST of hash_to_curve.cu.
+#define SHA512_PREFIX_MAX 289
+struct Sha512Prefix {
+    uint8_t b[SHA512_PREFIX_MAX + 7];
+    uint32_t len;
+};
+
+// dom2(1, context) for a context of at most 255 bytes (the caller checks the length)
+static inline void ed25519ph_dom2(Sha512Prefix &d, const uint8_t *context, size_t context_len)
+{
+    const char *tag = "SigEd25519 no Ed25519 collisions";
+    d = Sha512Prefix{};
+    for (int j = 0; j < 32; j++) d.b[j] = (uint8_t)tag[j];
+    d.b[32] = 1;                                                  // phflag
+    d.b[33] = (uint8_t)context_len;
+    for (size_t j = 0; j < context_len; j++) d.b[34 + j] = context[j];
+    d.len = (uint32_t)(34 + context_len);
+}
+
+// SHA-512(P || X || M) with the blocks assembled in registers: P the public prefix (PRE = 1: `plen` bytes at `pre`;
+// PRE = 0: none), X = NX register strings of 32 bytes (X0, then X1 when NX = 2; eight little-endian words each, their
+// bytes in order), M = `len` bytes at `msg` (any alignment).  dig: 16 LE words.  Where each byte comes from depends on
+// the lengths only, so X may be secret (the signer's nonce prefix).  With PRE = 0, X starts the first block at a fixed
+// word index; with a prefix, X is shifted by plen mod 8 bytes once and each word of the first blocks takes its X part
+// by a masked select over the shifted words (no register array is indexed at run time).
+template <int NX, int PRE>
+__device__ __forceinline__ void sha512_pxm(uint32_t dig[16], const uint8_t *pre, uint32_t plen, const uint32_t X0[8],
+                                           const uint32_t X1[8], const uint8_t *__restrict__ msg, size_t len)
 {
     uint64_t h[8] = {0x6a09e667f3bcc908ULL, 0xbb67ae8584caa73bULL, 0x3c6ef372fe94f82bULL, 0xa54ff53a5f1d36f1ULL,
                      0x510e527fade682d1ULL, 0x9b05688c2b3e6c1fULL, 0x1f83d9abfb41bd6bULL, 0x5be0cd19137e2179ULL};
-    const size_t total = 64 + len;                               // message bytes of the hash input
-    const size_t nblocks = (total + 1 + 16 + 127) / 128;
     // big-endian 64-bit word from two LE 32-bit words holding 8 consecutive bytes
 #define SHA_BE64(lo, hi) (((uint64_t)__byte_perm((lo), 0, 0x0123) << 32) | (uint64_t)__byte_perm((hi), 0, 0x0123))
+    if (!PRE) {
+        const size_t total = 32 * NX + len;                      // message bytes of the hash input
+        const size_t nblocks = (total + 1 + 16 + 127) / 128;
 #pragma unroll 1
-    for (size_t blk = 0; blk < nblocks; blk++) {
-        uint64_t w[16];
-        const size_t base = blk * 128;
+        for (size_t blk = 0; blk < nblocks; blk++) {
+            uint64_t w[16];
+            const size_t base = blk * 128;
 #pragma unroll
-        for (int j = 0; j < 16; j++) {
-            const size_t off = base + 8 * j;                     // first input byte of this word
-            uint64_t v;
-            if (blk == 0 && j < 4) v = SHA_BE64(R[2 * j], R[2 * j + 1]);
-            else if (blk == 0 && j < 8) v = SHA_BE64(A[2 * (j - 4)], A[2 * (j - 4) + 1]);
-            else {
-                v = 0;
-                if (off + 8 <= total) {                          // eight message bytes
+            for (int j = 0; j < 16; j++) {
+                const size_t off = base + 8 * j;                 // first input byte of this word
+                uint64_t v;
+                if (blk == 0 && j < 4) v = SHA_BE64(X0[2 * j], X0[2 * j + 1]);
+                else if (NX == 2 && blk == 0 && j < 8) v = SHA_BE64(X1[2 * (j - 4)], X1[2 * (j - 4) + 1]);
+                else {
+                    v = 0;
+                    if (off + 8 <= total) {                      // eight message bytes
 #pragma unroll
-                    for (int b = 0; b < 8; b++) v = (v << 8) | (uint64_t)msg[off - 64 + b];
-                } else if (off <= total) {                       // tail of the message, then the 0x80 marker
+                        for (int b = 0; b < 8; b++) v = (v << 8) | (uint64_t)msg[off - 32 * NX + b];
+                    } else if (off <= total) {                   // tail of the message, then the 0x80 marker
+#pragma unroll
+                        for (int b = 0; b < 8; b++) {
+                            const size_t q = off + b;
+                            const uint64_t byte = q < total ? (uint64_t)msg[q - 32 * NX] : (q == total ? 0x80u : 0u);
+                            v = (v << 8) | byte;
+                        }
+                    }
+                }
+                w[j] = v;
+            }
+            if (blk == nblocks - 1) w[15] = (uint64_t)total * 8; // bit length (w[14] stays 0: inputs < 2^61 bytes)
+            sha512_compress_regs(h, w);
+        }
+    } else {
+        const size_t mstart = plen + 32 * NX, total = mstart + len;
+        const size_t nblocks = (total + 1 + 16 + 127) / 128;
+        const uint32_t sh = 8 * (plen & 7), w0 = plen >> 3;      // X starts sh bits into word w0 of the input
+        uint64_t XS[4 * NX + 1];                                 // X shifted right by sh bits, as input words w0..w0+4NX
+        {
+            uint64_t XW[4 * NX];
+#pragma unroll
+            for (int k = 0; k < 4; k++) XW[k] = SHA_BE64(X0[2 * k], X0[2 * k + 1]);
+#pragma unroll
+            for (int k = 4; k < 4 * NX; k++) XW[k] = SHA_BE64(X1[2 * (k - 4)], X1[2 * (k - 4) + 1]);
+#pragma unroll
+            for (int k = 0; k <= 4 * NX; k++) {
+                const uint64_t hi = k < 4 * NX ? XW[k] >> sh : 0;
+                const uint64_t lo = k ? (XW[k - 1] << (56 - sh)) << 8 : 0;   // << (64 - sh), 0 when sh = 0
+                XS[k] = hi | lo;
+            }
+        }
+#pragma unroll 1
+        for (size_t blk = 0; blk < nblocks; blk++) {
+            uint64_t w[16];
+            const size_t base = blk * 128;
+#pragma unroll
+            for (int j = 0; j < 16; j++) {
+                const size_t off = base + 8 * j, g = off >> 3;
+                uint64_t v = 0;
+                if (off + 8 <= plen) {                           // eight prefix bytes
+#pragma unroll
+                    for (int b = 0; b < 8; b++) v = (v << 8) | (uint64_t)pre[off + b];
+                } else if (off >= mstart && off + 8 <= total) {  // eight message bytes
+#pragma unroll
+                    for (int b = 0; b < 8; b++) v = (v << 8) | (uint64_t)msg[off - mstart + b];
+                } else if (off < total + 1) {                    // prefix / X / message / 0x80 boundaries
+                    uint64_t xm = 0;                             // byte mask of X in this word
 #pragma unroll
                     for (int b = 0; b < 8; b++) {
                         const size_t q = off + b;
-                        const uint64_t byte = q < total ? (uint64_t)msg[q - 64] : (q == total ? 0x80u : 0u);
+                        const uint64_t byte = q < plen ? (uint64_t)pre[q]
+                                              : q < mstart ? 0u
+                                              : q < total ? (uint64_t)msg[q - mstart] : (q == total ? 0x80u : 0u);
                         v = (v << 8) | byte;
+                        xm = (xm << 8) | (q >= plen && q < mstart ? 0xffu : 0u);
                     }
+                    uint64_t xv = 0;
+#pragma unroll
+                    for (int k = 0; k <= 4 * NX; k++) xv |= XS[k] & (0ULL - (uint64_t)(g == w0 + (size_t)k));
+                    v |= xv & xm;
                 }
+                w[j] = v;
             }
-            w[j] = v;
+            if (blk == nblocks - 1) w[15] = (uint64_t)total * 8;
+            sha512_compress_regs(h, w);
         }
-        if (blk == nblocks - 1) w[15] = (uint64_t)total * 8;     // bit length (w[14] stays 0: inputs < 2^61 bytes)
-        sha512_compress_regs(h, w);
     }
 #undef SHA_BE64
 #pragma unroll
@@ -188,6 +269,13 @@ __device__ __forceinline__ void sha512_ram(uint32_t dig[16], const uint32_t R[8]
         dig[2 * i] = __byte_perm((uint32_t)(h[i] >> 32), 0, 0x0123);
         dig[2 * i + 1] = __byte_perm((uint32_t)h[i], 0, 0x0123);
     }
+}
+
+// SHA-512(R || A || M): the hash of batch.rs:179-191 / verifying.rs:515-523, one call per signature.
+__device__ __forceinline__ void sha512_ram(uint32_t dig[16], const uint32_t R[8], const uint32_t A[8], const uint8_t *__restrict__ msg,
+                                           size_t len)
+{
+    sha512_pxm<2, 0>(dig, nullptr, 0, R, A, msg, len);
 }
 
 // ---------------------------------------------------------------- Keccak-f[1600]

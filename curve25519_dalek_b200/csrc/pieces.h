@@ -3,6 +3,7 @@
 // of its neighbours.  Used by the codecs, X25519, hash-to-group, the plain path of verify_each and the double-base batch.
 #pragma once
 #include <algorithm>
+#include <type_traits>
 
 #include "engine.h"
 
@@ -12,7 +13,8 @@
 // ctx->msg_offs, the fixed-width inputs in ctx->points_in (first all of `in`, then all of `in2`), the outputs in
 // ctx->points.  launch(d_msgs, d_offs, d_in, d_in2, m, d_out, d_out2, stream) enqueues the kernel of one piece of m items
 // and returns an engine code; d_offs points at the piece's m + 1 offsets, which stay absolute (d_msgs is the base of the
-// whole staged buffer).  Pieces hold `piece` items (0: 2^16 from 2^17 items up, else one piece).  Sets last_kernel_ms
+// whole staged buffer).  A callback that takes one more size_t argument also receives lo, the index of the piece's first
+// item in the batch (for per-item data the kernel reads from elsewhere, such as the signer's expanded keys).  Pieces hold `piece` items (0: 2^16 from 2^17 items up, else one piece).  Sets last_kernel_ms
 // to the device span of the whole batch, copies included, and last_kernel_launches to the number of pieces.
 template <typename Launch>
 static int run_pieces(dalek_b200_ctx *ctx, const uint8_t *msgs, const uint64_t *offs, const uint8_t *in, size_t in_sz,
@@ -45,8 +47,12 @@ static int run_pieces(dalek_b200_ctx *ctx, const uint8_t *msgs, const uint64_t *
         }
         if (in_sz) CUDA_TRY(ctx, cudaMemcpyAsync(d_in + lo * in_sz, in + lo * in_sz, m * in_sz, cudaMemcpyHostToDevice, st));
         if (in2_sz) CUDA_TRY(ctx, cudaMemcpyAsync(d_in2 + lo * in2_sz, in2 + lo * in2_sz, m * in2_sz, cudaMemcpyHostToDevice, st));
-        if ((rc = launch(d_msgs, d_offs + lo, d_in + lo * in_sz, d_in2 + lo * in2_sz, m, d_out + lo * out_sz, d_out2 + lo * out2_sz, st)))
-            return rc;
+        if constexpr (std::is_invocable_v<Launch &, const uint8_t *, const uint64_t *, const uint8_t *, const uint8_t *, size_t,
+                                          uint8_t *, uint8_t *, cudaStream_t, size_t>)
+            rc = launch(d_msgs, d_offs + lo, d_in + lo * in_sz, d_in2 + lo * in2_sz, m, d_out + lo * out_sz, d_out2 + lo * out2_sz, st, lo);
+        else
+            rc = launch(d_msgs, d_offs + lo, d_in + lo * in_sz, d_in2 + lo * in2_sz, m, d_out + lo * out_sz, d_out2 + lo * out2_sz, st);
+        if (rc) return rc;
         ctx->launches++;
         CUDA_TRY(ctx, cudaGetLastError());
         CUDA_TRY(ctx, cudaMemcpyAsync(out + lo * out_sz, d_out + lo * out_sz, m * out_sz, cudaMemcpyDeviceToHost, st));

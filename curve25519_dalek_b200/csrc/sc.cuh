@@ -1,5 +1,9 @@
 // sc.cuh -- arithmetic modulo the group order l = 2^252 + 27742317777372353535851937790883648493
-// on 32-bit words (device).  Values cross this header as 8 little-endian 32-bit words.
+// on 32-bit words.  Values cross this header as 8 little-endian 32-bit words.  Device code under nvcc; a plain C++
+// compiler builds it for the host (tests/host/sc_host_check.cpp), with SC_L / SC_MU as host constants.
+//
+// Branch-free in the values: every conditional subtraction of l is a masked select, so that the signer (sign.cu) can
+// reduce secrets (r, k a + r) here.  Loop counts are fixed.
 //
 // The reference uses five 52-bit limbs with Montgomery reduction, R = 2^260
 // (curve25519-dalek/src/backend/serial/u64/scalar.rs:60-343).  Only canonical values are
@@ -10,9 +14,15 @@
 
 #include "constants.cuh"   // SC_L[8], SC_MU[9]
 
+#if defined(__CUDACC__)
+#define SC_HD __device__ __forceinline__     // SC_L / SC_MU are __constant__ here
+#else
+#define SC_HD inline
+#endif
+
 // out[na+nb] = a[na] * b[nb]
 template <int NA, int NB>
-__device__ __forceinline__ void mp_mul(uint32_t *out, const uint32_t *a, const uint32_t *b)
+SC_HD void mp_mul(uint32_t *out, const uint32_t *a, const uint32_t *b)
 {
 #pragma unroll
     for (int i = 0; i < NA + NB; i++) out[i] = 0;
@@ -31,7 +41,7 @@ __device__ __forceinline__ void mp_mul(uint32_t *out, const uint32_t *a, const u
 
 // r = a - b over N words, returns borrow
 template <int N>
-__device__ __forceinline__ uint32_t mp_sub(uint32_t *r, const uint32_t *a, const uint32_t *b)
+SC_HD uint32_t mp_sub(uint32_t *r, const uint32_t *a, const uint32_t *b)
 {
     uint64_t borrow = 0;
 #pragma unroll
@@ -44,7 +54,7 @@ __device__ __forceinline__ uint32_t mp_sub(uint32_t *r, const uint32_t *a, const
 }
 
 // 1 if a >= l (a: 8 words)
-__device__ __forceinline__ uint32_t sc_ge_l(const uint32_t *a)
+SC_HD uint32_t sc_ge_l(const uint32_t *a)
 {
     uint32_t t[8], l[8];
 #pragma unroll
@@ -53,11 +63,11 @@ __device__ __forceinline__ uint32_t sc_ge_l(const uint32_t *a)
 }
 
 // Scalar::from_canonical_bytes test (C/scalar.rs:259-263): bit 255 clear and value < l
-__device__ __forceinline__ uint32_t sc_is_canonical(const uint32_t *a) { return 1u - sc_ge_l(a); }
+SC_HD uint32_t sc_is_canonical(const uint32_t *a) { return 1u - sc_ge_l(a); }
 
 // x (16 words, < 2^512) mod l -> r (8 words).  Scalar::from_bytes_mod_order_wide value
 // (C/scalar.rs:248-250, u64/scalar.rs:89-116).
-__device__ __forceinline__ void sc_reduce512(uint32_t *r, const uint32_t *x)
+SC_HD void sc_reduce512(uint32_t *r, const uint32_t *x)
 {
     uint32_t mu[9], l[9], q2[18], r2[18];
 #pragma unroll
@@ -71,20 +81,18 @@ __device__ __forceinline__ void sc_reduce512(uint32_t *r, const uint32_t *x)
     uint32_t t[9];
     mp_sub<9>(t, x, r2);                      // r1 - r2 mod b^9  (0 <= result < 3l)
 #pragma unroll 1
-    for (int it = 0; it < 2; it++) {
+    for (int it = 0; it < 2; it++) {                  // t -= l while t >= l, as a masked select
         uint32_t u[9];
-        uint32_t borrow = mp_sub<9>(u, t, l);
-        if (!borrow) {
+        const uint32_t keep = 0u - mp_sub<9>(u, t, l); // all ones: t < l, keep t
 #pragma unroll
-            for (int i = 0; i < 9; i++) t[i] = u[i];
-        }
+        for (int i = 0; i < 9; i++) t[i] = (t[i] & keep) | (u[i] & ~keep);
     }
 #pragma unroll
     for (int i = 0; i < 8; i++) r[i] = t[i];
 }
 
 // r = a mod l for a 256-bit a (Scalar::from_bytes_mod_order, C/scalar.rs:235-244)
-__device__ __forceinline__ void sc_reduce256(uint32_t *r, const uint32_t *a)
+SC_HD void sc_reduce256(uint32_t *r, const uint32_t *a)
 {
     uint32_t x[16];
 #pragma unroll
@@ -93,7 +101,7 @@ __device__ __forceinline__ void sc_reduce256(uint32_t *r, const uint32_t *a)
 }
 
 // r = a * b mod l (any 256-bit a, b) -- Mul for Scalar (C/scalar.rs:317-322)
-__device__ __forceinline__ void sc_mul(uint32_t *r, const uint32_t *a, const uint32_t *b)
+SC_HD void sc_mul(uint32_t *r, const uint32_t *a, const uint32_t *b)
 {
     uint32_t p[16];
     mp_mul<8, 8>(p, a, b);
@@ -101,7 +109,7 @@ __device__ __forceinline__ void sc_mul(uint32_t *r, const uint32_t *a, const uin
 }
 
 // r = a + b mod l, inputs < l (C/scalar.rs:334-349)
-__device__ __forceinline__ void sc_add(uint32_t *r, const uint32_t *a, const uint32_t *b)
+SC_HD void sc_add(uint32_t *r, const uint32_t *a, const uint32_t *b)
 {
     uint32_t s[8], u[8], l[8];
     uint64_t carry = 0;
@@ -109,18 +117,19 @@ __device__ __forceinline__ void sc_add(uint32_t *r, const uint32_t *a, const uin
     for (int i = 0; i < 8; i++) { uint64_t t = (uint64_t)a[i] + b[i] + carry; s[i] = (uint32_t)t; carry = t >> 32; }
 #pragma unroll
     for (int i = 0; i < 8; i++) l[i] = SC_L[i];
-    uint32_t borrow = mp_sub<8>(u, s, l);     // inputs < l < 2^253: no carry out of 256 bits
+    const uint32_t keep = 0u - mp_sub<8>(u, s, l);   // inputs < l < 2^253: no carry out of 256 bits
 #pragma unroll
-    for (int i = 0; i < 8; i++) r[i] = borrow ? s[i] : u[i];
+    for (int i = 0; i < 8; i++) r[i] = (s[i] & keep) | (u[i] & ~keep);
 }
 
 // r = -a mod l for a < l (C/scalar.rs:366-374 after its reduction step)
-__device__ __forceinline__ void sc_neg(uint32_t *r, const uint32_t *a)
+SC_HD void sc_neg(uint32_t *r, const uint32_t *a)
 {
     uint32_t l[8], u[8], nz = 0;
 #pragma unroll
     for (int i = 0; i < 8; i++) { l[i] = SC_L[i]; nz |= a[i]; }
     mp_sub<8>(u, l, a);
+    const uint32_t m = 0u - ((nz | (0u - nz)) >> 31);   // all ones iff a != 0
 #pragma unroll
-    for (int i = 0; i < 8; i++) r[i] = nz ? u[i] : 0;
+    for (int i = 0; i < 8; i++) r[i] = u[i] & m;
 }

@@ -2,6 +2,8 @@
 //   VerifyingKey::from_bytes + verify        ed25519-dalek/src/verifying.rs:167-175, :203-219
 //   VerifyingKey::verify_strict              ed25519-dalek/src/verifying.rs:359-382
 //   RCompute                                 ed25519-dalek/src/verifying.rs:496-557
+//   verify_prehashed[_strict]                ed25519-dalek/src/verifying.rs:230-257, :424-459 (the same paths with the
+//                                            Ed25519ph challenge SHA-512(dom2 || R || A || PH): k_verify_each_ph, k_hram_ph)
 //   EdwardsPoint::vartime_double_scalar_mul_basepoint   curve25519-dalek/src/edwards.rs:1388-1397
 //       (serial backend scalar_mul/vartime_double_base.rs:23-72)
 // Unlike verify_batch, `verify` recomputes R' = [s]B - [k]A and compares its ENCODING with the signature's R
@@ -48,10 +50,13 @@ __device__ __forceinline__ uint32_t is_small_order(const ge_p3 &p)
 #ifndef EACH_MIN_BLOCKS
 #define EACH_MIN_BLOCKS 2
 #endif
-__global__ void __launch_bounds__(128, EACH_MIN_BLOCKS)
-k_verify_each(const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ offs, const uint32_t *__restrict__ sigs,
-              const uint32_t *__restrict__ keys, size_t n, int strict, const ge_niels_packed *__restrict__ base_row0,
-              uint8_t *__restrict__ out)
+// PH = 0: k = SHA-512(R || A || M), message i at msgs + offs[i]; PH = 1 (Ed25519ph, verifying.rs:530-535): k =
+// SHA-512(dom2 || R || A || PH), prehash i at msgs + 64 i (offs unused).  Everything after the challenge is shared.
+template <int PH>
+__device__ __forceinline__ void verify_each_body(const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ offs,
+                                                 const Sha512Prefix *dom, const uint32_t *__restrict__ sigs,
+                                                 const uint32_t *__restrict__ keys, size_t n, int strict,
+                                                 const ge_niels_packed *__restrict__ base_row0, uint8_t *__restrict__ out)
 {
     __shared__ double s_B[8 * 15];                               // (j+1) B as balanced FP64 affine Niels, j = 0..7
     if (threadIdx.x < 8) {
@@ -72,8 +77,11 @@ k_verify_each(const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ off
     uint32_t h[8];
     {
         uint32_t dig[16];
-        const uint64_t lo = offs[i], hi = offs[i + 1];
-        sha512_ram(dig, R, Ak, msgs + lo, (size_t)(hi - lo));
+        if (PH) sha512_pxm<2, 1>(dig, dom->b, dom->len, R, Ak, msgs + 64 * i, 64);
+        else {
+            const uint64_t lo = offs[i], hi = offs[i + 1];
+            sha512_ram(dig, R, Ak, msgs + lo, (size_t)(hi - lo));
+        }
         sc_reduce512(h, dig);
     }
     ge_p3 A;
@@ -146,11 +154,31 @@ k_verify_each(const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ off
     out[i] = v;
 }
 
+__global__ void __launch_bounds__(128, EACH_MIN_BLOCKS)
+k_verify_each(const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ offs, const uint32_t *__restrict__ sigs,
+              const uint32_t *__restrict__ keys, size_t n, int strict, const ge_niels_packed *__restrict__ base_row0,
+              uint8_t *__restrict__ out)
+{
+    verify_each_body<0>(msgs, offs, nullptr, sigs, keys, n, strict, base_row0, out);
+}
+
+// Ed25519ph: phs holds n 64-byte prehashes
+__global__ void __launch_bounds__(128, EACH_MIN_BLOCKS)
+k_verify_each_ph(const uint8_t *__restrict__ phs, const __grid_constant__ Sha512Prefix dom, const uint32_t *__restrict__ sigs,
+                 const uint32_t *__restrict__ keys, size_t n, int strict, const ge_niels_packed *__restrict__ base_row0,
+                 uint8_t *__restrict__ out)
+{
+    verify_each_body<1>(phs, nullptr, &dom, sigs, keys, n, strict, base_row0, out);
+}
+
 static int verify_each_dev(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const uint64_t *d_offs, const uint32_t *d_sigs,
-                           const uint32_t *d_keys, size_t n, int strict, uint8_t *d_out, cudaStream_t st)
+                           const uint32_t *d_keys, size_t n, int strict, uint8_t *d_out, cudaStream_t st,
+                           const Sha512Prefix *ph_dom = nullptr)
 {
     if (!n) return 0;
-    k_verify_each<<<cdiv(n, 128), 128, 0, st>>>(d_msgs, d_offs, d_sigs, d_keys, n, strict, (const ge_niels_packed *)ctx->base_table.p, d_out);
+    const ge_niels_packed *base = (const ge_niels_packed *)ctx->base_table.p;
+    if (ph_dom) k_verify_each_ph<<<cdiv(n, 128), 128, 0, st>>>(d_msgs, *ph_dom, d_sigs, d_keys, n, strict, base, d_out);
+    else k_verify_each<<<cdiv(n, 128), 128, 0, st>>>(d_msgs, d_offs, d_sigs, d_keys, n, strict, base, d_out);
     ctx->launches++;
     CUDA_TRY(ctx, cudaGetLastError());
     return 0;
@@ -351,15 +379,16 @@ k_verify_each_comb(const uint32_t *__restrict__ sigs, const uint32_t *__restrict
 }
 
 // Verification (verify or verify_strict) of n signatures (device inputs) through per-key comb tables; *used = 0 if the keys do not repeat
-// enough (or the tables would not fit) and the caller should run k_verify_each instead.
+// enough (or the tables would not fit) and the caller should run k_verify_each instead.  ph_dom: Ed25519ph (d_msgs = n prehashes).
 static int verify_each_comb(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const uint64_t *d_offs, const uint32_t *d_sigs,
-                            const uint32_t *d_keys, size_t n, int strict, uint8_t *d_out, bool *used)
+                            const uint32_t *d_keys, size_t n, int strict, uint8_t *d_out, bool *used,
+                            const Sha512Prefix *ph_dom = nullptr)
 {
     *used = false;
     if (!n || !ctx->opt_each_comb || !ctx->opt_field_f64) return 0;
     int rc;
     EachFront f;
-    if ((rc = verify_each_front(ctx, d_msgs, d_offs, d_sigs, d_keys, n, &f))) return rc;
+    if ((rc = verify_each_front(ctx, d_msgs, d_offs, d_sigs, d_keys, n, &f, ph_dom))) return rc;
     const size_t tab_bytes = f.nkeys * EACH_KEY_DOUBLES * sizeof(double);
     if (tab_bytes > ((size_t)8 << 30)) return 0;
     if (ctx->opt_each_comb == 1 && f.nkeys * 8 > n) return 0;             // a table costs about what eight plain verifications cost
@@ -445,6 +474,38 @@ int ed25519_b200_verify_each_flat(dalek_b200_ctx *ctx, const uint8_t *msgs_flat,
                         });
         if (rc) return rc;
     }
+    uint8_t any = 0;
+    for (size_t i = 0; i < n; i++) any |= results[i];
+    return any ? ED25519_ERR_VERIFY : DALEK_OK;
+}
+
+// verify_prehashed[_strict] (verifying.rs:230-257, :424-459): both paths of verify_each on the resident copies of the
+// inputs, with the challenge of Ed25519ph.  The prehashes have a fixed stride, so no offsets cross PCIe.
+int ed25519_b200_verify_prehashed_each(dalek_b200_ctx *ctx, const uint8_t *prehashes, const uint8_t *context, size_t context_len,
+                                       const uint8_t *sigs, const uint8_t *pubkeys, size_t n, int strict, uint8_t *results)
+{
+    if (!ctx || (n && (!prehashes || !sigs || !pubkeys || !results)) || (context_len && !context) || context_len > 255)
+        return DALEK_E_INVALID_ARG;
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    CallTimer timer(ctx);
+    if (!n) return DALEK_OK;
+    int rc;
+    if ((rc = base_table_ensure(ctx))) return rc;
+    Sha512Prefix dom;
+    ed25519ph_dom2(dom, context, context_len);
+    if ((rc = ws_reserve(ctx, ctx->misc1, n * 64))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->points_in, n * 96))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->misc6, n))) return rc;
+    uint8_t *d_ph = (uint8_t *)ctx->misc1.p, *d_sigs = (uint8_t *)ctx->points_in.p, *d_keys = d_sigs + n * 64, *d_out = (uint8_t *)ctx->misc6.p;
+    cudaStream_t st = ctx->stream;
+    CUDA_TRY(ctx, cudaMemcpyAsync(d_ph, prehashes, n * 64, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(d_sigs, sigs, n * 64, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(d_keys, pubkeys, n * 32, cudaMemcpyHostToDevice, st));
+    bool comb = false;
+    if ((rc = verify_each_comb(ctx, d_ph, nullptr, (const uint32_t *)d_sigs, (const uint32_t *)d_keys, n, strict, d_out, &comb, &dom))) return rc;
+    if (!comb && (rc = verify_each_dev(ctx, d_ph, nullptr, (const uint32_t *)d_sigs, (const uint32_t *)d_keys, n, strict, d_out, st, &dom))) return rc;
+    CUDA_TRY(ctx, cudaMemcpyAsync(results, d_out, n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaStreamSynchronize(st));
     uint8_t any = 0;
     for (size_t i = 0; i < n; i++) any |= results[i];
     return any ? ED25519_ERR_VERIFY : DALEK_OK;

@@ -22,7 +22,7 @@ static inline unsigned cdiv(size_t a, unsigned b) { return (unsigned)((a + b - 1
 
 #define X25519_THREADS 128
 #define X25519_COMB_THREADS 384
-#define X25519_COMB_DOUBLES (64 * 8 * COMB_ENTRY)
+#define X25519_COMB_DOUBLES COMB_BASE_DOUBLES
 
 __global__ void __launch_bounds__(X25519_THREADS)
 k_x25519(const uint32_t *__restrict__ scalars, const uint32_t *__restrict__ us, size_t n, uint32_t *__restrict__ out,
@@ -57,23 +57,18 @@ k_x25519_base(const uint32_t *__restrict__ scalars, const double *__restrict__ t
     __syncthreads();
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    ge64_p3 acc; ge64_identity(acc);
-    int carry = 0;
+    ge64_p3 acc;
     uint32_t w = 0;
-#pragma unroll 1
-    for (int pos = 0; pos < 64; pos++) {
+    comb_mul_base_nibbles(acc, s_tab, [&](int pos) {
         if ((pos & 7) == 0) {                                     // one scalar word per 8 digits, clamped as it is read
             w = scalars[8 * i + (pos >> 3)];
             w &= pos == 0 ? 0xfffffff8u : 0xffffffffu;
             w = pos == 56 ? ((w & 0x7fffffffu) | 0x40000000u) : w;
         }
-        int d = (int)(w & 15) + carry; w >>= 4;
-        if (pos < 63) { carry = (d + 8) >> 4; d -= carry << 4; }
-        const int m = d >> 31;
-        ge64_niels q;
-        comb_select(q, s_tab + (size_t)pos * 8 * COMB_ENTRY, (uint32_t)((d + m) ^ m));
-        ge64_madd(acc, acc, q, (uint32_t)(d < 0));
-    }
+        const uint32_t v = w & 15;
+        w >>= 4;
+        return v;
+    });
     fe64 num, den, inv, u;
     fe64_add(num, acc.Z, acc.Y);                                  // 2
     fe64_sub(den, acc.Z, acc.Y); fe64_carry(den, den);            // 1
@@ -85,17 +80,18 @@ k_x25519_base(const uint32_t *__restrict__ scalars, const double *__restrict__ t
     for (int j = 0; j < 8; j++) out[8 * i + j] = r[j];
 }
 
-static int x25519_table_ensure(dalek_b200_ctx *ctx)
+// the comb table of B, built once per context (with the dynamic shared-memory limit of k_x25519_base)
+int comb_base_table_ensure(dalek_b200_ctx *ctx)
 {
-    if (ctx->x25519_table_ready) return 0;
+    if (ctx->comb_base_table_ready) return 0;
     int rc;
-    if ((rc = ws_reserve(ctx, ctx->x25519_table, X25519_COMB_DOUBLES * sizeof(double)))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->comb_base_table, X25519_COMB_DOUBLES * sizeof(double)))) return rc;
     CUDA_TRY(ctx, cudaFuncSetAttribute(k_x25519_base, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)(X25519_COMB_DOUBLES * sizeof(double))));
-    k_x25519_base_table<<<4, 128, 0, ctx->stream>>>((double *)ctx->x25519_table.p);
+    k_x25519_base_table<<<4, 128, 0, ctx->stream>>>((double *)ctx->comb_base_table.p);
     ctx->launches++;
     CUDA_TRY(ctx, cudaGetLastError());
-    ctx->x25519_table_ready = true;
+    ctx->comb_base_table_ready = true;
     return 0;
 }
 
@@ -160,8 +156,8 @@ int dalek_b200_x25519_public_keys(dalek_b200_ctx *ctx, const uint8_t *scalars, s
     if (!n) return DALEK_OK;
     CallTimer timer(ctx);
     int rc;
-    if ((rc = x25519_table_ensure(ctx))) return rc;
-    const double *table = (const double *)ctx->x25519_table.p;
+    if ((rc = comb_base_table_ensure(ctx))) return rc;
+    const double *table = (const double *)ctx->comb_base_table.p;
     const size_t smem = X25519_COMB_DOUBLES * sizeof(double);
     rc = run_pieces(ctx, nullptr, nullptr, scalars, 32, nullptr, 0, out, 32, nullptr, 0, n,
                     [&](const uint8_t *, const uint64_t *, const uint8_t *dk, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *,

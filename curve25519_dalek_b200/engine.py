@@ -87,6 +87,10 @@ def load_library():
     lib.ed25519_b200_last_zs.argtypes = [vp, vp, sz]
     lib.dalek_b200_edwards_mul_base_batch.argtypes = [vp, vp, sz, vp, vp]
     lib.ed25519_b200_sign_batch_flat.argtypes = [vp, vp, vp, vp, sz, vp, vp]
+    lib.ed25519_b200_verifying_keys.argtypes = [vp, vp, sz, vp]
+    lib.ed25519_b200_sign_flat.argtypes = [vp, vp, sz, vp, vp, sz, vp]
+    lib.ed25519_b200_sign_prehashed.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp]
+    lib.ed25519_b200_verify_prehashed_each.argtypes = [vp, vp, vp, sz, vp, vp, sz, C.c_int, vp]
     lib.dalek_b200_edwards_to_montgomery_batch.argtypes = [vp, vp, sz, vp]
     lib.dalek_b200_x25519_batch.argtypes = [vp, vp, vp, sz, vp, vp]
     lib.dalek_b200_x25519_batch_dev.argtypes = [vp, vp, vp, sz, vp, vp]
@@ -105,8 +109,8 @@ class EngineError(RuntimeError):
 
 class SignatureError(Exception):
     """ed25519_dalek::SignatureError (ed25519-dalek/src/errors.rs:23-53): `.kind` is one of
-    'Verify', 'ArrayLength', 'ScalarFormat', 'PointDecompression'."""
-    KINDS = {1: "Verify", 2: "ArrayLength", 3: "ScalarFormat", 4: "PointDecompression"}
+    'Verify', 'ArrayLength', 'ScalarFormat', 'PointDecompression', 'PrehashedContextLength'."""
+    KINDS = {1: "Verify", 2: "ArrayLength", 3: "ScalarFormat", 4: "PointDecompression", 5: "PrehashedContextLength"}
 
     def __init__(self, code):
         self.code = code
@@ -421,6 +425,39 @@ class Engine:
                                                                C.addressof(comp) if want_compressed else None))
         return limbs, (bytes(comp)[:32 * n] if want_compressed else None)
 
+    # ---- signing (secret keys; constant time) ----
+    def verifying_keys(self, seeds, n):
+        """SigningKey::from_bytes(seed).verifying_key() for n 32-byte seeds -> n x 32 B."""
+        out = (C.c_uint8 * (32 * max(n, 1)))()
+        self._check(self.lib.ed25519_b200_verifying_keys(self.h, _ptr(seeds), n, C.addressof(out)))
+        return bytes(out)[:32 * n]
+
+    def sign_flat(self, seeds, n_seeds, msgs_flat, offsets, n):
+        """Signer::try_sign for n flat messages with n_seeds = n keys (seed i signs message i) or 1 -> n x 64 B."""
+        out = (C.c_uint8 * (64 * max(n, 1)))()
+        self._check(self.lib.ed25519_b200_sign_flat(self.h, _ptr(seeds), n_seeds, _ptr(msgs_flat), _ptr(offsets), n,
+                                                    C.addressof(out)))
+        return bytes(out)[:64 * n]
+
+    def sign_prehashed(self, seeds, n_seeds, prehashes, n, context=None):
+        """SigningKey::sign_prehashed (Ed25519ph) for n 64-byte prehashes and one context: (rc, n x 64 B); rc 5 is
+        PrehashedContextLength (a context longer than 255 bytes)."""
+        out = (C.c_uint8 * (64 * max(n, 1)))()
+        ctx = bytes(context) if context is not None else b""
+        rc = self._check(self.lib.ed25519_b200_sign_prehashed(self.h, _ptr(seeds), n_seeds, _ptr(prehashes), n,
+                                                              _ptr(ctx) if ctx else None, len(ctx), C.addressof(out)))
+        return rc, bytes(out)[:64 * n]
+
+    def verify_prehashed_each(self, prehashes, sigs, pubkeys, n, context=None, strict=False):
+        """verify_prehashed (or verify_prehashed_strict) of n signatures over 64-byte prehashes with one context:
+        (rc, results) as in verify_each_flat."""
+        res = (C.c_uint8 * max(n, 1))()
+        ctx = bytes(context) if context is not None else b""
+        rc = self._check(self.lib.ed25519_b200_verify_prehashed_each(self.h, _ptr(prehashes), _ptr(ctx) if ctx else None, len(ctx),
+                                                                     _ptr(sigs), _ptr(pubkeys), n, 1 if strict else 0,
+                                                                     C.addressof(res)))
+        return rc, list(res)[:n]
+
     def sign_batch_flat(self, seeds, msgs_flat, offsets, n):
         pks = (C.c_uint8 * (32 * max(n, 1)))()
         sigs = (C.c_uint8 * (64 * max(n, 1)))()
@@ -595,6 +632,85 @@ def x25519_public_keys(secrets, engine=None):
     raw = eng.x25519_public_keys(b"".join(ks), len(ks))
     outs = [raw[32 * i:32 * i + 32] for i in range(len(ks))]
     return outs[0] if single else outs
+
+
+def _items(xs, size, what):
+    single = isinstance(xs, (bytes, bytearray))
+    items = [bytes(xs)] if single else [bytes(x) for x in xs]
+    if any(len(x) != size for x in items):
+        raise ValueError("%s are %d bytes each" % (what, size))
+    return single, items
+
+
+def ed25519_verifying_keys(seeds, engine=None):
+    """SigningKey::from_bytes(seed).verifying_key() (signing.rs:106, :171) for each 32-byte seed: one seed gives its
+    32-byte VerifyingKey, a list gives the list."""
+    single, ks = _items(seeds, 32, "Ed25519 seeds")
+    eng = engine or default_engine()
+    raw = eng.verifying_keys(b"".join(ks), len(ks))
+    outs = [raw[32 * i:32 * i + 32] for i in range(len(ks))]
+    return outs[0] if single else outs
+
+
+def _sign_args(seeds, n):
+    single_key, ks = _items(seeds, 32, "Ed25519 seeds")
+    if not single_key and len(ks) not in (1, n):
+        raise ValueError("one seed, or one seed per message")
+    return ks
+
+
+def ed25519_sign(seeds, messages, engine=None):
+    """Signer::sign (signing.rs:566-571) on the GPU.  `messages` is one message (bytes) or a list; `seeds` is one 32-byte
+    seed, which signs every message, or a list with one seed per message.  Returns the 64-byte signature, or the list."""
+    single = isinstance(messages, (bytes, bytearray))
+    msgs = [bytes(messages)] if single else [bytes(m) for m in messages]
+    ks = _sign_args(seeds, len(msgs))
+    eng = engine or default_engine()
+    flat, offs, n = _flat_messages(msgs)
+    raw = eng.sign_flat(b"".join(ks), len(ks) if n else 0, flat, offs, n) if n else b""
+    outs = [raw[64 * i:64 * i + 64] for i in range(n)]
+    return outs[0] if single else outs
+
+
+def _prehash_items(prehashed):
+    """64-byte digests, or objects with .digest() such as hashlib.sha512 (the reference's MsgDigest)."""
+    single = isinstance(prehashed, (bytes, bytearray)) or hasattr(prehashed, "digest")
+    items = [prehashed] if single else list(prehashed)
+    out = [bytes(p.digest()) if hasattr(p, "digest") else bytes(p) for p in items]
+    if any(len(p) != 64 for p in out):
+        raise ValueError("Ed25519ph prehashes are 64-byte digests")
+    return single, out
+
+
+def ed25519_sign_prehashed(seeds, prehashed, context=None, engine=None):
+    """SigningKey::sign_prehashed (signing.rs:312, Ed25519ph) on the GPU.  `prehashed` is one digest or a list (64 bytes
+    each, or objects with .digest() such as hashlib.sha512(message)); `seeds` as in ed25519_sign.  Raises
+    SignatureError(5) (PrehashedContextLength) for a context longer than 255 bytes."""
+    single, phs = _prehash_items(prehashed)
+    ks = _sign_args(seeds, len(phs))
+    eng = engine or default_engine()
+    n = len(phs)
+    rc, raw = eng.sign_prehashed(b"".join(ks), len(ks) if n else 0, b"".join(phs), n, context)
+    if rc:
+        raise SignatureError(rc)
+    outs = [raw[64 * i:64 * i + 64] for i in range(n)]
+    return outs[0] if single else outs
+
+
+def ed25519_verify_prehashed(prehashed, signatures, verifying_keys, context=None, strict=False, engine=None):
+    """VerifyingKey::verify_prehashed / verify_prehashed_strict (verifying.rs:230-257, :424-459) of each signature: the
+    list of result codes (0 Ok, 1 Verify, 3 ScalarFormat, 4 PointDecompression), or one code for a single item.  A
+    context longer than 255 bytes raises ValueError."""
+    single, phs = _prehash_items(prehashed)
+    _, sigs = _items([signatures] if single else signatures, 64, "signatures")
+    _, keys = _items([verifying_keys] if single else verifying_keys, 32, "verifying keys")
+    if not (len(phs) == len(sigs) == len(keys)):
+        raise ValueError("prehashes, signatures and verifying keys must have the same length")
+    if context is not None and len(bytes(context)) > 255:
+        raise ValueError("an Ed25519ph context is at most 255 bytes")
+    eng = engine or default_engine()
+    _, res = eng.verify_prehashed_each(b"".join(phs), b"".join(sigs), b"".join(keys), len(phs), context, strict)
+    return res[0] if single else res
 
 
 class _Precomputation:

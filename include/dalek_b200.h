@@ -42,6 +42,7 @@ typedef struct dalek_b200_ctx dalek_b200_ctx;
 #define ED25519_ERR_ARRAY_LENGTH 2        /* InternalError::ArrayLength        (E/errors.rs:41-49) */
 #define ED25519_ERR_SCALAR_FORMAT 3       /* InternalError::ScalarFormat       (E/errors.rs:27) */
 #define ED25519_ERR_POINT_DECOMPRESSION 4 /* InternalError::PointDecompression (E/errors.rs:26) */
+#define ED25519_ERR_PREHASHED_CONTEXT_LENGTH 5 /* InternalError::PrehashedContextLength (E/errors.rs:50) */
 /* engine errors */
 #define DALEK_E_INVALID_ARG (-1)
 #define DALEK_E_NO_DEVICE (-2)
@@ -84,8 +85,9 @@ int dalek_b200_last_kernel_ms(const dalek_b200_ctx *ctx, float *ms, int *launche
  * verify_batch call, the largest kernel of that path; summed over the pieces of a host-streamed call). */
 int dalek_b200_last_stage_ms(const dalek_b200_ctx *ctx, const char *stage, float *ms);
 /* Milliseconds between CUDA events recorded on the context's stream at entry of the last MSM / verify_batch /
- * precomputed-MSM / X25519 / to_montgomery_batch / hash-to-group call and after the last work it enqueued (all of the call's streams joined): the device time
- * of that call, copies of host-buffer calls included. */
+ * precomputed-MSM / X25519 / to_montgomery_batch / hash-to-group call, or of the last ed25519_b200_verifying_keys /
+ * sign_flat / sign_prehashed / verify_prehashed_each call, and after the last work it enqueued (all of the call's streams
+ * joined): the device time of that call, copies of host-buffer calls included. */
 int dalek_b200_last_call_ms(const dalek_b200_ctx *ctx, float *ms);
 
 /* -------- EdwardsPoint multiscalar multiplication --------------------------------------- */
@@ -378,12 +380,42 @@ int ed25519_b200_verify_each_flat_dev(dalek_b200_ctx *ctx, const void *d_msgs_fl
 /* Debug/parity aid: the 16-byte z_i coefficients drawn in the last verify_batch call. */
 int ed25519_b200_last_zs(dalek_b200_ctx *ctx, uint8_t *zs_out, size_t n);
 
-/* -------- input synthesis (benchmarks / tests): fixed-base multiples and RFC 8032 signing ---- */
-/* out[i] = scalars[i] * B as extended limbs (EdwardsPoint::mul_base, C/edwards.rs:918-928). */
+/* -------- ed25519 signing (secret-key operations) ------------------------------------------------
+ * Host buffers; each call blocks and streams the batch in pieces like the codecs.  n = 0 is a successful no-op; a NULL
+ * buffer with n > 0 is DALEK_E_INVALID_ARG.  Flat messages follow the rule of the hash-to-group block.  Seeds are the
+ * 32-byte SecretKeys of SigningKey::from_bytes (E/signing.rs:106).  The signer is constant time in the secrets (the seed,
+ * its expansion, the nonce r): uniform control flow, full-row scans of the comb table of B, branch-free arithmetic mod l;
+ * only the lengths of the messages and of the context shape the work.  The device copies of the seeds and of their
+ * expansions are cleared before a call returns.  No option affects these calls.
+ *
+ * SigningKey::from_bytes(seed).verifying_key() (E/signing.rs:106, :171; hazmat.rs:84-99): n x 32 B seeds -> n x 32 B
+ * VerifyingKey bytes. */
+int ed25519_b200_verifying_keys(dalek_b200_ctx *ctx, const uint8_t *seeds, size_t n, uint8_t *pubkeys_out);
+/* Signer::try_sign -> raw_sign (E/signing.rs:566-571, :854-904): sigs_out n x 64 B, signature i over message i.
+ * n_seeds is n (seed i signs message i) or 1 (one key signs every message); any other value is DALEK_E_INVALID_ARG. */
+int ed25519_b200_sign_flat(dalek_b200_ctx *ctx, const uint8_t *seeds, size_t n_seeds, const uint8_t *msgs_flat,
+                           const uint64_t *msg_offsets, size_t n, uint8_t *sigs_out);
+/* SigningKey::sign_prehashed -> raw_sign_prehashed (Ed25519ph, E/signing.rs:312, :917-976): prehashes n x 64 B, the
+ * finalized MsgDigest of each message (PH(M) = SHA-512(M) for RFC 8032); one context of context_len <= 255 bytes for
+ * the batch (NULL only with context_len = 0: None and Some(b"") hash alike).  context_len > 255 returns
+ * ED25519_ERR_PREHASHED_CONTEXT_LENGTH.  n_seeds as in sign_flat. */
+int ed25519_b200_sign_prehashed(dalek_b200_ctx *ctx, const uint8_t *seeds, size_t n_seeds, const uint8_t *prehashes, size_t n,
+                                const uint8_t *context, size_t context_len, uint8_t *sigs_out);
+/* VerifyingKey::verify_prehashed (strict = 0) / verify_prehashed_strict (strict = 1) (E/verifying.rs:230-257, :424-459)
+ * for n independent signatures: results, return value and error precedence as in ed25519_b200_verify_each_flat, with the
+ * challenge k = SHA-512(dom2(1, C) || R || A || PH) mod l (RCompute with a prehash context, E/verifying.rs:496-557).
+ * prehashes: n x 64 B.  context_len > 255 is DALEK_E_INVALID_ARG (the reference only debug-asserts it). */
+int ed25519_b200_verify_prehashed_each(dalek_b200_ctx *ctx, const uint8_t *prehashes, const uint8_t *context,
+                                       size_t context_len, const uint8_t *sigs, const uint8_t *pubkeys, size_t n,
+                                       int strict, uint8_t *results);
+
+/* -------- input synthesis (benchmarks / tests): fixed-base multiples and keys + signatures ---- */
+/* out[i] = scalars[i] * B as extended limbs (EdwardsPoint::mul_base, C/edwards.rs:918-928).  Public scalars only:
+ * variable-time table lookups. */
 int dalek_b200_edwards_mul_base_batch(dalek_b200_ctx *ctx, const uint8_t *scalars, size_t n,
                                       uint64_t *out_limbs /* n x 20 */, uint8_t *out_compressed /* n x 32, nullable */);
-/* Deterministic Ed25519 keygen + sign on the GPU: seeds n x 32 B -> pubkeys n x 32 B, sigs n x 64 B
- * (E/signing.rs, hazmat.rs:40-99); message layout and checks as in verify_batch_flat. */
+/* Keys and signatures in one call: seeds n x 32 B -> pubkeys n x 32 B, sigs n x 64 B; ed25519_b200_verifying_keys
+ * followed by ed25519_b200_sign_flat with n_seeds = n (constant time); message layout and checks as in verify_batch_flat. */
 int ed25519_b200_sign_batch_flat(dalek_b200_ctx *ctx, const uint8_t *seeds, const uint8_t *msgs_flat,
                                  const uint64_t *msg_offsets, size_t n, uint8_t *pubkeys_out,
                                  uint8_t *sigs_out);
