@@ -1,6 +1,6 @@
 // api.cu -- the extern "C" boundary of libdalek_b200.so (include/dalek_b200.h): context handling,
-// host<->device staging and the MSM entry points.  verify_batch lives in batch.cu, the
-// constant-time / Ristretto entry points in straus.cu.
+// host<->device staging and the vartime MSM entry points (Edwards and Ristretto).  verify_batch lives in batch.cu, the
+// constant-time MSM and the Ristretto double-base batch in straus.cu.
 #include <cstring>
 #include <new>
 #include <random>
@@ -122,18 +122,16 @@ int dalek_b200_last_call_ms(const dalek_b200_ctx *ctx, float *ms)
 }  // extern "C"
 
 // ------------------------------------------------------------------------------------------
-static size_t point_in_bytes(int fmt) { return fmt == DALEK_POINTS_COMPRESSED ? 32 : 160; }
-
-// device scalars/points -> window sums in ctx->red? -> result.  Returns reference-level code.
-// Inputs (host or device) -> bucket sums -> window accumulators (-> result if d_result).
+// Inputs (host or device) -> bucket sums -> window accumulators (-> result if d_result); ctx->flags[0] is set if a
+// point does not decode.
 // Host inputs are streamed in chunks on a dedicated copy stream: while chunk k+1 crosses PCIe,
 // chunk k is converted, sorted and added into the (persistent) bucket sums.
 static int run_msm(dalek_b200_ctx *ctx, const void *scalars, const void *points_in, bool on_device, int point_fmt, size_t n,
                    size_t n_window /* the size the window width is chosen from: n, or the shard size of a sharded MSM */,
-                   ge_p3_raw *d_windows, int *bad_out, MsmResult *d_result)
+                   ge_p3_raw *d_windows, MsmResult *d_result)
 {
     int rc;
-    const size_t pin = point_in_bytes(point_fmt);
+    const size_t pin = msm_point_bytes(point_fmt);
     cudaStream_t st = ctx->stream;
     const int c = msm_choose_window_bits(ctx, n_window);
     // the reference's dispatch (edwards.rs:1025-1029): below 190 points vartime Straus -- here three launches
@@ -191,63 +189,71 @@ static int run_msm(dalek_b200_ctx *ctx, const void *scalars, const void *points_
         }
     }
     if (!straus && (rc = msm_reduce_finish(ctx, c, d_windows, d_result))) return rc;
-    if (bad_out) CUDA_TRY(ctx, cudaMemcpyAsync(bad_out, ctx->flags.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     return 0;
 }
 
-static int finish_msm(dalek_b200_ctx *ctx, const ge_p3_raw *d_windows, int ranks, size_t n_total,
-                      uint8_t out_compressed[32], uint64_t out_limbs[20], uint32_t *is_identity, bool already_combined = false)
+int msm_read_result(dalek_b200_ctx *ctx, const MsmResult *d_result, const int *d_bad, const uint32_t *d_enc,
+                    uint8_t out_compressed[32], uint64_t out_limbs[20])
 {
     int rc;
-    int c = msm_choose_window_bits(ctx, n_total);
-    int nwin = msm_window_count_for_bits(c);
-    if ((rc = ws_reserve(ctx, ctx->result, sizeof(MsmResult)))) return rc;
-    if (!already_combined && (rc = msm_combine_windows(ctx, d_windows, ranks, nwin, c, (MsmResult *)ctx->result.p))) return rc;
-    if ((rc = pinned_reserve(ctx, sizeof(MsmResult) + 64))) return rc;
+    cudaStream_t st = ctx->stream;
+    if ((rc = pinned_reserve(ctx, sizeof(MsmResult) + 128))) return rc;
     MsmResult *h = (MsmResult *)ctx->h_pinned;
-    CUDA_TRY(ctx, cudaMemcpyAsync(h, ctx->result.p, sizeof(MsmResult), cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    int *h_bad = (int *)((char *)ctx->h_pinned + sizeof(MsmResult));
+    uint8_t *h_enc = (uint8_t *)ctx->h_pinned + sizeof(MsmResult) + 64;
+    CUDA_TRY(ctx, cudaMemcpyAsync(h, d_result, sizeof(MsmResult), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(h_bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+    if (d_enc) CUDA_TRY(ctx, cudaMemcpyAsync(h_enc, d_enc, 32, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaStreamSynchronize(st));
     float ms = 0.f;
     if ((ms = elapsed_ms(ctx->ev_a, ctx->ev_b)) >= 0.f) ctx->last_kernel_ms = ms;
-    if (out_compressed) memcpy(out_compressed, h->compressed, 32);
+    if (out_compressed) memcpy(out_compressed, d_enc ? h_enc : (const uint8_t *)h->compressed, 32);
     if (out_limbs) memcpy(out_limbs, h->limbs, 160);
-    if (is_identity) *is_identity = h->is_identity;
-    return 0;
+    return *h_bad ? DALEK_NONE : DALEK_OK;
 }
 
+// One whole MSM, read back.  Ristretto points also give the Ristretto encoding of the result in out_compressed.  The
+// public entry points check the point format.
 static int msm_common(dalek_b200_ctx *ctx, const void *scalars, const void *points, bool on_device, int point_fmt,
                       size_t n, uint8_t out_compressed[32], uint64_t out_limbs[20])
 {
-    if (!ctx || (n && (!scalars || !points)) || (point_fmt != DALEK_POINTS_COMPRESSED && point_fmt != DALEK_POINTS_EXTENDED))
-        return DALEK_E_INVALID_ARG;
-    if (n >= (1ull << 31)) return DALEK_E_INVALID_ARG;
+    if (!ctx || (n && (!scalars || !points)) || n >= (1ull << 31)) return DALEK_E_INVALID_ARG;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     CallTimer timer(ctx);
     int rc;
-    int c = msm_choose_window_bits(ctx, n);
-    int nwin = msm_window_count_for_bits(c);
+    const int nwin = msm_window_count_for_bits(msm_choose_window_bits(ctx, n));
     if ((rc = ws_reserve(ctx, ctx->misc0, (size_t)nwin * sizeof(ge_p3_raw)))) return rc;
-    if ((rc = pinned_reserve(ctx, sizeof(MsmResult) + 64))) return rc;
-    int *h_bad = (int *)((char *)ctx->h_pinned + sizeof(MsmResult));
-    *h_bad = 0;
-    if ((rc = ws_reserve(ctx, ctx->result, sizeof(MsmResult)))) return rc;
-    if ((rc = run_msm(ctx, scalars, points, on_device, point_fmt, n, n, (ge_p3_raw *)ctx->misc0.p, h_bad, (MsmResult *)ctx->result.p))) return rc;
-    if ((rc = finish_msm(ctx, (const ge_p3_raw *)ctx->misc0.p, 1, n, out_compressed, out_limbs, nullptr, true))) return rc;
-    return *h_bad ? DALEK_NONE : DALEK_OK;
+    if ((rc = ws_reserve(ctx, ctx->result, sizeof(MsmResult) + 32))) return rc;
+    MsmResult *d_res = (MsmResult *)ctx->result.p;
+    uint32_t *d_enc = point_fmt == DALEK_POINTS_RISTRETTO ? (uint32_t *)(d_res + 1) : nullptr;
+    if ((rc = run_msm(ctx, scalars, points, on_device, point_fmt, n, n, (ge_p3_raw *)ctx->misc0.p, d_res))) return rc;
+    if (d_enc && (rc = ristretto_encode_result(ctx, d_res, d_enc))) return rc;
+    return msm_read_result(ctx, d_res, (const int *)ctx->flags.p, d_enc, out_compressed, out_limbs);
 }
+
+static bool edwards_format(int point_fmt) { return point_fmt == DALEK_POINTS_COMPRESSED || point_fmt == DALEK_POINTS_EXTENDED; }
 
 extern "C" {
 
 int dalek_b200_edwards_vartime_msm(dalek_b200_ctx *ctx, const uint8_t *scalars, const void *points, int point_fmt,
                                    size_t n, uint8_t out_compressed[32], uint64_t out_limbs[20])
 {
+    if (!edwards_format(point_fmt)) return DALEK_E_INVALID_ARG;
     return msm_common(ctx, scalars, points, false, point_fmt, n, out_compressed, out_limbs);
 }
 
 int dalek_b200_edwards_vartime_msm_dev(dalek_b200_ctx *ctx, const void *d_scalars, const void *d_points, int point_fmt,
                                        size_t n, uint8_t out_compressed[32], uint64_t out_limbs[20])
 {
+    if (!edwards_format(point_fmt)) return DALEK_E_INVALID_ARG;
     return msm_common(ctx, d_scalars, d_points, true, point_fmt, n, out_compressed, out_limbs);
+}
+
+int dalek_b200_ristretto_vartime_msm(dalek_b200_ctx *ctx, const uint8_t *scalars, const uint8_t *points, size_t n,
+                                     uint8_t out_compressed[32])
+{
+    if (!out_compressed) return DALEK_E_INVALID_ARG;
+    return msm_common(ctx, scalars, points, false, DALEK_POINTS_RISTRETTO, n, out_compressed, nullptr);
 }
 
 int dalek_b200_msm_window_count(dalek_b200_ctx *ctx, size_t n_shard)
@@ -297,8 +303,7 @@ __global__ void k_records_to_windows(const uint64_t *__restrict__ in, int ranks,
 static int partial_enqueue(dalek_b200_ctx *ctx, const void *scalars, const void *points, bool on_device, int point_fmt,
                            size_t n_local, size_t n_shard, int *nwin_out)
 {
-    if (!ctx || (n_local && (!scalars || !points)) || n_local > n_shard ||
-        (point_fmt != DALEK_POINTS_COMPRESSED && point_fmt != DALEK_POINTS_EXTENDED) || n_local >= (1ull << 31))
+    if (!ctx || (n_local && (!scalars || !points)) || n_local > n_shard || !edwards_format(point_fmt) || n_local >= (1ull << 31))
         return DALEK_E_INVALID_ARG;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     int rc;
@@ -306,7 +311,7 @@ static int partial_enqueue(dalek_b200_ctx *ctx, const void *scalars, const void 
     const int nwin = msm_window_count_for_bits(c);
     if ((rc = ws_reserve(ctx, ctx->misc0, (size_t)nwin * sizeof(ge_p3_raw)))) return rc;
     if ((rc = ws_reserve(ctx, ctx->misc1, (size_t)nwin * 160 + 8))) return rc;
-    if ((rc = run_msm(ctx, scalars, points, on_device, point_fmt, n_local, n_shard, (ge_p3_raw *)ctx->misc0.p, nullptr, nullptr))) return rc;
+    if ((rc = run_msm(ctx, scalars, points, on_device, point_fmt, n_local, n_shard, (ge_p3_raw *)ctx->misc0.p, nullptr))) return rc;
     k_windows_to_record<<<(nwin + 1 + 63) / 64, 64, 0, ctx->stream>>>((const ge_p3_raw *)ctx->misc0.p, nwin, (const int *)ctx->flags.p,
                                                                      (uint64_t *)ctx->misc1.p);
     ctx->launches++;
@@ -355,7 +360,8 @@ int msm_partial_enqueue_record(dalek_b200_ctx *ctx, const void *scalars, const v
     return DALEK_OK;
 }
 
-// records (host or device) -> Horner over windows -> result read-back
+// records (host or device) -> Horner over windows -> result read-back.  Not msm_read_result: the device span of an
+// open ..._partial_async call ends after the read-back copies, and only such a call refreshes last_kernel_ms.
 int msm_combine_records(dalek_b200_ctx *ctx, const void *records, bool on_device, size_t rec_bytes, int ranks, size_t n_shard,
                         uint8_t out_compressed[32], uint64_t out_limbs[20])
 {

@@ -9,6 +9,7 @@
 #include <utility>
 #include <vector>
 
+#include "../../include/dalek_b200.h"
 #include "ge.cuh"
 
 struct DevBuf {
@@ -148,10 +149,14 @@ int pinned_reserve(dalek_b200_ctx *ctx, size_t bytes);
 // kinds of prepared device point arrays: the bucket kernel reads PK_NIELS only; the vartime Straus path takes either
 enum { PK_NIELS = 0 /* ge_niels_packed, 96 B */, PK_PNIELS = 1 /* ge_pniels_packed, 128 B */ };
 
+// Bytes per input point of a format DALEK_POINTS_*: 32 for the compressed Edwards and Ristretto encodings, 160 for
+// extended limbs.
+inline size_t msm_point_bytes(int point_fmt) { return point_fmt == DALEK_POINTS_EXTENDED ? 160 : 32; }
+
 // Convert n input points (device memory, format DALEK_POINTS_*) into packed Niels form.
-// Compressed inputs give affine Niels (decompression yields Z = 1) and set *d_bad (device int) nonzero if any fails
-// to decode.  Extended inputs give affine Niels too, normalised to Z = 1 with one inversion per 1024 points; with
-// kind = PK_PNIELS they give projective Niels instead (no inversion, for the latency-bound Straus path).
+// Compressed Edwards and Ristretto inputs give affine Niels (decoding yields Z = 1) and set *d_bad (device int) nonzero
+// if any fails to decode.  Extended inputs give affine Niels too, normalised to Z = 1 with one inversion per 1024 points;
+// with kind = PK_PNIELS they give projective Niels instead (no inversion, for the latency-bound Straus path).
 // msm_prepared_kind tells which kind a format and a requested kind give.
 int msm_prepare_points(dalek_b200_ctx *ctx, const void *d_in, int point_fmt, size_t n, void *d_out,
                        int *d_bad, int kind = PK_NIELS);
@@ -161,9 +166,6 @@ int msm_prepared_kind(int point_fmt, int kind);
 int msm_choose_window_bits(const dalek_b200_ctx *ctx, size_t n);
 int msm_window_count_for_bits(int c);
 
-// Bucket MSM over device inputs: writes `nwin` window accumulators (raw p3) to d_windows.
-int msm_window_sums(dalek_b200_ctx *ctx, const uint32_t *d_scalars /* n x 8 words */, const ge_niels_packed *d_points,
-                    size_t n, int c, ge_p3_raw *d_windows);
 // total = sum over ranks of windows, Horner-combined; writes compressed (8 words) + canonical
 // limbs51 (20 u64) + identity flag to d_result (layout: 8 u32 | pad | 20 u64 | u32 flag).
 struct MsmResult { uint32_t compressed[8]; uint64_t limbs[20]; uint32_t is_identity; uint32_t pad; };
@@ -176,12 +178,14 @@ int msm_prepare_points_on(dalek_b200_ctx *ctx, cudaStream_t st, const void *d_in
 // window width for `n_short` scalars of `short_bits` bits plus `n_long` full-width scalars (verify_batch)
 int msm_choose_window_bits_mixed(const dalek_b200_ctx *ctx, size_t n_short, int short_bits, size_t n_long);
 int msm_reduce_finish(dalek_b200_ctx *ctx, int c, ge_p3_raw *d_windows, MsmResult *d_result, bool flat = false);
-int msm_fill_identity(dalek_b200_ctx *ctx, ge_p3_raw *d_out, uint32_t count);
-// window sums + Horner + encode in one go (single-shard case)
-int msm_full(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const ge_niels_packed *d_points, size_t n, int c,
-             ge_p3_raw *d_windows, MsmResult *d_result);
 int msm_combine_windows(dalek_b200_ctx *ctx, const ge_p3_raw *d_windows, int ranks, int nwin, int c,
                         MsmResult *d_result);
+// Blocking read-back of an MSM enqueued on ctx->stream (api.cu): the MsmResult at d_result, the status flag at d_bad
+// and, if d_enc is given, the 32-byte Ristretto encoding at d_enc, which then goes to out_compressed instead of the
+// Edwards one.  Sets last_kernel_ms from ev_a .. ev_b and fills the non-null outputs.  Returns DALEK_NONE if the flag
+// is set (a point did not decode), else DALEK_OK, or a negative engine code.
+int msm_read_result(dalek_b200_ctx *ctx, const MsmResult *d_result, const int *d_bad, const uint32_t *d_enc,
+                    uint8_t out_compressed[32], uint64_t out_limbs[20]);
 
 // ---- sharded MSM building blocks (api.cu), shared with the single-process multi-GPU entry points (multi.cu) ----
 // Enqueue the MSM of one shard on ctx's stream; its record (window accumulators + status word) is copied to
@@ -213,5 +217,5 @@ int base_table_ensure(dalek_b200_ctx *ctx);
 #define COMB_BASE_DOUBLES (64 * 8 * 15)
 int comb_base_table_ensure(dalek_b200_ctx *ctx);
 
-int ristretto_prepare_points(dalek_b200_ctx *ctx, const void *d_in, size_t n, void *d_out, int *d_bad);
+// RistrettoPoint::compress of an MSM result (straus.cu): 8 words at d_enc
 int ristretto_encode_result(dalek_b200_ctx *ctx, const MsmResult *d_res, uint32_t *d_enc);

@@ -80,6 +80,23 @@ __global__ void __launch_bounds__(128, 3) k_prep_compressed(const uint4 *__restr
     for (int k = 0; k < 6; k++) o[k] = make_uint4(p.w[4 * k], p.w[4 * k + 1], p.w[4 * k + 2], p.w[4 * k + 3]);
 }
 
+// CompressedRistretto -> affine Niels with the Ristretto decoding rules (ristretto.rs:266-345); the decoded point is
+// affine (Z = 1), so it goes straight to the form of the bucket kernel
+template <int F64>
+__global__ void k_prep_ristretto(const uint32_t *__restrict__ in, ge_niels_packed *__restrict__ out, size_t n, int *__restrict__ bad)
+{
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t enc[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) enc[k] = in[8 * i + k];
+    ge_p3 P;
+    if (!ristretto_decompress<F64>(P, enc)) { atomicOr(bad, 1); ge_p3_identity(P); }
+    ge_niels nl; ge_affine_to_niels(nl, P.X, P.Y);
+    ge_niels_packed pk; ge_niels_pack(pk, nl);
+    out[i] = pk;
+}
+
 // Extended points (X : Y : Z : T) -> affine Niels ((Y+X)/Z, (Y-X)/Z, 2d T/Z): the projective Niels point divided by Z,
 // so every input with Z != 0 stands for the same group element as before, T/Z = xy or not.  The bucket kernel then
 // adds every point with the 7M mixed addition in each of its ~16 windows instead of the 8M projective one, and
@@ -233,6 +250,9 @@ int msm_prepare_points_on(dalek_b200_ctx *ctx, cudaStream_t st, const void *d_in
     if (point_fmt == DALEK_POINTS_COMPRESSED) {
         if (ctx->opt_decompress_f64) k_prep_compressed<1><<<cdiv(n, 128), 128, 0, st>>>((const uint4 *)d_in, (ge_niels_packed *)d_out, n, d_bad);
         else k_prep_compressed<0><<<cdiv(n, 128), 128, 0, st>>>((const uint4 *)d_in, (ge_niels_packed *)d_out, n, d_bad);
+    } else if (point_fmt == DALEK_POINTS_RISTRETTO) {
+        if (ctx->opt_decompress_f64) k_prep_ristretto<1><<<cdiv(n, 128), 128, 0, st>>>((const uint32_t *)d_in, (ge_niels_packed *)d_out, n, d_bad);
+        else k_prep_ristretto<0><<<cdiv(n, 128), 128, 0, st>>>((const uint32_t *)d_in, (ge_niels_packed *)d_out, n, d_bad);
     } else if (kind == PK_PNIELS) {
         k_prep_extended_pniels<<<cdiv(n, 128), 128, 0, st>>>((const uint64_t *)d_in, (ge_pniels_packed *)d_out, n);
     } else {
@@ -990,40 +1010,6 @@ int msm_reduce_finish(dalek_b200_ctx *ctx, int c, ge_p3_raw *d_windows, MsmResul
     }
     CUDA_TRY(ctx, cudaGetLastError());
     return 0;
-}
-
-__global__ void k_fill_identity(ge_p3_raw *__restrict__ out, uint32_t count)
-{
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= count) return;
-    ge_p3 id; ge_p3_identity(id);
-    ge_p3_raw r; ge_p3_store_raw(r, id);
-    out[i] = r;
-}
-
-int msm_fill_identity(dalek_b200_ctx *ctx, ge_p3_raw *d_out, uint32_t count)
-{
-    if (!count) return 0;
-    k_fill_identity<<<cdiv(count, 128), 128, 0, ctx->stream>>>(d_out, count);
-    ctx->launches++;
-    CUDA_TRY(ctx, cudaGetLastError());
-    return 0;
-}
-
-int msm_window_sums(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const ge_niels_packed *d_points, size_t n,
-                    int c, ge_p3_raw *d_windows)
-{
-    int rc;
-    if ((rc = msm_accumulate_chunk(ctx, d_scalars, d_points, n, c, true))) return rc;
-    return msm_reduce_finish(ctx, c, d_windows, nullptr);
-}
-
-int msm_full(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const ge_niels_packed *d_points, size_t n, int c,
-             ge_p3_raw *d_windows, MsmResult *d_result)
-{
-    int rc;
-    if ((rc = msm_accumulate_chunk(ctx, d_scalars, d_points, n, c, true))) return rc;
-    return msm_reduce_finish(ctx, c, d_windows, d_result);
 }
 
 int msm_combine_windows(dalek_b200_ctx *ctx, const ge_p3_raw *d_windows, int ranks, int nwin, int c, MsmResult *d_result)

@@ -97,7 +97,7 @@ int dalek_b200_edwards_vartime_msm_multi(dalek_b200_multi *m, const uint8_t *sca
         if (cudaMalloc(&m->d_gather, rec * ndev) != cudaSuccess) { m->last_error = "cudaMalloc of the gather buffer failed"; return DALEK_E_NOMEM; }
         m->gather_cap = rec * ndev;
     }
-    const size_t pin = point_fmt == DALEK_POINTS_COMPRESSED ? 32 : 160;
+    const size_t pin = msm_point_bytes(point_fmt);
     std::vector<int> rcs(ndev, 0);
     auto shard = [&](int r) {
         dalek_b200_ctx *c = m->ctx[r];

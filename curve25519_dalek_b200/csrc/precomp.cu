@@ -84,15 +84,6 @@ __global__ void k_add_results(const MsmResult *__restrict__ a, const MsmResult *
     out->pad = 0;
 }
 
-static size_t in_bytes(int fmt) { return fmt == DALEK_POINTS_EXTENDED ? 160 : 32; }
-
-// device input in format `fmt` -> packed affine Niels points at d_out
-static int prepare(dalek_b200_ctx *ctx, const void *d_in, int fmt, size_t n, ge_niels_packed *d_out, int *d_bad)
-{
-    if (fmt == DALEK_POINTS_RISTRETTO) return ristretto_prepare_points(ctx, d_in, n, d_out, d_bad);
-    return msm_prepare_points(ctx, d_in, fmt, n, d_out, d_bad);
-}
-
 extern "C" {
 
 int dalek_b200_precomp_new(dalek_b200_ctx *ctx, const void *static_points, int point_fmt, size_t n, dalek_b200_precomp **out)
@@ -113,15 +104,15 @@ int dalek_b200_precomp_new(dalek_b200_ctx *ctx, const void *static_points, int p
         return DALEK_E_NOMEM;
     }
     auto fail = [&](int code) { cudaFree(pre->d_points); delete pre; return code; };
-    if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * in_bytes(point_fmt)))) return fail(rc);
+    if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * msm_point_bytes(point_fmt)))) return fail(rc);
     if ((rc = ws_reserve(ctx, ctx->flags, 64))) return fail(rc);
     if ((rc = pinned_reserve(ctx, 256))) return fail(rc);
     int *h_bad = (int *)ctx->h_pinned;
     *h_bad = 0;
     if (cudaMemsetAsync(ctx->flags.p, 0, 64, st) != cudaSuccess) return fail(DALEK_E_CUDA);
-    if (n && cudaMemcpyAsync(ctx->points_in.p, static_points, n * in_bytes(point_fmt), cudaMemcpyHostToDevice, st) != cudaSuccess)
+    if (n && cudaMemcpyAsync(ctx->points_in.p, static_points, n * msm_point_bytes(point_fmt), cudaMemcpyHostToDevice, st) != cudaSuccess)
         return fail(DALEK_E_CUDA);
-    if ((rc = prepare(ctx, ctx->points_in.p, point_fmt, n, pre->d_points, (int *)ctx->flags.p))) return fail(rc);
+    if ((rc = msm_prepare_points(ctx, ctx->points_in.p, point_fmt, n, pre->d_points, (int *)ctx->flags.p))) return fail(rc);
     if (cudaMemcpyAsync(h_bad, ctx->flags.p, 4, cudaMemcpyDeviceToHost, st) != cudaSuccess) return fail(DALEK_E_CUDA);
     if (cudaStreamSynchronize(st) != cudaSuccess) return fail(DALEK_E_CUDA);
     if (*h_bad) { ctx->last_error = "a static point does not decode"; return fail(DALEK_NONE); }
@@ -173,7 +164,7 @@ int dalek_b200_precomp_mixed_msm(dalek_b200_ctx *ctx, const dalek_b200_precomp *
     CallTimer timer(ctx);
     int rc;
     cudaStream_t st = ctx->stream;
-    const size_t din = in_bytes(dynamic_fmt);
+    const size_t din = msm_point_bytes(dynamic_fmt);
     const bool use_table = pre->d_table != nullptr && n_static > 0;
     // window widths: the table fixes the static width; the dynamic part picks its own
     const int c = use_table ? pre->c : msm_choose_window_bits(ctx, n_static + n_dynamic);
@@ -186,7 +177,6 @@ int dalek_b200_precomp_mixed_msm(dalek_b200_ctx *ctx, const dalek_b200_precomp *
     if ((rc = ws_reserve(ctx, ctx->flags, 64))) return rc;
     if ((rc = ws_reserve(ctx, ctx->misc0, (size_t)nwin * sizeof(ge_p3_raw)))) return rc;
     if ((rc = ws_reserve(ctx, ctx->result, 3 * sizeof(MsmResult) + 64))) return rc;
-    if ((rc = pinned_reserve(ctx, sizeof(MsmResult) + 128))) return rc;
     CUDA_TRY(ctx, cudaMemsetAsync(ctx->flags.p, 0, 64, st));
     uint32_t *d_ss = (uint32_t *)ctx->scalars.p, *d_ds = d_ss + 8 * n_static;
     MsmResult *d_res = (MsmResult *)ctx->result.p, *d_r1 = d_res + 1, *d_r2 = d_res + 2;
@@ -218,7 +208,7 @@ int dalek_b200_precomp_mixed_msm(dalek_b200_ctx *ctx, const dalek_b200_precomp *
     if (use_table) {
         if ((rc = msm_reduce_finish(ctx, c, (ge_p3_raw *)ctx->misc0.p, n_dynamic ? d_r1 : d_res, true))) return rc;
         if (n_dynamic) {
-            if ((rc = prepare(ctx, ctx->points_in.p, dynamic_fmt, n_dynamic, d_dpts, (int *)ctx->flags.p))) return rc;
+            if ((rc = msm_prepare_points(ctx, ctx->points_in.p, dynamic_fmt, n_dynamic, d_dpts, (int *)ctx->flags.p))) return rc;
             if ((rc = msm_accumulate_chunk(ctx, d_ds, d_dpts, n_dynamic, c_dyn, true))) return rc;
             if ((rc = msm_reduce_finish(ctx, c_dyn, (ge_p3_raw *)ctx->misc0.p, d_r2))) return rc;
             k_add_results<<<1, 1, 0, st>>>(d_r1, d_r2, d_res);
@@ -226,26 +216,15 @@ int dalek_b200_precomp_mixed_msm(dalek_b200_ctx *ctx, const dalek_b200_precomp *
         }
     } else {
         if (n_dynamic) {
-            if ((rc = prepare(ctx, ctx->points_in.p, dynamic_fmt, n_dynamic, d_dpts, (int *)ctx->flags.p))) return rc;
+            if ((rc = msm_prepare_points(ctx, ctx->points_in.p, dynamic_fmt, n_dynamic, d_dpts, (int *)ctx->flags.p))) return rc;
             if ((rc = msm_accumulate_chunk(ctx, d_ds, d_dpts, n_dynamic, c, false))) return rc;
         }
         if ((rc = msm_reduce_finish(ctx, c, (ge_p3_raw *)ctx->misc0.p, d_res))) return rc;
     }
-    uint32_t *d_enc = (uint32_t *)((char *)ctx->result.p + 3 * sizeof(MsmResult));
-    if (pre->ristretto && (rc = ristretto_encode_result(ctx, d_res, d_enc))) return rc;
-    MsmResult *h = (MsmResult *)ctx->h_pinned;
-    int *h_bad = (int *)((char *)ctx->h_pinned + sizeof(MsmResult));
-    uint8_t *h_enc = (uint8_t *)ctx->h_pinned + sizeof(MsmResult) + 64;
-    CUDA_TRY(ctx, cudaMemcpyAsync(h, d_res, sizeof(MsmResult), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(ctx, cudaMemcpyAsync(h_bad, ctx->flags.p, 4, cudaMemcpyDeviceToHost, st));
-    if (pre->ristretto) CUDA_TRY(ctx, cudaMemcpyAsync(h_enc, d_enc, 32, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(ctx, cudaStreamSynchronize(st));
-    float ms = 0.f;
-    if ((ms = elapsed_ms(ctx->ev_a, ctx->ev_b)) >= 0.f) ctx->last_kernel_ms = ms;
-    if (*h_bad) return DALEK_NONE;                      // optional_mixed_multiscalar_mul: a dynamic point was None
-    if (out_compressed) memcpy(out_compressed, pre->ristretto ? h_enc : (const uint8_t *)h->compressed, 32);
-    if (out_limbs) memcpy(out_limbs, h->limbs, 160);
-    return DALEK_OK;
+    uint32_t *d_enc = pre->ristretto ? (uint32_t *)(d_res + 3) : nullptr;
+    if (d_enc && (rc = ristretto_encode_result(ctx, d_res, d_enc))) return rc;
+    // DALEK_NONE: a dynamic point was None (optional_mixed_multiscalar_mul)
+    return msm_read_result(ctx, d_res, (const int *)ctx->flags.p, d_enc, out_compressed, out_limbs);
 }
 
 }  // extern "C"

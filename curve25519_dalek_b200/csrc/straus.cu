@@ -1,5 +1,5 @@
 // straus.cu -- constant-time multiscalar multiplication (the MultiscalarMul contract,
-// curve25519-dalek/src/traits.rs:78-134) and the Ristretto forwarders.
+// curve25519-dalek/src/traits.rs:78-134), the Ristretto double-base batch and the Ristretto encoding of MSM results.
 //
 // Reference algorithm: Straus with radix-16 signed digits and a constant-time 8-entry table scan
 // per point (src/backend/serial/scalar_mul/straus.rs:103-144, src/window.rs:54-76, :97-105,
@@ -149,23 +149,18 @@ int straus_ct_msm(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const void *d_
     if ((rc = ws_reserve(ctx, ctx->buckets, std::max<size_t>(1, n) * sizeof(ge_p3_raw)))) return rc;
     if ((rc = ws_reserve(ctx, ctx->red_a, std::max<size_t>(1, (n + 7) / 8) * sizeof(ge_p3_raw)))) return rc;
     ge_p3_raw *a = (ge_p3_raw *)ctx->buckets.p, *b = (ge_p3_raw *)ctx->red_a.p;
-    if (n == 0) {
-        k_store_identity<<<1, 1, 0, st>>>(a);
+    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, st));                // ev_a .. ev_b: the products (also recorded for n = 0)
+    if (n == 0) k_store_identity<<<1, 1, 0, st>>>(a);
+    else k_ct_scalar_mul<<<cdiv(n, 64), 64, 0, st>>>(d_scalars, (const ge_pniels_packed *)d_points_pniels, n, a);
+    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, st));
+    ctx->launches++;
+    ctx->last_kernel_launches = 1;
+    for (size_t cur = n; cur > 1;) {
+        size_t nxt = (cur + 7) / 8;
+        k_sum_level<<<cdiv(nxt, 64), 64, 0, st>>>(a, cur, b, nxt);
         ctx->launches++;
-    } else {
-        CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, st));
-        k_ct_scalar_mul<<<cdiv(n, 64), 64, 0, st>>>(d_scalars, (const ge_pniels_packed *)d_points_pniels, n, a);
-        CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, st));
-        ctx->launches++;
-        ctx->last_kernel_launches = 1;
-        size_t cur = n;
-        while (cur > 1) {
-            size_t nxt = (cur + 7) / 8;
-            k_sum_level<<<cdiv(nxt, 64), 64, 0, st>>>(a, cur, b, nxt);
-            ctx->launches++;
-            std::swap(a, b);
-            cur = nxt;
-        }
+        std::swap(a, b);
+        cur = nxt;
     }
     return msm_combine_windows(ctx, a, 1, 1, 4, d_result);
 }
@@ -331,24 +326,7 @@ static int double_base_status(dalek_b200_ctx *ctx, const DoubleBasePlan &plan, i
 }
 
 // ------------------------------------------------------------------------------------------
-// Ristretto vartime MSM: decode with the Ristretto rules, then the Edwards bucket MSM; encode the
-// result with RistrettoPoint::compress (ristretto.rs:980-994).
-// The decoded point is affine (Z = 1), so it goes straight to the affine Niels form of the bucket kernel.
-template <int F64>
-__global__ void k_prep_ristretto(const uint32_t *__restrict__ in, ge_niels_packed *__restrict__ out, size_t n, int *__restrict__ bad)
-{
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    uint32_t enc[8];
-#pragma unroll
-    for (int k = 0; k < 8; k++) enc[k] = in[8 * i + k];
-    ge_p3 P;
-    if (!ristretto_decompress<F64>(P, enc)) { atomicOr(bad, 1); ge_p3_identity(P); }
-    ge_niels nl; ge_affine_to_niels(nl, P.X, P.Y);
-    ge_niels_packed pk; ge_niels_pack(pk, nl);
-    out[i] = pk;
-}
-
+// The result of a Ristretto MSM (vartime or precomputed): RistrettoPoint::compress (ristretto.rs:980-994)
 __global__ void k_ristretto_encode_result(const MsmResult *__restrict__ res, uint32_t *__restrict__ out)
 {
     ge_p3 p;
@@ -359,18 +337,6 @@ __global__ void k_ristretto_encode_result(const MsmResult *__restrict__ res, uin
     for (int k = 0; k < 8; k++) out[k] = enc[k];
 }
 
-// CompressedRistretto (device, n x 32 B) -> packed affine Niels; *d_bad set if one does not decode
-int ristretto_prepare_points(dalek_b200_ctx *ctx, const void *d_in, size_t n, void *d_out, int *d_bad)
-{
-    if (!n) return 0;
-    if (ctx->opt_decompress_f64) k_prep_ristretto<1><<<cdiv(n, 128), 128, 0, ctx->stream>>>((const uint32_t *)d_in, (ge_niels_packed *)d_out, n, d_bad);
-    else k_prep_ristretto<0><<<cdiv(n, 128), 128, 0, ctx->stream>>>((const uint32_t *)d_in, (ge_niels_packed *)d_out, n, d_bad);
-    ctx->launches++;
-    CUDA_TRY(ctx, cudaGetLastError());
-    return 0;
-}
-
-// RistrettoPoint::compress of an MSM result (device): 8 words at d_enc
 int ristretto_encode_result(dalek_b200_ctx *ctx, const MsmResult *d_res, uint32_t *d_enc)
 {
     k_ristretto_encode_result<<<1, 1, 0, ctx->stream>>>(d_res, d_enc);
@@ -391,7 +357,7 @@ int dalek_b200_edwards_ct_msm(dalek_b200_ctx *ctx, const uint8_t *scalars, const
     cudaStream_t st = ctx->stream;
     for (size_t i = 0; i < n; i++)
         if (scalars[32 * i + 31] & 0x80) { ctx->last_error = "scalar with bit 255 set (Scalar invariant #1)"; return DALEK_E_INVALID_ARG; }
-    size_t pin = point_fmt == DALEK_POINTS_COMPRESSED ? 32 : 160;
+    const size_t pin = msm_point_bytes(point_fmt);
     if ((rc = ws_reserve(ctx, ctx->scalars, std::max<size_t>(1, n) * 32))) return rc;
     if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * pin))) return rc;
     if ((rc = ws_reserve(ctx, ctx->points, std::max<size_t>(1, n) * sizeof(ge_pniels_packed)))) return rc;
@@ -412,18 +378,9 @@ int dalek_b200_edwards_ct_msm(dalek_b200_ctx *ctx, const uint8_t *scalars, const
         if ((rc = msm_prepare_points(ctx, ctx->points_in.p, point_fmt, n, ctx->points.p, (int *)ctx->flags.p, PK_PNIELS))) return rc;
     }
     if ((rc = straus_ct_msm(ctx, (const uint32_t *)ctx->scalars.p, d_pn, n, (MsmResult *)ctx->result.p))) return rc;
-    if ((rc = pinned_reserve(ctx, sizeof(MsmResult) + 64))) return rc;
-    MsmResult *h = (MsmResult *)ctx->h_pinned;
-    int *h_bad = (int *)((char *)ctx->h_pinned + sizeof(MsmResult));
-    CUDA_TRY(ctx, cudaMemcpyAsync(h, ctx->result.p, sizeof(MsmResult), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(ctx, cudaMemcpyAsync(h_bad, ctx->flags.p, 4, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(ctx, cudaStreamSynchronize(st));
-    float ms = 0.f;
-    if (n && (ms = elapsed_ms(ctx->ev_a, ctx->ev_b)) >= 0.f) ctx->last_kernel_ms = ms;
-    if (*h_bad) { ctx->last_error = "a compressed point does not decode (multiscalar_mul takes points, not Options)"; return DALEK_E_INVALID_ARG; }
-    if (out_compressed) memcpy(out_compressed, h->compressed, 32);
-    if (out_limbs) memcpy(out_limbs, h->limbs, 160);
-    return DALEK_OK;
+    rc = msm_read_result(ctx, (const MsmResult *)ctx->result.p, (const int *)ctx->flags.p, nullptr, out_compressed, out_limbs);
+    if (rc == DALEK_NONE) { ctx->last_error = "a compressed point does not decode (multiscalar_mul takes points, not Options)"; return DALEK_E_INVALID_ARG; }
+    return rc;
 }
 
 int dalek_b200_ristretto_double_base_batch(dalek_b200_ctx *ctx, const uint8_t *a, const uint8_t *b, const uint8_t G[32],
@@ -458,42 +415,6 @@ int dalek_b200_ristretto_double_base_batch(dalek_b200_ctx *ctx, const uint8_t *a
     if ((rc = double_base_status(ctx, plan, &status))) return rc;
     if (status) return DALEK_NONE;                                   // G or H does not decode; `out` is unspecified
     return DALEK_OK;
-}
-
-int dalek_b200_ristretto_vartime_msm(dalek_b200_ctx *ctx, const uint8_t *scalars, const uint8_t *points, size_t n,
-                                     uint8_t out_compressed[32])
-{
-    if (!ctx || !out_compressed || (n && (!scalars || !points)) || n >= (1ull << 31)) return DALEK_E_INVALID_ARG;
-    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    int rc;
-    cudaStream_t st = ctx->stream;
-    if ((rc = ws_reserve(ctx, ctx->scalars, std::max<size_t>(1, n) * 32))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * 32))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points, std::max<size_t>(1, n) * sizeof(ge_niels_packed)))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->flags, 64))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->result, sizeof(MsmResult) + 64))) return rc;
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->flags.p, 0, 64, st));
-    if (n) {
-        CUDA_TRY(ctx, cudaMemcpyAsync(ctx->scalars.p, scalars, n * 32, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(ctx, cudaMemcpyAsync(ctx->points_in.p, points, n * 32, cudaMemcpyHostToDevice, st));
-        if (ctx->opt_decompress_f64) k_prep_ristretto<1><<<cdiv(n, 128), 128, 0, st>>>((const uint32_t *)ctx->points_in.p, (ge_niels_packed *)ctx->points.p, n, (int *)ctx->flags.p);
-        else k_prep_ristretto<0><<<cdiv(n, 128), 128, 0, st>>>((const uint32_t *)ctx->points_in.p, (ge_niels_packed *)ctx->points.p, n, (int *)ctx->flags.p);
-        ctx->launches++;
-    }
-    int c = msm_choose_window_bits(ctx, n);
-    int nwin = msm_window_count_for_bits(c);
-    if ((rc = ws_reserve(ctx, ctx->misc0, (size_t)nwin * sizeof(ge_p3_raw)))) return rc;
-    if ((rc = msm_full(ctx, (const uint32_t *)ctx->scalars.p, (const ge_niels_packed *)ctx->points.p, n, c, (ge_p3_raw *)ctx->misc0.p, (MsmResult *)ctx->result.p))) return rc;
-    uint32_t *d_enc = (uint32_t *)((char *)ctx->result.p + sizeof(MsmResult));
-    k_ristretto_encode_result<<<1, 1, 0, st>>>((const MsmResult *)ctx->result.p, d_enc);
-    ctx->launches++;
-    if ((rc = pinned_reserve(ctx, 128))) return rc;
-    int *h_bad = (int *)((char *)ctx->h_pinned + 64);
-    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_pinned, d_enc, 32, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(ctx, cudaMemcpyAsync(h_bad, ctx->flags.p, 4, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(ctx, cudaStreamSynchronize(st));
-    memcpy(out_compressed, ctx->h_pinned, 32);
-    return *h_bad ? DALEK_NONE : DALEK_OK;
 }
 
 }  // extern "C"

@@ -68,7 +68,7 @@ k_straus_vartime(const int8_t *__restrict__ nafs, const ge_pniels_packed *__rest
     }
 }
 
-// sum scalars[i] * points[i] for n < 2^16 prepared points (PK_NIELS / PK_PNIELS); result like msm_full
+// sum scalars[i] * points[i] for n < 2^16 prepared points (PK_NIELS / PK_PNIELS); result like msm_reduce_finish
 int straus_vartime_msm(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const void *d_points, int point_kind, size_t n,
                        MsmResult *d_result)
 {

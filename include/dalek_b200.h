@@ -288,7 +288,9 @@ int dalek_b200_ristretto_double_base_batch(dalek_b200_ctx *ctx, const uint8_t *a
                                            const uint8_t G[32], const uint8_t H[32], size_t n,
                                            uint8_t *out);
 /* RistrettoPoint::vartime_multiscalar_mul over compressed Ristretto points
- * (C/ristretto.rs:980-994); result as CompressedRistretto. */
+ * (C/ristretto.rs:980-994); result as CompressedRistretto.  Runs like dalek_b200_edwards_vartime_msm, to which the
+ * reference forwards (vartime Straus below 190 pairs, host buffers streamed in chunks); DALEK_NONE if a point does
+ * not decode (C/ristretto.rs:266-345). */
 int dalek_b200_ristretto_vartime_msm(dalek_b200_ctx *ctx, const uint8_t *scalars,
                                      const uint8_t *points, size_t n, uint8_t out_compressed[32]);
 

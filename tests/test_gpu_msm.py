@@ -154,6 +154,18 @@ def test_small_msm_straus_path_and_bucket_path_agree(eng, oracle, n):
     assert rc == 1
 
 
+def test_edwards_msm_rejects_ristretto_points(eng):
+    """DALEK_POINTS_RISTRETTO (2) is a format of the Ristretto entry points only: the Edwards MSM calls reject it"""
+    n = 3
+    sb, pts = bytes(32 * n), bytes(32 * n)
+    out = (C.c_uint8 * 32)()
+    windows = (C.c_uint64 * (20 * eng.msm_window_count(n)))()
+    lib, h = eng.lib, eng.h
+    assert lib.dalek_b200_edwards_vartime_msm(h, sb, pts, 2, n, C.addressof(out), None) == -1
+    assert lib.dalek_b200_edwards_ct_msm(h, sb, pts, 2, n, C.addressof(out), None) == -1
+    assert lib.dalek_b200_edwards_msm_partial(h, sb, pts, 2, n, n, C.addressof(windows)) == -1
+
+
 def test_msm_sharded_partial_combine(eng, oracle):
     """SURVEY 8(e): contiguous shards -> window accumulators -> combine == single MSM.  The window width comes from
     the SHARD size (the work one GPU does), identical on every rank."""

@@ -9,9 +9,9 @@ tests/golden/ristretto.json holds vectors that fire each of the five rejection t
 first, the middle and the last slot of an otherwise valid input.
 
 The encoder (ristretto.rs:500-533) picks rotate and the signs from the representative it is given, so the same
-Ristretto point is fed as P + T for every T of the 4-torsion, with Z != 1.  The Ristretto MSM never takes the
-small-Straus path, so with field_f64 = 1 the bucket pipeline runs on nearly empty windows only here.  The MSM points
-are t_j B, and the group has prime order l, so the expected result of sum s_i P_i is encode(((sum s_i t_i) mod l) B)
+Ristretto point is fed as P + T for every T of the 4-torsion, with Z != 1.  Like the Edwards MSM, the Ristretto MSM
+runs vartime Straus below 190 pairs when small_straus = 1 and field_f64 = 1; the size test also runs with
+small_straus = 0, so that the bucket pipeline still runs on nearly empty windows.  The MSM points are t_j B, and the group has prime order l, so the expected result of sum s_i P_i is encode(((sum s_i t_i) mod l) B)
 for any 256-bit scalars."""
 import contextlib
 import json
@@ -29,7 +29,7 @@ from test_gpu_msm_variants import VARIANTS
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 L = pyref.L
-DEFAULTS = dict(field_f64=1, acc_tma=0, window_bits=0, decompress_f64=1, double_base_comb=1)
+DEFAULTS = dict(field_f64=1, acc_tma=0, window_bits=0, decompress_f64=1, double_base_comb=1, small_straus=1)
 NPOOL = 64
 EDGES = [2**256 - 1, L + 1, 1, L - 1, 2**255 - 1, 2**252, L, 0]      # nonzero first, so that n = 1 .. 3 are not trivial
 E4 = (0, 2, 4, 6)                 # EIGHT_TORSION[2k] (u64/constants.rs): the identity and the points of E[4]
@@ -267,21 +267,22 @@ def test_precomputation_extended_dynamic_coset_invariance(eng, oracle, pool, cos
         pre.close()
 
 
-# ---- 3. the vartime MSM by size, bucket-kernel form and decode field ----
+# ---- 3. the vartime MSM by size, bucket-kernel form, decode field and small-input path ----
 SIZES = [0, 1, 2, 3, 17, 189, 190, 191, 1000]
 
 
+@pytest.mark.parametrize("small_straus", [1, 0])
 @pytest.mark.parametrize("f64", [1, 0])
 @pytest.mark.parametrize("variant", list(VARIANTS))
 @pytest.mark.parametrize("n", SIZES)
-def test_vartime_msm_sizes_and_forms(eng, oracle, pool, n, variant, f64):
+def test_vartime_msm_sizes_and_forms(eng, oracle, pool, n, variant, f64, small_straus):
     sb, pts, scalars, idx, want = pool.case(n)
-    if n <= 191 and (variant, f64) == ("f64", 1):
+    if n <= 191 and (variant, f64, small_straus) == ("f64", 1, 1):
         # the oracle's own MSM on the decoded points agrees (scalars reduced: the group has order l)
         P = [oracle.ristretto_decompress(pool.enc[j]) for j in idx]
         got = oracle.msm("optional", [b32(s % L) for s in scalars], P)
         assert oracle.ristretto_compress(got) == want
-    with options(eng, decompress_f64=f64, **form(variant)):
+    with options(eng, decompress_f64=f64, small_straus=small_straus, **form(variant)):
         rc, got = eng.ristretto_vartime_msm(sb, pts, n)
     assert rc == 0 and got == want
 
@@ -297,10 +298,11 @@ def test_vartime_msm_every_window_width(eng, pool, c):
 
 
 def test_vartime_msm_large(eng, pool):
-    n = (1 << 16) + 3
-    sb, pts, _, _, want = pool.case(n)
-    rc, got = eng.ristretto_vartime_msm(sb, pts, n)
-    assert rc == 0 and got == want
+    """2^18 + 3 pairs: the host inputs are streamed in chunks"""
+    for n in ((1 << 16) + 3, (1 << 18) + 3):
+        sb, pts, _, _, want = pool.case(n)
+        rc, got = eng.ristretto_vartime_msm(sb, pts, n)
+        assert rc == 0 and got == want, n
 
 
 # ---- 4. results equal to the identity encode as 32 zero bytes ----
