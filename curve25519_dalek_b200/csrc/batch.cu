@@ -662,19 +662,27 @@ static int verify_reserve(dalek_b200_ctx *ctx, size_t n, VerifyBufs &b)
     return 0;
 }
 
-// Front end for signatures [i0, i1) (i0 a multiple of verify_chunk): hashing on stream_hash; transcript and coefficients
+// What one verify_batch[es] call adds to the context's options.
+struct VerifyCall {
+    // signatures per transcript: the batch size of a verify_batches call, else the verify_chunk option.  0 (the
+    // default): ONE transcript over the whole batch, the reference's (batch.rs:168-222); it needs every hram first, so
+    // it runs in verify_whole_transcript after the last piece.  > 0: one transcript per chunk.
+    uint32_t chunk;
+    const uint64_t *d_key_points;   // device: the callers' decompressed key points (..._points calls), or null
+    size_t batch;                   // 0: one verdict (verify_batch); > 0: independent batches of this many signatures
+    int32_t *verdicts;              // one per batch (batch > 0)
+};
+
+// Front end for signatures [i0, i1) (i0 a multiple of call.chunk): hashing on stream_hash; transcript and coefficients
 // on a high-priority stream (the main one for even pieces, stream3 for odd ones: a transcript kernel is a
 // latency-bound chain of Keccak permutations on few warps, so consecutive pieces should overlap);
 // decompression on the low-priority stream.  All wait for `ready` if given.
-static int verify_front(dalek_b200_ctx *ctx, const VerifyBufs &b, const uint8_t *d_msgs, const uint64_t *d_offs,
-                        const uint32_t *d_sigs, const uint32_t *d_keys, size_t n, size_t i0, size_t i1, cudaEvent_t ready,
-                        int piece = 0)
+static int verify_front(dalek_b200_ctx *ctx, const VerifyCall &call, const VerifyBufs &b, const uint8_t *d_msgs, const uint64_t *d_offs,
+                        const uint32_t *d_sigs, const uint32_t *d_keys, size_t n, size_t i0, size_t i1, cudaEvent_t ready, int piece)
 {
     cudaStream_t st = (piece & 1) ? ctx->stream3 : ctx->stream, st2 = ctx->stream2, sh = ctx->stream_hash;
     const size_t cnt = i1 - i0;
-    // verify_chunk = 0 (default): ONE transcript over the whole batch, the reference's (batch.rs:168-222); it needs every
-    // hram first, so it runs in verify_whole_transcript after the last piece.  > 0: one transcript per chunk (opt-in).
-    const uint32_t chunk = (uint32_t)ctx->opt_verify_chunk;
+    const uint32_t chunk = call.chunk;
     if (ready) { CUDA_TRY(ctx, cudaStreamWaitEvent(sh, ready, 0)); CUDA_TRY(ctx, cudaStreamWaitEvent(st2, ready, 0)); }
     if (cnt) {
         // the hashing -> transcript chain has little parallelism in its second stage: enqueue it first.  SHA-512 of every
@@ -705,12 +713,12 @@ static int verify_front(dalek_b200_ctx *ctx, const VerifyBufs &b, const uint8_t 
         if (cnt) k_key_dedupe<<<cdiv(cnt, 256), 256, 0, st2>>>(d_keys, i0, cnt, b.table, b.tmask, b.rep, b.uniq, b.dense, b.counters,
                                                                make_uint4(ctx->hash_seed[0], ctx->hash_seed[1], ctx->hash_seed[2], ctx->hash_seed[3]));
         CUDA_TRY(ctx, cudaMemcpyAsync(b.counters + 1 + piece, b.counters, 4, cudaMemcpyDeviceToDevice, st2));
-        if (cnt && ctx->key_points) k_prep_A_points<1><<<cdiv(cnt, 128), 128, 0, st2>>>(ctx->key_points, b.uniq, lo, hi, i0, cnt, points_A);
+        if (cnt && call.d_key_points) k_prep_A_points<1><<<cdiv(cnt, 128), 128, 0, st2>>>(call.d_key_points, b.uniq, lo, hi, i0, cnt, points_A);
         else if (cnt && ctx->opt_decompress_f64) k_prep_A<1><<<cdiv(cnt, 128), 128, 0, st2>>>(d_keys, b.uniq, lo, hi, i0, cnt, points_A, b.flags, b.bad_key);
         else if (cnt) k_prep_A<0><<<cdiv(cnt, 128), 128, 0, st2>>>(d_keys, b.uniq, lo, hi, i0, cnt, points_A, b.flags, b.bad_key);
         ctx->launches += cnt ? 2 : 0;
     } else if (cnt) {
-        if (ctx->key_points) k_prep_A_points<1><<<cdiv(cnt, 128), 128, 0, st2>>>(ctx->key_points, nullptr, nullptr, nullptr, i0, cnt, points_A);
+        if (call.d_key_points) k_prep_A_points<1><<<cdiv(cnt, 128), 128, 0, st2>>>(call.d_key_points, nullptr, nullptr, nullptr, i0, cnt, points_A);
         else if (ctx->opt_decompress_f64) k_prep_A<1><<<cdiv(cnt, 128), 128, 0, st2>>>(d_keys, nullptr, nullptr, nullptr, i0, cnt, points_A, b.flags, b.bad_key);
         else k_prep_A<0><<<cdiv(cnt, 128), 128, 0, st2>>>(d_keys, nullptr, nullptr, nullptr, i0, cnt, points_A, b.flags, b.bad_key);
         ctx->launches++;
@@ -728,12 +736,12 @@ static int verify_front(dalek_b200_ctx *ctx, const VerifyBufs &b, const uint8_t 
     return 0;
 }
 
-// verify_chunk = 0: the reference's single transcript over all n signatures (batch.rs:168-222) -- a strictly
+// call.chunk = 0: the reference's single transcript over all n signatures (batch.rs:168-222) -- a strictly
 // sequential sponge (1.73 Keccak permutations per signature), one warp -- then the coefficients.  Runs on the main
 // stream after the hashing of every piece.
-static int verify_whole_transcript(dalek_b200_ctx *ctx, const VerifyBufs &b, const uint32_t *d_sigs, size_t n)
+static int verify_whole_transcript(dalek_b200_ctx *ctx, const VerifyCall &call, const VerifyBufs &b, const uint32_t *d_sigs, size_t n)
 {
-    if (ctx->opt_verify_chunk || !n) return 0;
+    if (call.chunk || !n) return 0;
     cudaStream_t st = ctx->stream;
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_join2, ctx->stream_hash));       // every piece is hashed on stream_hash
     CUDA_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_join2, 0));
@@ -820,6 +828,18 @@ static int verify_equation(dalek_b200_ctx *ctx, const VerifyBufs &b, size_t n, s
     return 0;
 }
 
+// Stage timings of a call: kernel_ms, the bucket kernel of its (first) equation, if it was measured; the R decompression
+// of every piece.
+static void verify_stage_times(dalek_b200_ctx *ctx, float kernel_ms)
+{
+    float ms = 0.f;
+    if (kernel_ms >= 0.f) ctx->last_kernel_ms = kernel_ms;
+    ctx->last_prep_ms = 0.f;
+    for (int k = 0; k < ctx->prep_pieces; k++)
+        if ((ms = elapsed_ms(ctx->ev_prep[k][0], ctx->ev_prep[k][1])) >= 0.f) ctx->last_prep_ms += ms;
+    trace_dump(ctx);
+}
+
 // the single verdict of verify_batch
 static int verify_tail(dalek_b200_ctx *ctx, const VerifyBufs &b, size_t n, int pieces)
 {
@@ -831,12 +851,7 @@ static int verify_tail(dalek_b200_ctx *ctx, const VerifyBufs &b, size_t n, int p
     int *hflags = (int *)((char *)ctx->h_pinned + sizeof(MsmResult));
     CUDA_TRY(ctx, cudaMemcpyAsync(hflags, b.flags, 16, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    float ms = 0.f;
-    if ((ms = elapsed_ms(ctx->ev_a, ctx->ev_b)) >= 0.f) ctx->last_kernel_ms = ms;
-    ctx->last_prep_ms = 0.f;
-    for (int k = 0; k < ctx->prep_pieces; k++)
-        if ((ms = elapsed_ms(ctx->ev_prep[k][0], ctx->ev_prep[k][1])) >= 0.f) ctx->last_prep_ms += ms;
-    trace_dump(ctx);
+    verify_stage_times(ctx, elapsed_ms(ctx->ev_a, ctx->ev_b));
     // error precedence follows the reference: VerifyingKey::from_bytes happens before verify_batch
     // can be called (PointDecompression); then s canonicity (batch.rs:208-211); then R / equation.
     if (hflags[FLAG_BAD_A]) return ED25519_ERR_POINT_DECOMPRESSION;
@@ -852,9 +867,10 @@ static int verify_tail(dalek_b200_ctx *ctx, const VerifyBufs &b, size_t n, int p
 // first -- every batch has its own transcript, so a non-zero prime-order part survives in a sum of batch equations
 // except with the probability a forgery survives batch.rs itself -- and only when it fails are halves re-tested down
 // to single batches.
-static int verify_batches_tail(dalek_b200_ctx *ctx, const VerifyBufs &b, size_t n, int pieces, size_t batch, int32_t *verdicts)
+static int verify_batches_tail(dalek_b200_ctx *ctx, const VerifyCall &call, const VerifyBufs &b, size_t n, int pieces)
 {
     int rc;
+    const size_t batch = call.batch;
     size_t nkeys = 0;
     const size_t nb = (n + batch - 1) / batch;
     if ((rc = verify_join(ctx, b, n, pieces, &nkeys))) return rc;
@@ -922,19 +938,12 @@ static int verify_batches_tail(dalek_b200_ctx *ctx, const VerifyBufs &b, size_t 
             todo.push_back({r.k0, mid, true});
         }
     }
-    {   // stage timings of the call, as in verify_tail (the first equation's bucket kernel; the R decompression of every piece)
-        float ms = 0.f;
-        if (first_kernel_ms >= 0.f) ctx->last_kernel_ms = first_kernel_ms;
-        ctx->last_prep_ms = 0.f;
-        for (int k = 0; k < ctx->prep_pieces; k++)
-            if ((ms = elapsed_ms(ctx->ev_prep[k][0], ctx->ev_prep[k][1])) >= 0.f) ctx->last_prep_ms += ms;
-        trace_dump(ctx);
-    }
+    verify_stage_times(ctx, first_kernel_ms);
     int any = 0;
     for (size_t k = 0; k < nb; k++) {
         int v = (status[k] & 4) ? ED25519_ERR_POINT_DECOMPRESSION : (status[k] & 1) ? ED25519_ERR_SCALAR_FORMAT
                 : ((status[k] & (2 | 8)) || !eq_ok[k]) ? ED25519_ERR_VERIFY : DALEK_OK;
-        verdicts[k] = v;
+        call.verdicts[k] = v;
         any |= v;
     }
     return any ? ED25519_ERR_VERIFY : DALEK_OK;
@@ -969,37 +978,81 @@ int verify_each_front(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const uint64_t
     return 0;
 }
 
-// batch = 0: one verdict (verify_batch); batch > 0: independent batches of that many signatures, verdicts[k] each
-static int verify_dev(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const uint64_t *d_offs, const uint32_t *d_sigs,
-                      const uint32_t *d_keys, size_t n, size_t batch, int32_t *verdicts)
+// Kinds of verify_batch[es] entry point: where the inputs live, whether the caller passes the decompressed key points,
+// whether the call returns one verdict per batch.
+enum { VERIFY_DEVICE = 1, VERIFY_POINTS = 2, VERIFY_BATCHES = 4 };
+
+// The arguments of one call: n messages back to back with n + 1 offsets, n signatures (R || s), n keys and, with
+// VERIFY_POINTS, the decompressed point of every key (20 u64 limbs each); all in host memory or all in device memory.
+struct VerifyArgs { const void *msgs, *offs, *sigs, *keys, *key_points; size_t n, batch; int32_t *verdicts; };
+
+// Every verify_batch[es] entry point: the argument check, then the device inputs read in place or the host inputs
+// streamed in up to 8 pieces, then the whole-batch transcript and the tail of the call.
+static int verify_call(dalek_b200_ctx *ctx, int kind, const VerifyArgs &a)
 {
-    int rc;
+    const bool on_device = kind & VERIFY_DEVICE, batches = kind & VERIFY_BATCHES;
+    const size_t n = a.n;
+    const uint8_t *msgs = (const uint8_t *)a.msgs;
+    const uint64_t *offs = (const uint64_t *)a.offs;
+    if (!ctx || (batches && (!a.batch || a.batch > (1u << 20)))) return DALEK_E_INVALID_ARG;
+    if (n && (!a.sigs || !a.keys || ((kind & VERIFY_POINTS) && !a.key_points) || (batches && !a.verdicts))) return DALEK_E_INVALID_ARG;
+    if (on_device ? n && !offs : !flat_messages_ok(msgs, offs, n)) return DALEK_E_INVALID_ARG;
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     CallTimer timer(ctx);
+    // every batch of a verify_batches call gets exactly the reference's transcript
+    VerifyCall call{(uint32_t)(a.batch ? a.batch : (size_t)ctx->opt_verify_chunk), on_device ? (const uint64_t *)a.key_points : nullptr,
+                    a.batch, a.verdicts};
+    int rc, pieces = 1;
     VerifyBufs b;
-    if ((rc = verify_reserve(ctx, n, b))) return rc;
-    CUDA_TRY(ctx, cudaMemsetAsync(b.flags, 0, 64, ctx->stream));
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, ctx->stream));
-    if ((rc = verify_front(ctx, b, d_msgs, d_offs, d_sigs, d_keys, n, 0, n, ctx->ev_fork))) return rc;
-    if ((rc = verify_whole_transcript(ctx, b, d_sigs, n))) return rc;
-    return batch ? verify_batches_tail(ctx, b, n, 1, batch, verdicts) : verify_tail(ctx, b, n, 1);
+    const uint32_t *d_sigs = (const uint32_t *)a.sigs;
+    if (on_device) {
+        if ((rc = verify_reserve(ctx, n, b))) return rc;
+        CUDA_TRY(ctx, cudaMemsetAsync(b.flags, 0, 64, ctx->stream));
+        CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, ctx->stream));
+        if ((rc = verify_front(ctx, call, b, msgs, offs, d_sigs, (const uint32_t *)a.keys, n, 0, n, ctx->ev_fork, 0))) return rc;
+    } else {
+        const uint8_t *sigs = (const uint8_t *)a.sigs, *pubkeys = (const uint8_t *)a.keys;
+        const uint64_t *key_points = (const uint64_t *)a.key_points;
+        size_t mbytes = n ? (size_t)offs[n] : 0;
+        if ((rc = ws_reserve(ctx, ctx->misc1, mbytes + 16))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->msg_offs, (n + 1) * 8))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * 96))) return rc;   // sigs + keys
+        if ((rc = verify_reserve(ctx, n, b))) return rc;
+        uint8_t *d_msgs = (uint8_t *)ctx->misc1.p, *d_sig8 = (uint8_t *)ctx->points_in.p, *d_keys = d_sig8 + n * 64;
+        if (key_points) {
+            if ((rc = ws_reserve(ctx, ctx->key_pts, std::max<size_t>(1, n) * 160))) return rc;
+            call.d_key_points = (const uint64_t *)ctx->key_pts.p;
+        }
+        uint64_t *d_offs = (uint64_t *)ctx->msg_offs.p;
+        d_sigs = (const uint32_t *)d_sig8;
+        cudaStream_t st = ctx->stream, sc = ctx->stream_copy;
+        CUDA_TRY(ctx, cudaMemsetAsync(b.flags, 0, 64, st));
+        CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, st));
+        CUDA_TRY(ctx, cudaStreamWaitEvent(sc, ctx->ev_fork, 0));
+        // stream the batch in up to 8 pieces (boundaries on call.chunk multiples): the copy of piece k+1
+        // overlaps hashing / decompression of piece k
+        const size_t vc = std::max<size_t>(1, call.chunk);
+        pieces = n >= (1u << 18) ? (int)std::min<long>(8, std::max<long>(1, ctx->opt_verify_pieces)) : 1;
+        size_t prev = 0;
+        for (int k = 0; k < pieces; k++) {
+            size_t i1 = k == pieces - 1 ? n : std::min(n, ((n * (k + 1) / pieces) / vc) * vc);     // equal pieces: the front end outlasts the copies
+            size_t i0 = prev, cnt = i1 - i0;
+            prev = i1;
+            if (cnt) {
+                size_t m0 = (size_t)offs[i0], m1 = (size_t)offs[i1];
+                if (m1 > m0) CUDA_TRY(ctx, cudaMemcpyAsync(d_msgs + m0, msgs + m0, m1 - m0, cudaMemcpyHostToDevice, sc));
+                CUDA_TRY(ctx, cudaMemcpyAsync(d_offs + i0, offs + i0, (cnt + 1) * 8, cudaMemcpyHostToDevice, sc));
+                CUDA_TRY(ctx, cudaMemcpyAsync(d_sig8 + i0 * 64, sigs + i0 * 64, cnt * 64, cudaMemcpyHostToDevice, sc));
+                CUDA_TRY(ctx, cudaMemcpyAsync(d_keys + i0 * 32, pubkeys + i0 * 32, cnt * 32, cudaMemcpyHostToDevice, sc));
+                if (key_points) CUDA_TRY(ctx, cudaMemcpyAsync((char *)ctx->key_pts.p + i0 * 160, key_points + 20 * i0, cnt * 160, cudaMemcpyHostToDevice, sc));
+            }
+            CUDA_TRY(ctx, cudaEventRecord(ctx->ev_grp[k], sc));
+            if ((rc = verify_front(ctx, call, b, d_msgs, d_offs, d_sigs, (const uint32_t *)d_keys, n, i0, i1, ctx->ev_grp[k], k))) return rc;
+        }
+    }
+    if ((rc = verify_whole_transcript(ctx, call, b, d_sigs, n))) return rc;
+    return call.batch ? verify_batches_tail(ctx, call, b, n, pieces) : verify_tail(ctx, b, n, pieces);
 }
-
-// every batch gets exactly the reference's transcript: signatures per transcript = batch size for the call
-struct ChunkOverride {
-    dalek_b200_ctx *ctx; long saved;
-    ChunkOverride(dalek_b200_ctx *c, size_t batch) : ctx(c), saved(c->opt_verify_chunk) { if (batch) c->opt_verify_chunk = (long)batch; }
-    ~ChunkOverride() { ctx->opt_verify_chunk = saved; }
-};
-
-static int verify_host(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets, const uint8_t *sigs,
-                       const uint8_t *pubkeys, size_t n, size_t batch, int32_t *verdicts, const uint64_t *key_points = nullptr);
-
-// device pointer to the callers' decompressed key points for the duration of one call (..._points entry points)
-struct KeyPointsGuard {
-    dalek_b200_ctx *ctx;
-    KeyPointsGuard(dalek_b200_ctx *c, const uint64_t *p) : ctx(c) { c->key_points = p; }
-    ~KeyPointsGuard() { ctx->key_points = nullptr; }
-};
 
 extern "C" {
 
@@ -1007,128 +1060,56 @@ int ed25519_b200_verify_batch_flat_dev(dalek_b200_ctx *ctx, const void *d_msgs_f
                                        const void *d_sigs, const void *d_pubkeys, size_t n, size_t msgs_bytes)
 {
     (void)msgs_bytes;
-    if (!ctx || (n && (!d_msg_offsets || !d_sigs || !d_pubkeys))) return DALEK_E_INVALID_ARG;
-    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    return verify_dev(ctx, (const uint8_t *)d_msgs_flat, (const uint64_t *)d_msg_offsets, (const uint32_t *)d_sigs,
-                      (const uint32_t *)d_pubkeys, n, 0, nullptr);
+    return verify_call(ctx, VERIFY_DEVICE, {d_msgs_flat, d_msg_offsets, d_sigs, d_pubkeys, nullptr, n, 0, nullptr});
 }
 
 int ed25519_b200_verify_batch_flat_points_dev(dalek_b200_ctx *ctx, const void *d_msgs_flat, const void *d_msg_offsets,
                                               const void *d_sigs, const void *d_pubkeys, const void *d_key_points, size_t n)
 {
-    if (!ctx || (n && (!d_msg_offsets || !d_sigs || !d_pubkeys || !d_key_points))) return DALEK_E_INVALID_ARG;
-    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    KeyPointsGuard guard(ctx, (const uint64_t *)d_key_points);
-    return verify_dev(ctx, (const uint8_t *)d_msgs_flat, (const uint64_t *)d_msg_offsets, (const uint32_t *)d_sigs,
-                      (const uint32_t *)d_pubkeys, n, 0, nullptr);
+    return verify_call(ctx, VERIFY_DEVICE | VERIFY_POINTS, {d_msgs_flat, d_msg_offsets, d_sigs, d_pubkeys, d_key_points, n, 0, nullptr});
 }
 
 int ed25519_b200_verify_batch_flat_points(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets,
                                           const uint8_t *sigs, const uint8_t *pubkeys, const uint64_t *key_points, size_t n)
 {
-    if (!ctx || (n && (!sigs || !pubkeys || !key_points))) return DALEK_E_INVALID_ARG;
-    return verify_host(ctx, msgs_flat, msg_offsets, sigs, pubkeys, n, 0, nullptr, key_points);
+    return verify_call(ctx, VERIFY_POINTS, {msgs_flat, msg_offsets, sigs, pubkeys, key_points, n, 0, nullptr});
 }
 
 int ed25519_b200_verify_batches_flat_dev(dalek_b200_ctx *ctx, const void *d_msgs_flat, const void *d_msg_offsets,
                                          const void *d_sigs, const void *d_pubkeys, size_t n, size_t batch_size, int32_t *verdicts)
 {
-    if (!ctx || !batch_size || batch_size > (1u << 20) || (n && (!d_msg_offsets || !d_sigs || !d_pubkeys || !verdicts))) return DALEK_E_INVALID_ARG;
-    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    ChunkOverride guard(ctx, batch_size);
-    return verify_dev(ctx, (const uint8_t *)d_msgs_flat, (const uint64_t *)d_msg_offsets, (const uint32_t *)d_sigs,
-                      (const uint32_t *)d_pubkeys, n, batch_size, verdicts);
+    return verify_call(ctx, VERIFY_DEVICE | VERIFY_BATCHES, {d_msgs_flat, d_msg_offsets, d_sigs, d_pubkeys, nullptr, n, batch_size, verdicts});
 }
 
 int ed25519_b200_verify_batches_flat(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets,
                                      const uint8_t *sigs, const uint8_t *pubkeys, size_t n, size_t batch_size, int32_t *verdicts)
 {
-    if (!ctx || !batch_size || batch_size > (1u << 20) || (n && (!sigs || !pubkeys || !verdicts))) return DALEK_E_INVALID_ARG;
-    ChunkOverride guard(ctx, batch_size);
-    return verify_host(ctx, msgs_flat, msg_offsets, sigs, pubkeys, n, batch_size, verdicts);
+    return verify_call(ctx, VERIFY_BATCHES, {msgs_flat, msg_offsets, sigs, pubkeys, nullptr, n, batch_size, verdicts});
 }
 
 int ed25519_b200_verify_batches_flat_points_dev(dalek_b200_ctx *ctx, const void *d_msgs_flat, const void *d_msg_offsets, const void *d_sigs,
                                                 const void *d_pubkeys, const void *d_key_points, size_t n, size_t batch_size, int32_t *verdicts)
 {
-    if (!ctx || !batch_size || batch_size > (1u << 20) || (n && (!d_msg_offsets || !d_sigs || !d_pubkeys || !d_key_points || !verdicts)))
-        return DALEK_E_INVALID_ARG;
-    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    ChunkOverride guard(ctx, batch_size);
-    KeyPointsGuard kp(ctx, (const uint64_t *)d_key_points);
-    return verify_dev(ctx, (const uint8_t *)d_msgs_flat, (const uint64_t *)d_msg_offsets, (const uint32_t *)d_sigs,
-                      (const uint32_t *)d_pubkeys, n, batch_size, verdicts);
+    return verify_call(ctx, VERIFY_DEVICE | VERIFY_POINTS | VERIFY_BATCHES,
+                       {d_msgs_flat, d_msg_offsets, d_sigs, d_pubkeys, d_key_points, n, batch_size, verdicts});
 }
 
 int ed25519_b200_verify_batches_flat_points(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets, const uint8_t *sigs,
                                             const uint8_t *pubkeys, const uint64_t *key_points, size_t n, size_t batch_size, int32_t *verdicts)
 {
-    if (!ctx || !batch_size || batch_size > (1u << 20) || (n && (!sigs || !pubkeys || !key_points || !verdicts)))
-        return DALEK_E_INVALID_ARG;
-    ChunkOverride guard(ctx, batch_size);
-    return verify_host(ctx, msgs_flat, msg_offsets, sigs, pubkeys, n, batch_size, verdicts, key_points);
+    return verify_call(ctx, VERIFY_POINTS | VERIFY_BATCHES, {msgs_flat, msg_offsets, sigs, pubkeys, key_points, n, batch_size, verdicts});
 }
 
 int ed25519_b200_verify_batch_flat(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets,
                                    const uint8_t *sigs, const uint8_t *pubkeys, size_t n)
 {
-    if (!ctx || (n && (!sigs || !pubkeys))) return DALEK_E_INVALID_ARG;
-    return verify_host(ctx, msgs_flat, msg_offsets, sigs, pubkeys, n, 0, nullptr);
+    return verify_call(ctx, 0, {msgs_flat, msg_offsets, sigs, pubkeys, nullptr, n, 0, nullptr});
 }
-
-}  // extern "C"
-
-static int verify_host(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets, const uint8_t *sigs,
-                       const uint8_t *pubkeys, size_t n, size_t batch, int32_t *verdicts, const uint64_t *key_points)
-{
-    if (!flat_messages_ok(msgs_flat, msg_offsets, n)) return DALEK_E_INVALID_ARG;
-    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    CallTimer timer(ctx);
-    int rc;
-    size_t mbytes = n ? (size_t)msg_offsets[n] : 0;
-    if ((rc = ws_reserve(ctx, ctx->misc1, mbytes + 16))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->msg_offs, (n + 1) * 8))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * 96))) return rc;   // sigs + keys
-    VerifyBufs b;
-    if ((rc = verify_reserve(ctx, n, b))) return rc;
-    uint8_t *d_msgs = (uint8_t *)ctx->misc1.p, *d_sigs = (uint8_t *)ctx->points_in.p, *d_keys = d_sigs + n * 64;
-    if (key_points && (rc = ws_reserve(ctx, ctx->key_pts, std::max<size_t>(1, n) * 160))) return rc;
-    KeyPointsGuard guard(ctx, key_points ? (const uint64_t *)ctx->key_pts.p : nullptr);
-    uint64_t *d_offs = (uint64_t *)ctx->msg_offs.p;
-    cudaStream_t st = ctx->stream, sc = ctx->stream_copy;
-    CUDA_TRY(ctx, cudaMemsetAsync(b.flags, 0, 64, st));
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, st));
-    CUDA_TRY(ctx, cudaStreamWaitEvent(sc, ctx->ev_fork, 0));
-    // stream the batch in up to 8 pieces (boundaries on verify_chunk multiples): the copy of piece k+1
-    // overlaps hashing / decompression of piece k
-    const size_t vc = (size_t)std::max<long>(1, ctx->opt_verify_chunk);
-    int K = n >= (1u << 18) ? (int)std::min<long>(8, std::max<long>(1, ctx->opt_verify_pieces)) : 1;
-    size_t prev = 0;
-    for (int k = 0; k < K; k++) {
-        size_t i1 = k == K - 1 ? n : std::min(n, ((n * (k + 1) / K) / vc) * vc);     // equal pieces: the front end outlasts the copies
-        size_t i0 = prev, cnt = i1 - i0;
-        prev = i1;
-        if (cnt) {
-            size_t m0 = (size_t)msg_offsets[i0], m1 = (size_t)msg_offsets[i1];
-            if (m1 > m0) CUDA_TRY(ctx, cudaMemcpyAsync(d_msgs + m0, msgs_flat + m0, m1 - m0, cudaMemcpyHostToDevice, sc));
-            CUDA_TRY(ctx, cudaMemcpyAsync(d_offs + i0, msg_offsets + i0, (cnt + 1) * 8, cudaMemcpyHostToDevice, sc));
-            CUDA_TRY(ctx, cudaMemcpyAsync(d_sigs + i0 * 64, sigs + i0 * 64, cnt * 64, cudaMemcpyHostToDevice, sc));
-            CUDA_TRY(ctx, cudaMemcpyAsync(d_keys + i0 * 32, pubkeys + i0 * 32, cnt * 32, cudaMemcpyHostToDevice, sc));
-            if (key_points) CUDA_TRY(ctx, cudaMemcpyAsync((char *)ctx->key_pts.p + i0 * 160, key_points + 20 * i0, cnt * 160, cudaMemcpyHostToDevice, sc));
-        }
-        CUDA_TRY(ctx, cudaEventRecord(ctx->ev_grp[k], sc));
-        if ((rc = verify_front(ctx, b, d_msgs, d_offs, (const uint32_t *)d_sigs, (const uint32_t *)d_keys, n, i0, i1, ctx->ev_grp[k], k))) return rc;
-    }
-    if ((rc = verify_whole_transcript(ctx, b, (const uint32_t *)d_sigs, n))) return rc;
-    return batch ? verify_batches_tail(ctx, b, n, K, batch, verdicts) : verify_tail(ctx, b, n, K);
-}
-
-extern "C" {
 
 int ed25519_b200_verify_batch(dalek_b200_ctx *ctx, const uint8_t *const *msgs, const size_t *msg_lens,
                               const uint8_t *sigs, const uint8_t *pubkeys, size_t n)
 {
-    if (!ctx || (n && (!msgs || !msg_lens || !sigs || !pubkeys))) return DALEK_E_INVALID_ARG;
+    if (n && (!msgs || !msg_lens)) return DALEK_E_INVALID_ARG;             // the gather reads these; verify_call checks the rest
     // gather the messages into one staging buffer (multi-threaded for large batches)
     std::vector<uint64_t> offs(n + 1);
     offs[0] = 0;

@@ -59,7 +59,6 @@ struct dalek_b200_ctx {
     // device workspaces (grown on demand, reused across calls)
     DevBuf scalars, points_in, points, digits, counts, offsets, sorted, buckets, red_a, red_b, red_c,
         red_d, key_pts, result, flags, misc0, misc1, misc2, misc3, misc4, misc5, zs, base_table, ntasks, task_off, tasks, task_sums, msg_offs, sum_desc, sum_part, key_table, key_acc, task_order, sig_status, misc6, each_pow, each_tab, each_kstat;
-    const uint64_t *key_points = nullptr;   // device: callers' decompressed key points for the current verify_batch call (or null)
     uint32_t hash_seed[4] = {0x243F6A88u, 0x85A308D3u, 0x13198A2Eu, 0x03707344u};   // key of the public-key de-duplication hash, redrawn per context
     int sum_desc_c = -1;
     bool base_table_ready = false;

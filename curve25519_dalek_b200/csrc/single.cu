@@ -172,10 +172,10 @@ k_verify_each_ph(const uint8_t *__restrict__ phs, const __grid_constant__ Sha512
 }
 
 static int verify_each_dev(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const uint64_t *d_offs, const uint32_t *d_sigs,
-                           const uint32_t *d_keys, size_t n, int strict, uint8_t *d_out, cudaStream_t st,
-                           const Sha512Prefix *ph_dom = nullptr)
+                           const uint32_t *d_keys, size_t n, int strict, uint8_t *d_out, const Sha512Prefix *ph_dom)
 {
     if (!n) return 0;
+    cudaStream_t st = ctx->stream;
     const ge_niels_packed *base = (const ge_niels_packed *)ctx->base_table.p;
     if (ph_dom) k_verify_each_ph<<<cdiv(n, 128), 128, 0, st>>>(d_msgs, *ph_dom, d_sigs, d_keys, n, strict, base, d_out);
     else k_verify_each<<<cdiv(n, 128), 128, 0, st>>>(d_msgs, d_offs, d_sigs, d_keys, n, strict, base, d_out);
@@ -381,8 +381,7 @@ k_verify_each_comb(const uint32_t *__restrict__ sigs, const uint32_t *__restrict
 // Verification (verify or verify_strict) of n signatures (device inputs) through per-key comb tables; *used = 0 if the keys do not repeat
 // enough (or the tables would not fit) and the caller should run k_verify_each instead.  ph_dom: Ed25519ph (d_msgs = n prehashes).
 static int verify_each_comb(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const uint64_t *d_offs, const uint32_t *d_sigs,
-                            const uint32_t *d_keys, size_t n, int strict, uint8_t *d_out, bool *used,
-                            const Sha512Prefix *ph_dom = nullptr)
+                            const uint32_t *d_keys, size_t n, int strict, uint8_t *d_out, bool *used, const Sha512Prefix *ph_dom)
 {
     *used = false;
     if (!n || !ctx->opt_each_comb || !ctx->opt_field_f64) return 0;
@@ -411,6 +410,30 @@ static int verify_each_comb(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const ui
     return 0;
 }
 
+// the return code of a per-signature call: Verify if any signature failed
+static int verify_each_summary(const uint8_t *results, size_t n)
+{
+    uint8_t any = 0;
+    for (size_t i = 0; i < n; i++) any |= results[i];
+    return any ? ED25519_ERR_VERIFY : DALEK_OK;
+}
+
+// The rest of a per-signature call whose inputs are in device memory: the per-key comb path, or the plain kernel when
+// the keys do not repeat enough; then the results are read back.  ph_dom: Ed25519ph (d_msgs = n prehashes).
+static int verify_each_resident(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const uint64_t *d_offs, const uint32_t *d_sigs,
+                                const uint32_t *d_keys, size_t n, int strict, const Sha512Prefix *ph_dom, uint8_t *results)
+{
+    int rc;
+    if ((rc = ws_reserve(ctx, ctx->misc6, std::max<size_t>(1, n)))) return rc;
+    uint8_t *d_out = (uint8_t *)ctx->misc6.p;
+    bool comb = false;
+    if ((rc = verify_each_comb(ctx, d_msgs, d_offs, d_sigs, d_keys, n, strict, d_out, &comb, ph_dom))) return rc;
+    if (!comb && (rc = verify_each_dev(ctx, d_msgs, d_offs, d_sigs, d_keys, n, strict, d_out, ph_dom))) return rc;
+    if (n) CUDA_TRY(ctx, cudaMemcpyAsync(results, d_out, n, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    return verify_each_summary(results, n);
+}
+
 extern "C" {
 
 int ed25519_b200_verify_each_flat_dev(dalek_b200_ctx *ctx, const void *d_msgs_flat, const void *d_msg_offsets, const void *d_sigs,
@@ -421,17 +444,8 @@ int ed25519_b200_verify_each_flat_dev(dalek_b200_ctx *ctx, const void *d_msgs_fl
     CallTimer timer(ctx);
     int rc;
     if ((rc = base_table_ensure(ctx))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->misc6, std::max<size_t>(1, n)))) return rc;
-    bool comb = false;
-    if ((rc = verify_each_comb(ctx, (const uint8_t *)d_msgs_flat, (const uint64_t *)d_msg_offsets, (const uint32_t *)d_sigs,
-                               (const uint32_t *)d_pubkeys, n, strict, (uint8_t *)ctx->misc6.p, &comb))) return rc;
-    if (!comb && (rc = verify_each_dev(ctx, (const uint8_t *)d_msgs_flat, (const uint64_t *)d_msg_offsets, (const uint32_t *)d_sigs,
-                                       (const uint32_t *)d_pubkeys, n, strict, (uint8_t *)ctx->misc6.p, ctx->stream))) return rc;
-    if (n) CUDA_TRY(ctx, cudaMemcpyAsync(results, ctx->misc6.p, n, cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    uint8_t any = 0;
-    for (size_t i = 0; i < n; i++) any |= results[i];
-    return any ? ED25519_ERR_VERIFY : DALEK_OK;
+    return verify_each_resident(ctx, (const uint8_t *)d_msgs_flat, (const uint64_t *)d_msg_offsets, (const uint32_t *)d_sigs,
+                                (const uint32_t *)d_pubkeys, n, strict, nullptr, results);
 }
 
 int ed25519_b200_verify_each_flat(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets, const uint8_t *sigs,
@@ -449,34 +463,25 @@ int ed25519_b200_verify_each_flat(dalek_b200_ctx *ctx, const uint8_t *msgs_flat,
         if ((rc = ws_reserve(ctx, ctx->misc1, mbytes + 16))) return rc;
         if ((rc = ws_reserve(ctx, ctx->msg_offs, (n + 1) * 8))) return rc;
         if ((rc = ws_reserve(ctx, ctx->points_in, n * 96))) return rc;
-        if ((rc = ws_reserve(ctx, ctx->misc6, n))) return rc;
-        uint8_t *d_msgs = (uint8_t *)ctx->misc1.p, *d_sigs = (uint8_t *)ctx->points_in.p, *d_keys = d_sigs + n * 64, *d_out = (uint8_t *)ctx->misc6.p;
+        uint8_t *d_msgs = (uint8_t *)ctx->misc1.p, *d_sigs = (uint8_t *)ctx->points_in.p, *d_keys = d_sigs + n * 64;
         uint64_t *d_offs = (uint64_t *)ctx->msg_offs.p;
         cudaStream_t st = ctx->stream;
         if (mbytes) CUDA_TRY(ctx, cudaMemcpyAsync(d_msgs, msgs_flat, mbytes, cudaMemcpyHostToDevice, st));
         CUDA_TRY(ctx, cudaMemcpyAsync(d_offs, msg_offsets, (n + 1) * 8, cudaMemcpyHostToDevice, st));
         CUDA_TRY(ctx, cudaMemcpyAsync(d_sigs, sigs, n * 64, cudaMemcpyHostToDevice, st));
         CUDA_TRY(ctx, cudaMemcpyAsync(d_keys, pubkeys, n * 32, cudaMemcpyHostToDevice, st));
-        bool comb = false;
-        if ((rc = verify_each_comb(ctx, d_msgs, d_offs, (const uint32_t *)d_sigs, (const uint32_t *)d_keys, n, strict, d_out, &comb))) return rc;
-        if (!comb && (rc = verify_each_dev(ctx, d_msgs, d_offs, (const uint32_t *)d_sigs, (const uint32_t *)d_keys, n, strict, d_out, st))) return rc;
-        CUDA_TRY(ctx, cudaMemcpyAsync(results, d_out, n, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(ctx, cudaStreamSynchronize(st));
-    } else {
-        // independent per signature: pieces alternate between two streams (copy-in -> kernel -> copy-out)
-        const ge_niels_packed *base = (const ge_niels_packed *)ctx->base_table.p;
-        rc = run_pieces(ctx, msgs_flat, msg_offsets, sigs, 64, pubkeys, 32, results, 1, nullptr, 0, n,
-                        [&](const uint8_t *d_msgs, const uint64_t *d_offs, const uint8_t *d_sigs, const uint8_t *d_keys, size_t m,
-                            uint8_t *d_out, uint8_t *, cudaStream_t st) {
-                            k_verify_each<<<cdiv(m, 128), 128, 0, st>>>(d_msgs, d_offs, (const uint32_t *)d_sigs, (const uint32_t *)d_keys,
-                                                                        m, strict, base, d_out);
-                            return 0;
-                        });
-        if (rc) return rc;
+        return verify_each_resident(ctx, d_msgs, d_offs, (const uint32_t *)d_sigs, (const uint32_t *)d_keys, n, strict, nullptr, results);
     }
-    uint8_t any = 0;
-    for (size_t i = 0; i < n; i++) any |= results[i];
-    return any ? ED25519_ERR_VERIFY : DALEK_OK;
+    // independent per signature: pieces alternate between two streams (copy-in -> kernel -> copy-out)
+    const ge_niels_packed *base = (const ge_niels_packed *)ctx->base_table.p;
+    rc = run_pieces(ctx, msgs_flat, msg_offsets, sigs, 64, pubkeys, 32, results, 1, nullptr, 0, n,
+                    [&](const uint8_t *d_msgs, const uint64_t *d_offs, const uint8_t *d_sigs, const uint8_t *d_keys, size_t m,
+                        uint8_t *d_out, uint8_t *, cudaStream_t st) {
+                        k_verify_each<<<cdiv(m, 128), 128, 0, st>>>(d_msgs, d_offs, (const uint32_t *)d_sigs, (const uint32_t *)d_keys,
+                                                                    m, strict, base, d_out);
+                        return 0;
+                    });
+    return rc ? rc : verify_each_summary(results, n);
 }
 
 // verify_prehashed[_strict] (verifying.rs:230-257, :424-459): both paths of verify_each on the resident copies of the
@@ -495,20 +500,12 @@ int ed25519_b200_verify_prehashed_each(dalek_b200_ctx *ctx, const uint8_t *preha
     ed25519ph_dom2(dom, context, context_len);
     if ((rc = ws_reserve(ctx, ctx->misc1, n * 64))) return rc;
     if ((rc = ws_reserve(ctx, ctx->points_in, n * 96))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->misc6, n))) return rc;
-    uint8_t *d_ph = (uint8_t *)ctx->misc1.p, *d_sigs = (uint8_t *)ctx->points_in.p, *d_keys = d_sigs + n * 64, *d_out = (uint8_t *)ctx->misc6.p;
+    uint8_t *d_ph = (uint8_t *)ctx->misc1.p, *d_sigs = (uint8_t *)ctx->points_in.p, *d_keys = d_sigs + n * 64;
     cudaStream_t st = ctx->stream;
     CUDA_TRY(ctx, cudaMemcpyAsync(d_ph, prehashes, n * 64, cudaMemcpyHostToDevice, st));
     CUDA_TRY(ctx, cudaMemcpyAsync(d_sigs, sigs, n * 64, cudaMemcpyHostToDevice, st));
     CUDA_TRY(ctx, cudaMemcpyAsync(d_keys, pubkeys, n * 32, cudaMemcpyHostToDevice, st));
-    bool comb = false;
-    if ((rc = verify_each_comb(ctx, d_ph, nullptr, (const uint32_t *)d_sigs, (const uint32_t *)d_keys, n, strict, d_out, &comb, &dom))) return rc;
-    if (!comb && (rc = verify_each_dev(ctx, d_ph, nullptr, (const uint32_t *)d_sigs, (const uint32_t *)d_keys, n, strict, d_out, st, &dom))) return rc;
-    CUDA_TRY(ctx, cudaMemcpyAsync(results, d_out, n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(ctx, cudaStreamSynchronize(st));
-    uint8_t any = 0;
-    for (size_t i = 0; i < n; i++) any |= results[i];
-    return any ? ED25519_ERR_VERIFY : DALEK_OK;
+    return verify_each_resident(ctx, d_ph, nullptr, (const uint32_t *)d_sigs, (const uint32_t *)d_keys, n, strict, &dom, results);
 }
 
 }  // extern "C"
