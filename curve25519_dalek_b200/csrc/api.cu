@@ -24,7 +24,6 @@ int dalek_b200_init(int device, dalek_b200_ctx **out)
     if (!ctx) return DALEK_E_NOMEM;
     ctx->device = device;
     ctx->sm_count = prop.multiProcessorCount;
-    ctx->l2_bytes = (size_t)prop.l2CacheSize;
     try { std::random_device rd; for (int i = 0; i < 4; i++) ctx->hash_seed[i] ^= rd(); } catch (...) { }   // results never depend on it
     int prio_lo = 0, prio_hi = 0;
     cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);       // (greatest priority is the lower number)

@@ -20,7 +20,6 @@ struct DevBuf {
 struct dalek_b200_ctx {
     int device = 0;
     int sm_count = 132;
-    size_t l2_bytes = (size_t)50 << 20;
     cudaStream_t stream = nullptr;
     cudaStream_t stream2 = nullptr;
     cudaStream_t stream_copy = nullptr;

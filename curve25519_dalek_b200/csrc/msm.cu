@@ -5,11 +5,14 @@
 // points, src/edwards.rs:1025-1029).  The reference walks 33-43 windows of 6-8 bits serially;
 // here all windows run at once with c = 4..20-bit signed digits:
 //
-//   k_digits            one thread per scalar: signed radix-2^c digits (scalar.rs:1093-1150
-//                       generalised to c > 8), histogram of bucket sizes, rank inside the bucket
-//   k_scan_*            exclusive scan of the bucket sizes per window (multi-block)
-//   k_scatter           counting-sort scatter: point indices grouped by (window, bucket)
-//   k_task_count/fill   buckets cut into tasks of <= task_len entries (skewed / adversarial inputs)
+//   k_sort_count/bins_scan/partition/fine
+//                       signed radix-2^c digits (scalar.rs:1093-1150 generalised to c > 8), point indices
+//                       grouped by (window, bucket) in a two-level counting sort: coarse bins of 2^F buckets
+//                       through HBM, the low F bits in shared memory; bucket sizes and offsets
+//   k_task_count, k_scan_*
+//                       buckets cut into tasks of <= task_len entries (skewed / adversarial inputs), per-window
+//                       exclusive scan of the task counts (multi-block)
+//   k_task_fill
 //   k_task_hist/scan/scatter
 //                       counting sort of the tasks by length: warps run equal trip counts and the
 //                       grid drains longest-first
@@ -22,8 +25,8 @@
 //   k_combine           total = total*2^c + window (pippenger.rs:159), compress
 //
 // Data layout in HBM: scalars n x 32 B; points packed affine Niels (96 B: every input format is normalised
-// to Z = 1 first), canonical 32-byte coordinates, 16-byte aligned for 128-bit loads; digit/rank entries 8 B per
-// (window, scalar); sorted indices 4 B per entry; bucket sums 160 B (10 x u32 limbs x 4).
+// to Z = 1 first), canonical 32-byte coordinates, 16-byte aligned for 128-bit loads; sort records 8 B per
+// non-zero digit; sorted indices 4 B per entry; bucket sums 160 B (10 x u32 limbs x 4).
 #include <algorithm>
 #include <cstdio>
 #include <utility>
@@ -299,39 +302,302 @@ int msm_choose_window_bits_mixed(const dalek_b200_ctx *ctx, size_t n_short, int 
 }
 
 // ------------------------------------------------------------------------------------------
-// digits + histogram.  entry = (int32 digit << 32) | rank
-// flat = 1: the digits of every window count into the buckets of window 0 (precomputed 2^(cw) P tables)
-__global__ void k_digits(const uint4 *__restrict__ scalars, size_t n, int c, int nwin, uint32_t nbuckets,
-                         uint32_t *__restrict__ counts, uint64_t *__restrict__ entries, int flat)
+// Counting sort of the digits by (window, bucket), two levels.  A coarse bin is 2^F consecutive buckets of one
+// bucket window (F = fine bits, msm_sort_fine_bits).
+//   k_sort_count      one CTA per tile of SORT_COUNT_TILE scalars: shared histogram over (window, coarse bin), one
+//                     global atomic per non-empty bin
+//   k_sort_bins_scan  one CTA per bucket window: exclusive scan of its coarse counts -> bin cursors
+//   k_sort_partition  one CTA per tile of SORT_TILE scalars, window by window: the tile's records are staged in
+//                     shared memory by coarse bin, one atomic per (tile, bin) reserves a run of the bin, and the
+//                     runs are written contiguously.  Record = (stored index | sign << 31, fine digit), 8 B.
+//   k_sort_fine       one CTA per coarse bin (per slice of SORT_FINE_CAP records of a bigger one): counting sort on
+//                     the low F bits in shared memory; writes the bin's counts, offsets and sorted entries
+// Every scattered store lands in shared memory; global memory sees runs and whole bins.  The order of the entries
+// inside a bucket depends on the order of the atomics: the bucket sums are the same group elements either way.
+// flat != 0 (a table stride): the digits of every window count into the buckets of window 0 (precomputed 2^(cw) P
+// tables) and the stored index is w * flat + i.
+#define SORT_THREADS 512
+#define SORT_COUNT_TILE 4096u     // scalars per CTA of k_sort_count
+#define SORT_TILE 2048u           // scalars per CTA of k_sort_partition (SORT_TILE / SORT_THREADS per thread)
+#define SORT_HIST_MAX 8192u       // (window, coarse bin) counters of one k_sort_count CTA
+#define SORT_NC_MAX 4096u         // coarse bins per window
+#define SORT_FINE_MAX 12          // fine bits
+#define SORT_BIN_MEAN 4096u       // coarse bins are added while their mean size on uniform digits is above this
+#define SORT_FINE_CAP 8192u       // records of a coarse bin (or of a slice of a bigger one) k_sort_fine holds in shared memory
+
+// Digit of the lowest remaining window of s (tests/msm_digit_cases.py): s is shifted right by c, carry in and out.
+__device__ __forceinline__ int32_t next_digit(uint32_t s[8], uint32_t &carry, int c)
 {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    uint4 a = scalars[2 * i], b = scalars[2 * i + 1];
-    uint32_t s[9] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w, 0};
-    const uint32_t mask = (1u << c) - 1, half = 1u << (c - 1);
-    uint32_t carry = 0;
-    for (int w = 0; w < nwin; w++) {
-        int o = w * c;
-        uint32_t raw = 0;
-        if (o < 256) {
-            int wi = o >> 5, bi = o & 31;
-            uint64_t two = (uint64_t)s[wi] | ((uint64_t)s[wi + 1] << 32);
-            raw = (uint32_t)(two >> bi) & mask;
-            if (o + c > 256) raw &= (1u << (256 - o)) - 1;
+    const uint32_t v = (s[0] & ((1u << c) - 1)) + carry;
+#pragma unroll
+    for (int k = 0; k < 7; k++) s[k] = __funnelshift_r(s[k], s[k + 1], c);
+    s[7] >>= c;
+    if (v > (1u << (c - 1))) { carry = 1; return (int32_t)v - (int32_t)(1u << c); }
+    carry = 0;
+    return (int32_t)v;
+}
+
+__device__ __forceinline__ void load_scalar(uint32_t s[8], const uint4 *__restrict__ scalars, size_t i)
+{
+    const uint4 a = scalars[2 * i], b = scalars[2 * i + 1];
+    s[0] = a.x; s[1] = a.y; s[2] = a.z; s[3] = a.w; s[4] = b.x; s[5] = b.y; s[6] = b.z; s[7] = b.w;
+}
+
+// In-place exclusive scan of v[0, len) in shared memory by the whole CTA; returns the total.  scr: 33 words.
+__device__ uint32_t block_excl_scan(uint32_t *v, uint32_t len, uint32_t *scr)
+{
+    const uint32_t t = threadIdx.x, lane = t & 31, wid = t >> 5, nw = blockDim.x >> 5;
+    const uint32_t per = (len + blockDim.x - 1) / blockDim.x, b = min(t * per, len), e = min(b + per, len);
+    __syncthreads();
+    uint32_t sum = 0;
+    for (uint32_t k = b; k < e; k++) sum += v[k];
+    uint32_t incl = sum;
+    for (int d = 1; d < 32; d <<= 1) { uint32_t x = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= (uint32_t)d) incl += x; }
+    if (lane == 31) scr[wid] = incl;
+    __syncthreads();
+    if (wid == 0) {
+        const uint32_t x = lane < nw ? scr[lane] : 0;
+        uint32_t y = x;
+        for (int d = 1; d < 32; d <<= 1) { uint32_t z = __shfl_up_sync(0xffffffffu, y, d); if (lane >= (uint32_t)d) y += z; }
+        if (lane < nw) scr[lane] = y - x;
+        if (lane == 31) scr[32] = y;
+    }
+    __syncthreads();
+    uint32_t run = scr[wid] + incl - sum;
+    for (uint32_t k = b; k < e; k++) { const uint32_t x = v[k]; v[k] = run; run += x; }
+    const uint32_t total = scr[32];
+    __syncthreads();
+    return total;
+}
+
+// Position inside ctr[key] for every live lane of the warp, one atomic per distinct key: the big bins that
+// k_sort_partition counts and k_sort_fine slices come from skewed digits, where most lanes share a key.  Every lane
+// of the warp must call it.
+__device__ __forceinline__ uint32_t warp_claim(uint32_t *ctr, uint32_t key, bool live)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t peers = __match_any_sync(0xffffffffu, live ? key : 0xffffffffu);
+    const uint32_t leader = __ffs(peers) - 1;
+    uint32_t base = 0;
+    if (live && lane == leader) base = atomicAdd(&ctr[key], (uint32_t)__popc(peers));
+    base = __shfl_sync(0xffffffffu, base, leader);
+    return base + __popc(peers & ((1u << lane) - 1));
+}
+
+__global__ void __launch_bounds__(SORT_THREADS)
+k_sort_count(const uint4 *__restrict__ scalars, size_t n, int c, int nact, int F, uint32_t nc, int flat,
+             uint32_t *__restrict__ ccount)
+{
+    __shared__ uint32_t h[SORT_HIST_MAX];
+    const uint32_t nh = (flat ? 1u : (uint32_t)nact) * nc;
+    for (uint32_t k = threadIdx.x; k < nh; k += SORT_THREADS) h[k] = 0;
+    __syncthreads();
+    for (uint32_t j = 0; j < SORT_COUNT_TILE / SORT_THREADS; j++) {
+        const size_t i = (size_t)blockIdx.x * SORT_COUNT_TILE + j * SORT_THREADS + threadIdx.x;
+        if (i >= n) break;
+        uint32_t s[8], carry = 0;
+        load_scalar(s, scalars, i);
+        for (int w = 0; w < nact; w++) {
+            const int32_t d = next_digit(s, carry, c);
+            if (d) atomicAdd(&h[(flat ? 0u : (uint32_t)w * nc) + (((uint32_t)(d < 0 ? -d : d) - 1) >> F)], 1u);
         }
-        uint32_t v = raw + carry;
-        int32_t d;
-        if (v > half) { d = (int32_t)v - (int32_t)(1u << c); carry = 1; } else { d = (int32_t)v; carry = 0; }
-        uint32_t rank = 0;
-        if (d != 0) {
-            uint32_t bkt = (uint32_t)(d < 0 ? -d : d) - 1;
-            rank = atomicAdd(&counts[(flat ? (size_t)0 : (size_t)w * nbuckets) + bkt], 1u);
-        }
-        entries[(size_t)w * n + i] = ((uint64_t)(uint32_t)d << 32) | rank;
+    }
+    __syncthreads();
+    for (uint32_t k = threadIdx.x; k < nh; k += SORT_THREADS)
+        if (h[k]) atomicAdd(&ccount[k], h[k]);
+}
+
+// A coarse bin of more than SORT_FINE_CAP records (skewed scalars; the short scalars of verify_batch put half of
+// their digits of one window into one bucket) is "big": k_sort_partition counts its buckets with global atomics and
+// k_sort_fine sorts it in slices of SORT_FINE_CAP records, one CTA per slice.  Slice 0 of every bin runs in CTA
+// [0, nbins); the further slices ("extra") in CTAs nbins + the bin's place in the extra-slice prefix.
+__device__ __forceinline__ uint32_t extra_slices(uint32_t cnt) { return cnt > SORT_FINE_CAP ? (cnt - 1) / SORT_FINE_CAP : 0; }
+
+// One CTA per bucket window: cursor = exclusive scan of the coarse counts (bin bases inside the window's segment),
+// xpre = exclusive scan of the bins' extra slices, xtot[w] = the window's extra slices.  The bucket counts and the
+// fill counters of big bins are zeroed here, ahead of the atomics of k_sort_partition and k_sort_fine.
+__global__ void __launch_bounds__(SORT_THREADS)
+k_sort_bins_scan(const uint32_t *__restrict__ ccount, uint32_t nc, int F, uint32_t nbuckets, uint32_t *__restrict__ ccursor,
+                 uint32_t *__restrict__ xpre, uint32_t *__restrict__ xtot, uint32_t *__restrict__ counts,
+                 uint32_t *__restrict__ fill)
+{
+    __shared__ uint32_t v[SORT_NC_MAX], scr[33];
+    const size_t o = (size_t)blockIdx.x * nc;
+    for (uint32_t k = threadIdx.x; k < nc; k += SORT_THREADS) v[k] = ccount[o + k];
+    block_excl_scan(v, nc, scr);
+    for (uint32_t k = threadIdx.x; k < nc; k += SORT_THREADS) { ccursor[o + k] = v[k]; v[k] = extra_slices(ccount[o + k]); }
+    const uint32_t total = block_excl_scan(v, nc, scr);
+    for (uint32_t k = threadIdx.x; k < nc; k += SORT_THREADS) xpre[o + k] = v[k];
+    if (threadIdx.x == 0) xtot[blockIdx.x] = total;
+    for (uint32_t k = 0; k < nc; k++) {
+        if ((k + 1 < nc ? v[k + 1] : total) == v[k]) continue;   // no extra slice: not big
+        const size_t b0 = (size_t)blockIdx.x * nbuckets + ((size_t)k << F);
+        for (uint32_t f = threadIdx.x; f < (1u << F); f += SORT_THREADS) { counts[b0 + f] = 0; fill[b0 + f] = 0; }
     }
 }
 
-// per-window exclusive scan of counts -> offsets (relative to the window's segment), multi-block:
+// dynamic shared memory: stage[SORT_TILE] (uint2) | cnt[nc] | gbase[nc] | scr[33]
+__global__ void __launch_bounds__(SORT_THREADS, 2)
+k_sort_partition(const uint4 *__restrict__ scalars, size_t n, int c, int nact, int F, uint32_t nc, uint32_t nbuckets, size_t flat,
+                 const uint32_t *__restrict__ ccount, uint32_t *__restrict__ ccursor, uint2 *__restrict__ records,
+                 uint32_t *__restrict__ counts)
+{
+    constexpr int SPT = SORT_TILE / SORT_THREADS;
+    extern __shared__ uint32_t sm[];
+    uint2 *stage = reinterpret_cast<uint2 *>(sm);
+    uint32_t *cnt = sm + 2 * SORT_TILE, *gbase = cnt + nc, *scr = gbase + nc;
+    const uint32_t fmask = (1u << F) - 1;
+    uint32_t s[SPT][8], carry[SPT];
+    size_t idx[SPT];
+#pragma unroll
+    for (int j = 0; j < SPT; j++) {
+        idx[j] = (size_t)blockIdx.x * SORT_TILE + j * SORT_THREADS + threadIdx.x;
+        carry[j] = 0;
+        if (idx[j] < n) load_scalar(s[j], scalars, idx[j]);
+        else for (int k = 0; k < 8; k++) s[j][k] = 0;          // zero digits: no record
+    }
+    for (int w = 0; w < nact; w++) {
+        const uint32_t wb = flat ? 0u : (uint32_t)w;           // bucket window
+        for (uint32_t k = threadIdx.x; k < nc; k += SORT_THREADS) cnt[k] = 0;
+        __syncthreads();
+        uint32_t bkt[SPT], rank[SPT], neg[SPT];
+#pragma unroll
+        for (int j = 0; j < SPT; j++) {
+            const int32_t d = next_digit(s[j], carry[j], c);
+            neg[j] = d < 0;
+            bkt[j] = d ? (uint32_t)(d < 0 ? -d : d) - 1 : 0xffffffffu;
+            if (d) rank[j] = atomicAdd(&cnt[bkt[j] >> F], 1u);
+        }
+        __syncthreads();
+        for (uint32_t k = threadIdx.x; k < nc; k += SORT_THREADS) {
+            const uint32_t v = cnt[k];
+            gbase[k] = v ? atomicAdd(&ccursor[(size_t)wb * nc + k], v) : 0;
+        }
+        const uint32_t total = block_excl_scan(cnt, nc, scr);  // cnt -> first staged slot of each bin
+#pragma unroll
+        for (int j = 0; j < SPT; j++) {
+            if (bkt[j] == 0xffffffffu) continue;
+            const uint32_t cb = bkt[j] >> F;
+            const uint32_t val = (flat ? (uint32_t)((size_t)w * flat + idx[j]) : (uint32_t)idx[j]) | (neg[j] << 31);
+            stage[cnt[cb] + rank[j]] = make_uint2(val, (bkt[j] & fmask) | (cb << 16));
+        }
+        __syncthreads();
+        uint2 *dst = records + (flat ? (size_t)0 : (size_t)w * n);
+        for (uint32_t k0 = 0; k0 < total; k0 += SORT_THREADS) {      // uniform trip count: warp_claim below
+            const uint32_t k = k0 + threadIdx.x;
+            const uint2 r = k < total ? stage[k] : make_uint2(0, 0);
+            const uint32_t cb = r.y >> 16, f = r.y & 0xffffu;
+            if (k < total) dst[gbase[cb] + (k - cnt[cb])] = make_uint2(r.x, f);
+            const bool big = k < total && ccount[(size_t)wb * nc + cb] > SORT_FINE_CAP;
+            if (__any_sync(0xffffffffu, big)) warp_claim(counts + (size_t)wb * nbuckets, (cb << F) | f, big);
+        }
+        __syncthreads();
+    }
+}
+
+// Slice 0 of every coarse bin in CTAs [0, nbins), the top windows first (the skewed bins of reduced scalars and of short
+// scalars are there); the extra slices of big bins after them.  The partition left ccursor at the end of the bin.
+// A bin of at most SORT_FINE_CAP records is counted and sorted in shared memory and written out coalesced.  A slice
+// of a big bin takes the bin's offsets from its complete counts, claims a run of each of its fine buckets with one
+// atomic on the bucket's fill counter, and places its records in shared memory.
+// dynamic shared memory: recs[SORT_FINE_CAP] (uint2) | out[SORT_FINE_CAP] | h[2^F] | scr[33]
+__global__ void __launch_bounds__(SORT_THREADS, 2)
+k_sort_fine(const uint2 *__restrict__ records, const uint32_t *__restrict__ ccount, const uint32_t *__restrict__ ccursor,
+            const uint32_t *__restrict__ xpre, const uint32_t *__restrict__ xtot, size_t n, int F, uint32_t nc,
+            uint32_t nbuckets, uint32_t nwin, int flat, uint32_t *__restrict__ counts, uint32_t *__restrict__ offsets,
+            uint32_t *__restrict__ sorted, uint32_t *__restrict__ fill)
+{
+    extern __shared__ uint32_t sm[];
+    __shared__ uint32_t s_bin, s_slice;
+    uint2 *recs = reinterpret_cast<uint2 *>(sm);
+    uint32_t *out = sm + 2 * SORT_FINE_CAP, *h = out + SORT_FINE_CAP, *scr = h + (1u << F);
+    const uint32_t nf = 1u << F, nbins = nwin * nc;
+    uint32_t bin, slice = 0;
+    if (blockIdx.x < nbins) {
+        bin = nbins - 1 - blockIdx.x;
+    } else {
+        if (threadIdx.x == 0) {
+            uint32_t t = blockIdx.x - nbins, w = 0;
+            while (w < nwin && t >= xtot[w]) t -= xtot[w++];
+            s_bin = nbins;                                  // past the last extra slice
+            if (w < nwin) {
+                const uint32_t *x = xpre + (size_t)w * nc;
+                uint32_t lo = 0, hi = nc - 1;               // the big bin: the last one with x[k] <= t
+                while (lo < hi) { const uint32_t mid = (lo + hi + 1) / 2; if (x[mid] <= t) lo = mid; else hi = mid - 1; }
+                s_bin = w * nc + lo;
+                s_slice = t - x[lo] + 1;
+            }
+        }
+        __syncthreads();
+        bin = s_bin; slice = s_slice;
+        if (bin >= nbins) return;
+    }
+    const uint32_t wb = bin / nc, cb = bin % nc;
+    const uint32_t cnt = ccount[bin], base = ccursor[bin] - cnt;
+    const size_t seg = flat ? (size_t)0 : (size_t)wb * n;
+    const size_t b0 = (size_t)wb * nbuckets + ((size_t)cb << F);
+    const uint2 *src = records + seg + base;
+    uint32_t *dst = sorted + seg + base;
+    constexpr uint32_t U = 4;                               // records in flight per thread
+    if (cnt <= SORT_FINE_CAP) {
+        for (uint32_t f = threadIdx.x; f < nf; f += SORT_THREADS) h[f] = 0;
+        __syncthreads();
+        for (uint32_t k0 = 0; k0 < cnt; k0 += U * SORT_THREADS) {
+            uint2 r[U];
+#pragma unroll
+            for (uint32_t u = 0; u < U; u++) {
+                const uint32_t k = k0 + u * SORT_THREADS + threadIdx.x;
+                r[u] = k < cnt ? src[k] : make_uint2(0, 0);
+            }
+#pragma unroll
+            for (uint32_t u = 0; u < U; u++) {
+                const uint32_t k = k0 + u * SORT_THREADS + threadIdx.x;
+                if (k < cnt) { recs[k] = r[u]; atomicAdd(&h[r[u].y], 1u); }
+            }
+        }
+        __syncthreads();
+        for (uint32_t f = threadIdx.x; f < nf; f += SORT_THREADS) counts[b0 + f] = h[f];
+        block_excl_scan(h, nf, scr);
+        for (uint32_t f = threadIdx.x; f < nf; f += SORT_THREADS) offsets[b0 + f] = base + h[f];
+        __syncthreads();
+        for (uint32_t k = threadIdx.x; k < cnt; k += SORT_THREADS) { const uint2 r = recs[k]; out[atomicAdd(&h[r.y], 1u)] = r.x; }
+        __syncthreads();
+        for (uint32_t k = threadIdx.x; k < cnt; k += SORT_THREADS) dst[k] = out[k];
+        return;
+    }
+    // a slice of a big bin; out[0, nf) = the slice's counts, then the positions of its runs in the bin
+    for (uint32_t f = threadIdx.x; f < nf; f += SORT_THREADS) { h[f] = counts[b0 + f]; out[f] = 0; }
+    block_excl_scan(h, nf, scr);
+    if (slice == 0)
+        for (uint32_t f = threadIdx.x; f < nf; f += SORT_THREADS) offsets[b0 + f] = base + h[f];
+    const uint32_t lo = slice * SORT_FINE_CAP, m = min(SORT_FINE_CAP, cnt - lo);
+    for (uint32_t k0 = 0; k0 < m; k0 += U * SORT_THREADS) {
+        uint2 r[U];
+#pragma unroll
+        for (uint32_t u = 0; u < U; u++) {
+            const uint32_t k = k0 + u * SORT_THREADS + threadIdx.x;
+            r[u] = k < m ? src[lo + k] : make_uint2(0, 0);
+        }
+#pragma unroll
+        for (uint32_t u = 0; u < U; u++) {
+            const uint32_t k = k0 + u * SORT_THREADS + threadIdx.x;
+            if (k < m) recs[k] = r[u];
+            warp_claim(out, r[u].y, k < m);
+        }
+    }
+    __syncthreads();
+    for (uint32_t f = threadIdx.x; f < nf; f += SORT_THREADS)
+        if (out[f]) out[f] = h[f] + atomicAdd(&fill[b0 + f], out[f]);
+    __syncthreads();
+    for (uint32_t k0 = 0; k0 < m; k0 += SORT_THREADS) {
+        const uint32_t k = k0 + threadIdx.x;
+        const uint2 r = k < m ? recs[k] : make_uint2(0, 0);
+        const uint32_t pos = warp_claim(out, r.y, k < m);
+        if (k < m) dst[pos] = r.x;
+    }
+}
+
+// per-window exclusive scan of the task counts -> task list offsets (relative to the window's list), multi-block:
 // k_scan_partial (sum of each 4096-entry part), k_scan_bases (exclusive scan of the part sums of a
 // window, one CTA per window), k_scan_apply (local scan + part base).
 #define SCAN_PART 4096u
@@ -384,30 +650,6 @@ __global__ void __launch_bounds__(1024) k_scan_apply(const uint32_t *__restrict_
     uint32_t run = part_base[blockIdx.x] + sh[threadIdx.x >> 5] + incl - sum;
 #pragma unroll
     for (int k = 0; k < 4; k++) { if (base + k < nbuckets) dst[base + k] = run; run += v[k]; }
-}
-
-// Launched per group of windows [w0, w1) sized so that the group's slice of `sorted` fits in half of the L2
-// (25 MB on an H100): the 4-byte scattered writes of one 32-byte sector then merge in L2 instead of each
-// costing a DRAM read-modify-write.
-// flat != 0: one bucket window; the stored index is w * flat + i, the position of 2^(cw) P_i in the point table
-__global__ void k_scatter(const uint64_t *__restrict__ entries, const uint32_t *__restrict__ offsets, size_t n,
-                          int w0, int w1, uint32_t nbuckets, uint32_t *__restrict__ sorted, size_t flat /* table stride, 0 = off */)
-{
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    for (int w = w0; w < w1; w++) {
-        uint64_t e = entries[(size_t)w * n + i];
-        int32_t d = (int32_t)(e >> 32);
-        if (d == 0) continue;
-        uint32_t neg = d < 0, bkt = (uint32_t)(neg ? -d : d) - 1;
-        if (flat) {
-            uint32_t pos = offsets[bkt] + (uint32_t)e;
-            sorted[pos] = (uint32_t)((size_t)w * flat + i) | (neg << 31);
-        } else {
-            uint32_t pos = offsets[(size_t)w * nbuckets + bkt] + (uint32_t)e;
-            sorted[(size_t)w * n + pos] = (uint32_t)i | (neg << 31);
-        }
-    }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -842,6 +1084,18 @@ k_combine(const ge_p3_raw *__restrict__ windows, int ranks, int nwin, int c, Msm
     res->pad = 0;
 }
 
+// Fine bits F of the digit sort: as few coarse bins per window as keep their mean size on uniform digits near
+// SORT_BIN_MEAN (half of what k_sort_fine holds in shared memory), within the shared histograms' sizes.
+// c = 16, 2^20 pairs: F = 7, 256 coarse bins of 128 buckets per window.
+static int msm_sort_fine_bits(size_t entries_per_window, int c, int hist_windows)
+{
+    int lg = std::max(0, c - 1 - SORT_FINE_MAX);            // log2 of the coarse bins per window
+    while (lg < c - 1 && ((size_t)SORT_BIN_MEAN << lg) < entries_per_window && (2u << lg) <= SORT_NC_MAX &&
+           ((size_t)hist_windows << (lg + 1)) <= SORT_HIST_MAX)
+        lg++;
+    return c - 1 - lg;
+}
+
 // ------------------------------------------------------------------------------------------
 // One chunk of (scalar, point) pairs: digits, counting sort, task lists and bucket accumulation.
 // `first` chunks start the buckets at the identity; later chunks add onto them.  All chunks of one
@@ -863,41 +1117,57 @@ int msm_accumulate_chunk(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const g
     const size_t max_tasks = total_buckets + (std::max<size_t>(1, n) * nact) / task_len + 1;
     const size_t max_heavy = (std::max<size_t>(1, n) * nact) / task_len + 1;
     const uint32_t parts = (nb + SCAN_PART - 1) / SCAN_PART;
+    const int F = msm_sort_fine_bits(flat ? n * (size_t)nact : n, c, flat ? 1 : nact);
+    const uint32_t nc = nb >> F;                                  // coarse bins per bucket window
     cudaStream_t st = ctx->stream;
     int rc;
-    // counts | heavy list (count + entries): one memset clears both
-    if ((rc = ws_reserve(ctx, ctx->counts, total_buckets * 4 + (1 + max_heavy) * 4))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->offsets, total_buckets * 4 + (size_t)nwin * parts * 4))) return rc;
+    // counts | coarse counts | heavy list (count + entries): one memset clears the coarse counts and the heavy count
+    if ((rc = ws_reserve(ctx, ctx->counts, (total_buckets + (size_t)nwin * nc + 1 + max_heavy) * 4))) return rc;
+    // offsets | scan part sums | coarse bin cursors | extra-slice prefix of the bins | extra slices per window
+    if ((rc = ws_reserve(ctx, ctx->offsets, (total_buckets + (size_t)nwin * parts + 2 * (size_t)nwin * nc + nwin) * 4))) return rc;
     if ((rc = ws_reserve(ctx, ctx->ntasks, total_buckets * 4))) return rc;
     if ((rc = ws_reserve(ctx, ctx->task_off, total_buckets * 4 + (nwin + 1) * 4))) return rc;
     if ((rc = ws_reserve(ctx, ctx->tasks, max_tasks * 8))) return rc;
     if ((rc = ws_reserve(ctx, ctx->task_sums, max_tasks * sizeof(ge_p3_raw)))) return rc;
     if ((rc = ws_reserve(ctx, ctx->task_order, (3 * TASK_BINS + max_tasks) * 4))) return rc;   // hist | cursor | start | order
+    // the sort's records: 8 B per non-zero digit, in (bucket window, coarse bin) order
     if ((rc = ws_reserve(ctx, ctx->digits, std::max<size_t>(1, n) * nact * 8))) return rc;
     if ((rc = ws_reserve(ctx, ctx->sorted, std::max<size_t>(1, n) * nact * 4))) return rc;
     if ((rc = ws_reserve(ctx, ctx->buckets, total_buckets * sizeof(ge_p3_raw)))) return rc;
     uint32_t *counts = (uint32_t *)ctx->counts.p, *offsets = (uint32_t *)ctx->offsets.p;
     uint32_t *ntasks = (uint32_t *)ctx->ntasks.p, *task_off = (uint32_t *)ctx->task_off.p;
     uint32_t *win_base = task_off + total_buckets;
-    uint32_t *heavy = counts + total_buckets;
-    uint32_t *part_sums = offsets + total_buckets;
+    uint32_t *ccount = counts + total_buckets, *heavy = ccount + (size_t)nwin * nc;
+    uint32_t *part_sums = offsets + total_buckets, *ccursor = part_sums + (size_t)nwin * parts;
+    uint32_t *xpre = ccursor + (size_t)nwin * nc, *xtot = xpre + (size_t)nwin * nc;
     uint2 *tasks = (uint2 *)ctx->tasks.p;
     uint32_t *t_hist = (uint32_t *)ctx->task_order.p, *t_cursor = t_hist + TASK_BINS, *t_start = t_cursor + TASK_BINS;
     uint32_t *order = t_start + TASK_BINS;
     ge_p3_raw *task_sums = (ge_p3_raw *)ctx->task_sums.p;
-    uint64_t *entries = (uint64_t *)ctx->digits.p;
+    uint2 *records = (uint2 *)ctx->digits.p;
     uint32_t *sorted = (uint32_t *)ctx->sorted.p;
     ge_p3_raw *buckets = (ge_p3_raw *)ctx->buckets.p;
 
-    CUDA_TRY(ctx, cudaMemsetAsync(counts, 0, (total_buckets + 1) * 4, st));
+    const size_t part_smem = SORT_TILE * 8 + (2 * (size_t)nc + 33) * 4;
+    const size_t fine_smem = SORT_FINE_CAP * 12 + ((1u << F) + 33) * 4;
+    CUDA_TRY(ctx, cudaFuncSetAttribute(k_sort_partition, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)part_smem));
+    CUDA_TRY(ctx, cudaFuncSetAttribute(k_sort_fine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fine_smem));
+    CUDA_TRY(ctx, cudaMemsetAsync(ccount, 0, ((size_t)nwin * nc + 1) * 4, st));
     CUDA_TRY(ctx, cudaMemsetAsync(t_hist, 0, 2 * TASK_BINS * 4, st));
     if (n) {
-        k_digits<<<cdiv(n, 256), 256, 0, st>>>((const uint4 *)d_scalars, n, c, nact, nb, counts, entries, flat ? 1 : 0);
+        k_sort_count<<<cdiv(n, SORT_COUNT_TILE), SORT_THREADS, 0, st>>>((const uint4 *)d_scalars, n, c, nact, F, nc, flat ? 1 : 0, ccount);
         ctx->launches++;
     }
-    k_scan_partial<<<nwin * parts, 1024, 0, st>>>(counts, nb, parts, part_sums);
-    k_scan_bases<<<nwin, 32, 0, st>>>(part_sums, parts);
-    k_scan_apply<<<nwin * parts, 1024, 0, st>>>(counts, part_sums, nb, parts, offsets);
+    // ntasks is free until k_task_count: it holds the fill counters of the big bins' buckets
+    k_sort_bins_scan<<<nwin, SORT_THREADS, 0, st>>>(ccount, nc, F, nb, ccursor, xpre, xtot, counts, ntasks);
+    if (n) {
+        k_sort_partition<<<cdiv(n, SORT_TILE), SORT_THREADS, part_smem, st>>>((const uint4 *)d_scalars, n, c, nact, F, nc, nb, flat,
+                                                                              ccount, ccursor, records, counts);
+        ctx->launches++;
+    }
+    const size_t extra = n * (size_t)nact / SORT_FINE_CAP;          // bounds the extra slices of all big bins
+    k_sort_fine<<<(unsigned)(nwin * nc + extra), SORT_THREADS, fine_smem, st>>>(records, ccount, ccursor, xpre, xtot, n, F, nc, nb,
+                                                                               (uint32_t)nwin, flat ? 1 : 0, counts, offsets, sorted, ntasks);
     k_task_count<<<cdiv(total_buckets, 256), 256, 0, st>>>(counts, (uint32_t)total_buckets, task_len, ntasks, heavy);
     k_scan_partial<<<nwin * parts, 1024, 0, st>>>(ntasks, nb, parts, part_sums);
     k_scan_bases<<<nwin, 32, 0, st>>>(part_sums, parts);
@@ -907,14 +1177,7 @@ int msm_accumulate_chunk(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const g
     k_task_hist<<<cdiv(max_tasks, 256), 256, 0, st>>>(tasks, counts, win_base + nwin, task_len, t_hist);
     k_task_scan<<<1, 256, 0, st>>>(t_hist, t_start);
     k_task_scatter<<<cdiv(max_tasks, 256), 256, 0, st>>>(tasks, counts, win_base + nwin, task_len, t_start, t_cursor, order);
-    ctx->launches += 12;
-    if (n) {
-        const int wg = (int)std::max<size_t>(1, std::min<size_t>((size_t)nact, (ctx->l2_bytes / 2) / (n * 4)));
-        for (int w0 = 0; w0 < nact; w0 += wg) {
-            k_scatter<<<cdiv(n, 256), 256, 0, st>>>(entries, offsets, n, w0, std::min(nact, w0 + wg), nb, sorted, flat);
-            ctx->launches++;
-        }
-    }
+    ctx->launches += 11;
     // the digit / sort passes above only read the scalars: the conversion of the points may still be running on another stream
     if (points_ready) CUDA_TRY(ctx, cudaStreamWaitEvent(st, points_ready, 0));
     if (first) CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, st));
