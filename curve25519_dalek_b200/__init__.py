@@ -14,6 +14,9 @@ touches the CPU checker used by the tests.  Names follow the reference:
   EdwardsPoint.hash_to_curve_batch / encode_to_curve_batch (src/edwards.rs:710-750, RFC 9380)
   ed25519_verifying_keys / ed25519_sign / ed25519_sign_prehashed / ed25519_verify_prehashed
       (ed25519-dalek/src/signing.rs:106-171, :312, :566-571; src/verifying.rs:230-257, :424-459)
+  EdwardsPoint.mul_batch / mul_clamped_batch / is_small_order_batch / is_torsion_free_batch and RistrettoPoint.mul_batch
+      (src/edwards.rs:890-941, :1405-1437; src/ristretto.rs:917-926): constant-time s * P per item, one scalar or one
+      point broadcast to the whole batch
 """
 from .engine import (Engine, MultiEngine, EngineError, EdwardsPoint, RistrettoPoint, SignatureError, verify_batch, default_engine,
                      library_path, load_library, POINTS_COMPRESSED, POINTS_EXTENDED, POINTS_RISTRETTO,

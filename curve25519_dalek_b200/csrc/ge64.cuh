@@ -72,7 +72,9 @@ FE_HD void ge64_padd(ge64_p3 &r, const ge64_p3 &p, const ge64_pniels &q, uint32_
     ge64_add_tail(r, a, b, c, D, neg);
 }
 
-// r = 2p (curve_models.rs:381-397 followed by :365-372).   4S + 4M, two balanced carries
+// r = 2p (curve_models.rs:381-397 followed by :365-372).   4S + 4M, two balanced carries.  T_OUT = false leaves r.T
+// unset (4S + 3M, the projective result of :357-363), for a doubling that only another doubling reads.
+template <bool T_OUT = true>
 FE_HD void ge64_dbl(ge64_p3 &r, const ge64_p3 &p)
 {
     FE64_ASSERT_SCALE(p.X, 1); FE64_ASSERT_SCALE(p.Y, 1); FE64_ASSERT_SCALE(p.Z, 1);
@@ -90,7 +92,7 @@ FE_HD void ge64_dbl(ge64_p3 &r, const ge64_p3 &p)
     fe64_mul(r.X, E, F);                                // 3 x 1
     fe64_mul(r.Y, Yp, Ym);                              // 2 x 2
     fe64_mul(r.Z, Ym, F);                               // 2 x 1
-    fe64_mul(r.T, E, Yp);                               // 3 x 2
+    if (T_OUT) fe64_mul(r.T, E, Yp);                    // 3 x 2
 }
 
 // r = p + q for two extended points on the FP64 field: q -> projective Niels on the fly (edwards.rs:528-535), 9M;

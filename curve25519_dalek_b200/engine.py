@@ -95,6 +95,9 @@ def load_library():
     lib.dalek_b200_x25519_batch.argtypes = [vp, vp, vp, sz, vp, vp]
     lib.dalek_b200_x25519_batch_dev.argtypes = [vp, vp, vp, sz, vp, vp]
     lib.dalek_b200_x25519_public_keys.argtypes = [vp, vp, sz, vp]
+    lib.dalek_b200_mul_batch.argtypes = [vp, vp, sz, vp, C.c_int, sz, sz, C.c_int, vp, vp]
+    lib.dalek_b200_mul_batch_dev.argtypes = [vp, vp, sz, vp, C.c_int, sz, sz, C.c_int, vp, vp]
+    lib.dalek_b200_edwards_torsion_batch.argtypes = [vp, vp, C.c_int, sz, vp]
     lib.dalek_b200_ristretto_from_uniform_bytes_batch.argtypes = [vp, vp, sz, vp]
     lib.dalek_b200_ristretto_hash_from_bytes_batch.argtypes = [vp, vp, vp, sz, vp]
     lib.dalek_b200_edwards_hash_to_curve_batch.argtypes = [vp, vp, vp, sz, vp, sz, vp]
@@ -335,6 +338,38 @@ class Engine:
         self._check(self.lib.dalek_b200_x25519_public_keys(self.h, _ptr(scalars), n, C.addressof(out)))
         return bytes(out)[:32 * n]
 
+    # ---- variable-base scalar multiplication ----
+    def mul_batch(self, scalars, n_scalars, points, n_points, n, point_fmt=POINTS_COMPRESSED, clamped=False, device_ptrs=False,
+                  out=None, want_ok=False):
+        """out[i] = s_i * P_i for n items (dalek_b200_mul_batch): n_scalars and n_points are each 1 (broadcast) or n.
+        Returns (rc, out, ok or None); rc 1 (DALEK_NONE) when a point does not decode (its ok byte is 0 and its slot holds
+        the identity).  Host buffers give bytes.  With device_ptrs the inputs are device buffers and the results go to
+        `out` (32 n bytes) and, with want_ok, an n-byte ok buffer on the engine's device, new uint8 tensors if not given."""
+        flags = 1 if clamped else 0
+        if device_ptrs:
+            ok = None
+            if out is None or want_ok:
+                import torch
+                dev = torch.device("cuda", self.device)
+                if out is None:
+                    out = torch.empty(32 * max(n, 1), dtype=torch.uint8, device=dev)
+                if want_ok:
+                    ok = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+            rc = self._check(self.lib.dalek_b200_mul_batch_dev(self.h, _ptr(scalars), n_scalars, _ptr(points), point_fmt, n_points, n,
+                                                               flags, _ptr(out), _ptr(ok)))
+            return rc, out, ok
+        res = (C.c_uint8 * (32 * max(n, 1)))() if out is None else out
+        ok = (C.c_uint8 * max(n, 1))() if want_ok else None
+        rc = self._check(self.lib.dalek_b200_mul_batch(self.h, _ptr(scalars), n_scalars, _ptr(points), point_fmt, n_points, n, flags,
+                                                       _ptr(res), C.addressof(ok) if want_ok else None))
+        return rc, (bytes(res)[:32 * n] if out is None else out), (bytes(ok)[:n] if want_ok else None)
+
+    def torsion_batch(self, points, n, point_fmt=POINTS_COMPRESSED):
+        """is_small_order | is_torsion_free << 1 | decoded << 2 per Edwards point (0 for an undecodable one), as bytes."""
+        out = (C.c_uint8 * max(n, 1))()
+        self._check(self.lib.dalek_b200_edwards_torsion_batch(self.h, _ptr(points), point_fmt, n, C.addressof(out)))
+        return bytes(out)[:n]
+
     # ---- hash to group ----
     def ristretto_from_uniform_bytes_batch(self, data, n):
         """RistrettoPoint::from_uniform_bytes for n x 64 B -> n x 32 B CompressedRistretto."""
@@ -569,6 +604,28 @@ class EdwardsPoint:
         return [raw[32 * i:32 * i + 32] for i in range(n)]
 
     @staticmethod
+    def mul_batch(scalars, points, engine=None):
+        """EdwardsPoint * Scalar (edwards.rs:890-899) for each pair of a 32-byte scalar (bit 255 clear) and a 32-byte
+        CompressedEdwardsY; a single scalar or a single point is used for every item.  Returns the CompressedEdwardsY of
+        the product, or the list.  An undecodable point raises ValueError."""
+        return _mul_batch(scalars, points, POINTS_COMPRESSED, False, engine)
+
+    @staticmethod
+    def mul_clamped_batch(bytes_list, points, engine=None):
+        """EdwardsPoint::mul_clamped (edwards.rs:932-941): any 32 bytes, clamped and not reduced; broadcast as mul_batch."""
+        return _mul_batch(bytes_list, points, POINTS_COMPRESSED, True, engine)
+
+    @staticmethod
+    def is_small_order_batch(points, engine=None):
+        """EdwardsPoint::is_small_order (edwards.rs:1405-1407) of each CompressedEdwardsY: a list of bool."""
+        return [bool(f & 1) for f in _torsion_flags(points, engine)]
+
+    @staticmethod
+    def is_torsion_free_batch(points, engine=None):
+        """EdwardsPoint::is_torsion_free (edwards.rs:1435-1437) of each CompressedEdwardsY: a list of bool."""
+        return [bool(f & 2) for f in _torsion_flags(points, engine)]
+
+    @staticmethod
     def hash_to_curve_batch(messages, dst, engine=None):
         """EdwardsPoint::hash_to_curve::<Sha512> (edwards.rs:736-750, RFC 9380 edwards25519_XMD:SHA-512_ELL2_RO_) for each
         message, with one domain separation tag of 1..255 bytes: the list of 32-byte CompressedEdwardsY encodings."""
@@ -584,6 +641,35 @@ class EdwardsPoint:
         flat, offs, n = _flat_messages(messages)
         raw = eng.edwards_encode_to_curve_batch(flat, offs, n, dst)
         return [raw[32 * i:32 * i + 32] for i in range(n)]
+
+
+def _mul_batch(scalars, points, fmt, clamped, engine):
+    single_s, ss = _items(scalars, 32, "scalars")
+    single_p, ps = _items(points, 32, "points")
+    if not single_s and not single_p and len(ss) != len(ps):
+        raise ValueError("scalars and points must have the same length (or one of them be a single item)")
+    n = len(ps) if single_s else len(ss)
+    if n == 0:
+        return []
+    if not clamped and any(s[31] & 0x80 for s in ss):
+        raise ValueError("a scalar has bit 255 set")
+    eng = engine or default_engine()
+    rc, raw, _ = eng.mul_batch(b"".join(ss), len(ss), b"".join(ps), len(ps), n, fmt, clamped=clamped)
+    if rc == 1:
+        raise ValueError("a point does not decode")
+    outs = [raw[32 * i:32 * i + 32] for i in range(n)]
+    return outs[0] if single_s and single_p else outs
+
+
+def _torsion_flags(points, engine):
+    _, ps = _items(points, 32, "points")
+    if not ps:
+        return []
+    eng = engine or default_engine()
+    flags = eng.torsion_batch(b"".join(ps), len(ps))
+    if any(f == 0 for f in flags):
+        raise ValueError("a point does not decode")
+    return flags
 
 
 def _flat_messages(messages):
@@ -807,6 +893,13 @@ class RistrettoPoint:
         if rc == 1:
             raise ValueError("G or H is not a valid Ristretto encoding")
         return out
+
+    @staticmethod
+    def mul_batch(scalars, points, engine=None):
+        """RistrettoPoint * Scalar (ristretto.rs:917-926) for each pair of a 32-byte scalar (bit 255 clear) and a 32-byte
+        CompressedRistretto; a single scalar or a single point is used for every item.  Returns the CompressedRistretto
+        of the product, or the list.  An undecodable point raises ValueError."""
+        return _mul_batch(scalars, points, POINTS_RISTRETTO, False, engine)
 
     @staticmethod
     def from_uniform_bytes_batch(data, engine=None):

@@ -51,7 +51,7 @@ typedef struct dalek_b200_ctx dalek_b200_ctx;
 
 #define DALEK_POINTS_COMPRESSED 0         /* n x 32 B CompressedEdwardsY */
 #define DALEK_POINTS_EXTENDED 1           /* n x 20 x u64 radix-2^51 limbs */
-#define DALEK_POINTS_RISTRETTO 2          /* n x 32 B CompressedRistretto (precomputation API only) */
+#define DALEK_POINTS_RISTRETTO 2          /* n x 32 B CompressedRistretto (precomputation API and variable-base multiplication) */
 
 /* -------- context ---------------------------------------------------------------------- */
 /* Create an engine context on CUDA device `device`.  Fails (no CPU fallback) if the device
@@ -85,7 +85,7 @@ int dalek_b200_last_kernel_ms(const dalek_b200_ctx *ctx, float *ms, int *launche
  * verify_batch call, the largest kernel of that path; summed over the pieces of a host-streamed call). */
 int dalek_b200_last_stage_ms(const dalek_b200_ctx *ctx, const char *stage, float *ms);
 /* Milliseconds between CUDA events recorded on the context's stream at entry of the last MSM / verify_batch /
- * precomputed-MSM / X25519 / to_montgomery_batch / hash-to-group call, or of the last ed25519_b200_verifying_keys /
+ * precomputed-MSM / X25519 / to_montgomery_batch / hash-to-group / mul_batch call, or of the last ed25519_b200_verifying_keys /
  * sign_flat / sign_prehashed / verify_prehashed_each call, and after the last work it enqueued (all of the call's streams
  * joined): the device time of that call, copies of host-buffer calls included. */
 int dalek_b200_last_call_ms(const dalek_b200_ctx *ctx, float *ms);
@@ -242,6 +242,36 @@ int dalek_b200_x25519_batch_dev(dalek_b200_ctx *ctx, const void *d_scalars, cons
                                 void *d_out, void *d_contributory);
 /* PublicKey::from(&StaticSecret) = mul_base_clamped(k).to_montgomery(); out: n x 32 B */
 int dalek_b200_x25519_public_keys(dalek_b200_ctx *ctx, const uint8_t *scalars, size_t n, uint8_t *out);
+
+/* -------- variable-base scalar multiplication -------------------------------------------------
+ * out[i] = s_i * P_i: EdwardsPoint * Scalar (C/edwards.rs:890-899 -> C/backend/serial/scalar_mul/variable_base.rs:11-48),
+ * EdwardsPoint::mul_clamped (C/edwards.rs:932-941) and RistrettoPoint * Scalar (C/ristretto.rs:917-926); with one point
+ * for the whole batch also BasepointTable::create(P) * s and mul_base_clamped (C/edwards.rs:1140-1230,
+ * C/ristretto.rs:1086-1103), which give the same points.
+ *   Broadcast: n_scalars and n_points are each 1 or n; 1 uses that input for every item, any other value is
+ *     DALEK_E_INVALID_ARG.  n = 0 is a successful no-op.  A NULL buffer with n > 0 is DALEK_E_INVALID_ARG, except ok.
+ *   Point formats: COMPRESSED (CompressedEdwardsY in and out), EXTENDED (20 radix-2^51 limbs in, any Z;
+ *     CompressedEdwardsY out), RISTRETTO (CompressedRistretto in and out, C/ristretto.rs:500-533).
+ *   An undecodable point gives ok[i] = 0 and the identity's encoding in its slot, and the call returns DALEK_NONE, as
+ *     dalek_b200_edwards_decompress_batch does; every other ok[i] is 1.
+ *   Scalars: 32 bytes little-endian with bit 255 clear (Scalar invariant #1, as in dalek_b200_edwards_ct_msm), else
+ *     DALEK_E_INVALID_ARG.  With flags = DALEK_MUL_CLAMPED any 32 bytes are accepted, clamped inside the call
+ *     (clamp_integer, C/scalar.rs:1407-1412) and not reduced; the reference has no clamped Ristretto multiplication,
+ *     so DALEK_MUL_CLAMPED with RISTRETTO is DALEK_E_INVALID_ARG.  Other flag bits are DALEK_E_INVALID_ARG.
+ *   Constant time in the scalars: no branch, loop bound or address depends on them (masked full scans of 8-entry
+ *     tables and a masked sign, window.rs:54-76).  Host-buffer calls stream the batch in pieces like the codecs and
+ *     clear the device copies of the scalars and of the results before they return.  No option affects these calls. */
+#define DALEK_MUL_CLAMPED 1
+int dalek_b200_mul_batch(dalek_b200_ctx *ctx, const uint8_t *scalars, size_t n_scalars, const void *points, int point_fmt,
+                         size_t n_points, size_t n, int flags, uint8_t *out /* n x 32 B */, uint8_t *ok /* n bytes, nullable */);
+/* same, every buffer a device pointer; blocks until done.  A scalar with bit 255 set (without the clamp flag) is
+ * reported after the batch ran: the call returns DALEK_E_INVALID_ARG and the outputs are unspecified. */
+int dalek_b200_mul_batch_dev(dalek_b200_ctx *ctx, const void *d_scalars, size_t n_scalars, const void *d_points, int point_fmt,
+                             size_t n_points, size_t n, int flags, void *d_out, void *d_ok);
+/* out[i] = is_small_order(P_i) | is_torsion_free(P_i) << 1 | decoded << 2 (C/edwards.rs:1405-1437; VerifyingKey::is_weak is
+ * is_small_order).  points: COMPRESSED or EXTENDED, anything else is DALEK_E_INVALID_ARG.  An undecodable point gives
+ * out[i] = 0; the call still returns DALEK_OK.  Host buffers, streamed in pieces. */
+int dalek_b200_edwards_torsion_batch(dalek_b200_ctx *ctx, const void *points, int point_fmt, size_t n, uint8_t *out);
 
 /* -------- hash to group ------------------------------------------------------------------------
  * Host buffers; each call blocks and streams the batch in pieces like the codecs.  The maps are total: these calls never
