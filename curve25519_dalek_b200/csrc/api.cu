@@ -59,7 +59,7 @@ void dalek_b200_destroy(dalek_b200_ctx *ctx)
     DevBuf *bufs[] = {&ctx->scalars, &ctx->points_in, &ctx->points, &ctx->digits, &ctx->counts, &ctx->offsets,
                       &ctx->sorted, &ctx->buckets, &ctx->red_a, &ctx->red_b, &ctx->red_c, &ctx->red_d, &ctx->key_pts,
                       &ctx->result, &ctx->flags, &ctx->misc0, &ctx->misc1, &ctx->misc2, &ctx->misc3,
-                      &ctx->misc4, &ctx->misc5, &ctx->zs, &ctx->base_table, &ctx->ntasks, &ctx->task_off, &ctx->tasks, &ctx->task_sums, &ctx->msg_offs, &ctx->sum_desc, &ctx->sum_part, &ctx->key_table, &ctx->key_acc, &ctx->task_order, &ctx->sig_status, &ctx->misc6, &ctx->each_pow, &ctx->each_tab, &ctx->each_kstat, &ctx->comb_base_table};
+                      &ctx->misc4, &ctx->misc5, &ctx->zs, &ctx->base_table, &ctx->ntasks, &ctx->task_off, &ctx->tasks, &ctx->task_sums, &ctx->msg_offs, &ctx->sum_desc, &ctx->sum_part, &ctx->key_table, &ctx->key_acc, &ctx->task_order, &ctx->sig_status, &ctx->misc6, &ctx->each_pow, &ctx->each_tab, &ctx->each_kstat, &ctx->comb_base_table, &ctx->prep_prod};
     for (DevBuf *b : bufs) if (b->p) cudaFree(b->p);
     if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
     cudaEventDestroy(ctx->ev_a); cudaEventDestroy(ctx->ev_b); cudaEventDestroy(ctx->ev_fork); cudaEventDestroy(ctx->ev_join);

@@ -58,6 +58,7 @@ struct dalek_b200_ctx {
     // device workspaces (grown on demand, reused across calls)
     DevBuf scalars, points_in, points, digits, counts, offsets, sorted, buckets, red_a, red_b, red_c,
         red_d, key_pts, result, flags, misc0, misc1, misc2, misc3, misc4, misc5, zs, base_table, ntasks, task_off, tasks, task_sums, msg_offs, sum_desc, sum_part, key_table, key_acc, task_order, sig_status, misc6, each_pow, each_tab, each_kstat;
+    DevBuf prep_prod;   // extended-point preparation: the Z product of each group of points (then its inverse), and running products
     uint32_t hash_seed[4] = {0x243F6A88u, 0x85A308D3u, 0x13198A2Eu, 0x03707344u};   // key of the public-key de-duplication hash, redrawn per context
     int sum_desc_c = -1;
     bool base_table_ready = false;
@@ -153,7 +154,8 @@ inline size_t msm_point_bytes(int point_fmt) { return point_fmt == DALEK_POINTS_
 
 // Convert n input points (device memory, format DALEK_POINTS_*) into packed Niels form.
 // Compressed Edwards and Ristretto inputs give affine Niels (decoding yields Z = 1) and set *d_bad (device int) nonzero
-// if any fails to decode.  Extended inputs give affine Niels too, normalised to Z = 1 with one inversion per 1024 points;
+// if any fails to decode.  Extended inputs give affine Niels too, normalised to Z = 1 with one inversion per call (three
+// launches on the given stream, with the context's prep_prod workspace);
 // with kind = PK_PNIELS they give projective Niels instead (no inversion, for the latency-bound Straus path).
 // msm_prepared_kind tells which kind a format and a requested kind give.
 int msm_prepare_points(dalek_b200_ctx *ctx, const void *d_in, int point_fmt, size_t n, void *d_out,

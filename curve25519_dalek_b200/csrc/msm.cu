@@ -103,14 +103,20 @@ __global__ void k_prep_ristretto(const uint32_t *__restrict__ in, ge_niels_packe
 // Extended points (X : Y : Z : T) -> affine Niels ((Y+X)/Z, (Y-X)/Z, 2d T/Z): the projective Niels point divided by Z,
 // so every input with Z != 0 stands for the same group element as before, T/Z = xy or not.  The bucket kernel then
 // adds every point with the 7M mixed addition in each of its ~16 windows instead of the 8M projective one, and
-// gathers 96 B per digit instead of 128 B.  The inversions use Montgomery's trick over the PREP_GROUP points of one
-// CTA (1024): a thread multiplies the Z of its PREP_PER_THREAD points, the lanes of a warp scan their products both ways
-// with shuffles, thread 0 inverts the product of the warp products (one inversion per CTA), and every thread then
-// walks its points backwards.  Z = 0 (not a point: bad limbs from the caller) is left out of the products, as
-// FieldElement::invert_batch skips zeros, and gives the identity; the other points of the group are unaffected.
-#define PREP_THREADS 128
-#define PREP_PER_THREAD 8
-#define PREP_GROUP (PREP_THREADS * PREP_PER_THREAD)      // points per inversion
+// gathers 96 B per digit instead of 128 B.  All the inversions are one Montgomery batch over the whole input, in three
+// short grid-wide passes over groups of PREP_GROUP points (one CTA per group):
+//   k_prep_zprod   the product of the Z of each group
+//   k_prep_invert  one CTA: the inverses of all the group products, with one field inversion
+//   k_prep_finish  each group again: the product of each thread's Z, its inverse from the group's inverse (Montgomery's
+//                  trick across the CTA), then every thread walks its points backwards and writes them
+// No CTA of the first and last pass waits on a serial inversion, so their CTAs are short and the digit sort of the main
+// stream gets SMs soon after it asks for them.  Z = 0 (not a point: bad limbs from the caller) is left out of the
+// products, as FieldElement::invert_batch skips zeros, and gives the identity; the other points of its group are
+// unaffected.
+#define PREP_THREADS 256
+#define PREP_PER_THREAD 4
+#define PREP_GROUP (PREP_THREADS * PREP_PER_THREAD)      // points per group: point k of thread t is base + k * PREP_THREADS + t
+#define PREP_NW (PREP_THREADS / 32)
 
 __device__ __forceinline__ void load_coord_f64(fe64 &h, const uint64_t *__restrict__ src)
 {
@@ -120,9 +126,25 @@ __device__ __forceinline__ void load_coord_f64(fe64 &h, const uint64_t *__restri
     fe t; fe_from_limbs51(t, l);
     fe64_from_fe_limbs(h, t);
 }
-__device__ __forceinline__ uint32_t fe64_nonzero(const fe64 &f)
+// the canonical 32 bytes of v if ok, else of the small constant c, to o[0], o[1]
+__device__ __forceinline__ void store_coord(uint4 *o, const fe64 &v, uint32_t ok, uint32_t c)
 {
-    fe t; fe64_to_fe(t, f);
+    fe f;
+    uint32_t w[8];
+    fe64_to_fe(f, v); fe_tobytes_words(w, f);
+#pragma unroll
+    for (int q = 0; q < 8; q++) w[q] = ok ? w[q] : (q == 0 ? c : 0u);
+    o[0] = make_uint4(w[0], w[1], w[2], w[3]);
+    o[1] = make_uint4(w[4], w[5], w[6], w[7]);
+}
+// Z of point i; returns 1 if it is non-zero mod p
+__device__ __forceinline__ uint32_t load_z(fe64 &h, const uint64_t *__restrict__ in, size_t i)
+{
+    uint64_t l[5];
+#pragma unroll
+    for (int k = 0; k < 5; k++) l[k] = __ldg(in + 20 * i + 10 + k);
+    fe t; fe_from_limbs51(t, l);
+    fe64_from_fe_limbs(h, t);
     return 1u - (uint32_t)fe_iszero(t);
 }
 __device__ __forceinline__ void fe64_shfl_up(fe64 &o, const fe64 &f, int d)
@@ -135,33 +157,32 @@ __device__ __forceinline__ void fe64_shfl_down(fe64 &o, const fe64 &f, int d)
 #pragma unroll
     for (int k = 0; k < 5; k++) o.v[k] = __shfl_down_sync(0xffffffffu, f.v[k], d);
 }
-
-__global__ void __launch_bounds__(PREP_THREADS, 3)
-k_prep_extended(const uint64_t *__restrict__ in, ge_niels_packed *__restrict__ out, size_t n)
+__device__ __forceinline__ void fe64_shfl_xor(fe64 &o, const fe64 &f, int m)
 {
-    constexpr int NW = PREP_THREADS / 32;
-    __shared__ fe64 s_warp[NW];                            // warp products, then their inverses
-    __shared__ fe64 s_pre[PREP_PER_THREAD][PREP_THREADS];  // running products, kept out of the registers
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const size_t g0 = (size_t)blockIdx.x * PREP_GROUP + tid;   // point k of this thread: g0 + k * PREP_THREADS
-    // running products pre[k] = Z_0 ... Z_k of this thread's points (zeros and points past n skipped)
-    fe64 acc;
-    uint32_t nz = 0;                                       // bit k: Z_k != 0
-    fe64_1(acc);
+#pragma unroll
+    for (int k = 0; k < 5; k++) o.v[k] = __shfl_xor_sync(0xffffffffu, f.v[k], m);
+}
+__device__ __forceinline__ void fe64_shfl_idx(fe64 &o, const fe64 &f, int src)
+{
+#pragma unroll
+    for (int k = 0; k < 5; k++) o.v[k] = __shfl_sync(0xffffffffu, f.v[k], src);
+}
+
+// p = the product of x over the first `width` lanes (a power of two), in each of them
+__device__ __forceinline__ void warp_product(fe64 &p, const fe64 &x, int width)
+{
+    fe64 t;
+    p = x;
 #pragma unroll 1
-    for (int k = 0; k < PREP_PER_THREAD; k++) {
-        const size_t i = g0 + (size_t)k * PREP_THREADS;
-        if (i < n) {
-            fe64 z, t;
-            load_coord_f64(z, in + 20 * i + 10);
-            const uint32_t ok = fe64_nonzero(z);
-            fe64_mul(t, acc, z); fe64_cmov(acc, t, ok);
-            nz |= ok << k;
-        }
-        s_pre[k][tid] = acc;
-    }
-    // products of the lanes below (lo) and above (hi) this one
-    fe64 lo = acc, hi = acc, t;
+    for (int m = width >> 1; m > 0; m >>= 1) { fe64_shfl_xor(t, p, m); fe64_mul(p, p, t); }
+}
+
+// Products of x over the other lanes of the warp: below = the lanes under this one, above = the lanes over it (1 if
+// none), all = the whole warp's, in every lane
+__device__ __forceinline__ void warp_other_products(const fe64 &x, fe64 &below, fe64 &above, fe64 &all)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    fe64 lo = x, hi = x, t;
 #pragma unroll 1
     for (int d = 1; d < 32; d <<= 1) {
         fe64_shfl_up(t, lo, d);
@@ -169,30 +190,110 @@ k_prep_extended(const uint64_t *__restrict__ in, ge_niels_packed *__restrict__ o
         fe64_shfl_down(t, hi, d);
         if (lane + d < 32) fe64_mul(hi, hi, t);
     }
-    if (lane == 31) s_warp[warp] = lo;
-    fe64_shfl_up(t, lo, 1); lo = t; if (lane == 0) fe64_1(lo);
-    fe64_shfl_down(t, hi, 1); hi = t; if (lane == 31) fe64_1(hi);
+    fe64_shfl_idx(all, lo, 31);
+    fe64_shfl_up(below, lo, 1); if (lane == 0) fe64_1(below);
+    fe64_shfl_down(above, hi, 1); if (lane == 31) fe64_1(above);
+}
+
+// Montgomery's trick across the CTA (blockDim.x a multiple of 32, at most 1024): every thread holds the product acc of
+// its own elements (never zero); inv = 1 / acc.  Two levels of warp_other_products, the lanes of each warp and then
+// the warp products in warp 0, around one inversion of the CTA's product (INVERT: warp 0 inverts it) or none (its
+// inverse is *tot_inv).  s_warp: one element per warp.
+template <bool INVERT>
+__device__ __forceinline__ void block_inverse(fe64 &inv, const fe64 &acc, fe64 *s_warp, const fe64 *tot_inv)
+{
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    fe64 below, above, all;
+    warp_other_products(acc, below, above, all);
+    if (lane == 0) s_warp[warp] = all;
     __syncthreads();
-    if (tid == 0) {                                        // Montgomery's trick on the NW warp products (never zero)
-        fe64 run[NW], inv;
-        run[0] = s_warp[0];
-#pragma unroll
-        for (int w = 1; w < NW; w++) fe64_mul(run[w], run[w - 1], s_warp[w]);
-        {   // on the integer field: the temporaries of the FP64 chain (fe64_pow22501) would make the kernel spill
-            fe q; fe64_to_fe(q, run[NW - 1]); fe_invert(q, q); fe64_from_fe_limbs(inv, q);
+    if (warp == 0) {
+        fe64 x, b, a, t;
+        if (lane < nw) x = s_warp[lane]; else fe64_1(x);
+        warp_other_products(x, b, a, all);
+        if (INVERT) {   // on the integer field: the temporaries of the FP64 chain (fe64_pow22501) would spill
+            fe q; fe64_to_fe(q, all); fe_invert(q, q); fe64_from_fe_limbs(t, q);
+        } else {
+            t = *tot_inv;
         }
-#pragma unroll
-        for (int w = NW - 1; w > 0; w--) {
-            fe64 iw;
-            fe64_mul(iw, inv, run[w - 1]);
-            fe64_mul(inv, inv, s_warp[w]);
-            s_warp[w] = iw;
-        }
-        s_warp[0] = inv;
+        fe64_mul(t, t, b); fe64_mul(t, t, a);
+        if (lane < nw) s_warp[lane] = t;
     }
     __syncthreads();
-    fe64 inv;                                              // 1 / pre[PREP_PER_THREAD - 1]
-    fe64_mul(inv, s_warp[warp], lo); fe64_mul(inv, inv, hi);
+    fe64_mul(inv, s_warp[warp], below); fe64_mul(inv, inv, above);
+}
+
+// Pass 1: prod[g] = the product of the non-zero Z of group g
+__global__ void __launch_bounds__(PREP_THREADS, 2)
+k_prep_zprod(const uint64_t *__restrict__ in, fe64 *__restrict__ prod, size_t n)
+{
+    __shared__ fe64 s_warp[PREP_NW];
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const size_t g0 = (size_t)blockIdx.x * PREP_GROUP + tid;
+    fe64 z[PREP_PER_THREAD], acc, t;
+    uint32_t ok[PREP_PER_THREAD];
+#pragma unroll
+    for (int k = 0; k < PREP_PER_THREAD; k++) {           // every load is issued before the first multiplication
+        const size_t i = g0 + (size_t)k * PREP_THREADS;
+        if (i < n) ok[k] = load_z(z[k], in, i); else { ok[k] = 0; fe64_1(z[k]); }
+    }
+    acc = z[0];
+    if (!ok[0]) fe64_1(acc);
+#pragma unroll
+    for (int k = 1; k < PREP_PER_THREAD; k++) { fe64_mul(t, acc, z[k]); fe64_cmov(acc, t, ok[k]); }
+    warp_product(t, acc, 32);
+    if (lane == 0) s_warp[warp] = t;
+    __syncthreads();
+    if (warp == 0) {
+        if (lane < PREP_NW) acc = s_warp[lane]; else fe64_1(acc);
+        warp_product(t, acc, PREP_NW);
+        if (lane == 0) prod[blockIdx.x] = t;
+    }
+}
+
+// Pass 2, one CTA: prod[g] <- 1 / prod[g] for all G groups.  Thread t takes a run of consecutive products
+// (running products in pre[]), and block_inverse makes the one inversion.
+__global__ void __launch_bounds__(PREP_THREADS)
+k_prep_invert(fe64 *__restrict__ prod, fe64 *__restrict__ pre, uint32_t G)
+{
+    __shared__ fe64 s_warp[PREP_NW];
+    const uint32_t per = (G + blockDim.x - 1) / blockDim.x, b = min(threadIdx.x * per, G), e = min(b + per, G);
+    fe64 acc, inv, t;
+    fe64_1(acc);
+    for (uint32_t k = b; k < e; k++) { fe64_mul(acc, acc, prod[k]); pre[k] = acc; }
+    block_inverse<true>(inv, acc, s_warp, nullptr);
+    for (uint32_t k = e; k-- > b;) {                      // invariant: inv = 1 / pre[k]
+        const fe64 x = prod[k];
+        if (k > b) fe64_mul(t, inv, pre[k - 1]); else t = inv;
+        prod[k] = t;
+        fe64_mul(inv, inv, x);
+    }
+}
+
+// Pass 3: every point of group g from the group's inverse ginv[g]
+__global__ void __launch_bounds__(PREP_THREADS, 2)
+k_prep_finish(const uint64_t *__restrict__ in, const fe64 *__restrict__ ginv, ge_niels_packed *__restrict__ out, size_t n)
+{
+    __shared__ fe64 s_warp[PREP_NW];
+    __shared__ fe64 s_pre[PREP_PER_THREAD - 1][PREP_THREADS];   // running products but the last, kept out of the registers
+    const uint32_t tid = threadIdx.x;
+    const size_t g0 = (size_t)blockIdx.x * PREP_GROUP + tid;
+    // running products pre[k] = Z_0 ... Z_k of this thread's points (zeros and points past n skipped)
+    fe64 acc, inv;
+    uint32_t nz = 0;                                       // bit k: Z_k != 0
+    fe64_1(acc);
+#pragma unroll 1
+    for (int k = 0; k < PREP_PER_THREAD; k++) {
+        const size_t i = g0 + (size_t)k * PREP_THREADS;
+        if (k > 0) s_pre[k - 1][tid] = acc;
+        if (i < n) {
+            fe64 z, t;
+            const uint32_t ok = load_z(z, in, i);
+            fe64_mul(t, acc, z); fe64_cmov(acc, t, ok);
+            nz |= ok << k;
+        }
+    }
+    block_inverse<false>(inv, acc, s_warp, ginv + blockIdx.x);   // 1 / pre[PREP_PER_THREAD - 1]
 #pragma unroll 1
     for (int k = PREP_PER_THREAD - 1; k >= 0; k--) {       // invariant: inv = 1 / pre[k]
         const size_t i = g0 + (size_t)k * PREP_THREADS;
@@ -200,25 +301,20 @@ k_prep_extended(const uint64_t *__restrict__ in, ge_niels_packed *__restrict__ o
         const uint32_t ok = (nz >> k) & 1u;
         const uint64_t *src = in + 20 * i;
         fe64 X, Y, zi, u, v;
-        load_coord_f64(u, src + 10);
+        load_coord_f64(u, src + 10);                       // Z_k again (the forward loop above read it)
         if (k > 0) fe64_mul(zi, inv, s_pre[k - 1][tid]); else zi = inv;   // 1 / Z_k
         fe64_mul(v, inv, u); fe64_cmov(inv, v, ok);
-        // each coordinate goes to its canonical bytes as soon as it is made (fewer live registers)
-        ge_niels_packed pk;
-        fe f;
+        // each coordinate goes to its canonical bytes, and out, as soon as it is made (fewer live registers); Z = 0
+        // gives the identity (1, 1, 0)
+        uint4 *o = reinterpret_cast<uint4 *>(out + i);
         load_coord_f64(X, src); load_coord_f64(Y, src + 5);
         fe64_add(u, Y, X); fe64_mul(v, u, zi);                         // 2 x 1
-        fe64_to_fe(f, v); fe_tobytes_words(pk.w, f);
+        store_coord(o, v, ok, 1u);
         fe64_sub(u, Y, X); fe64_mul(v, u, zi);
-        fe64_to_fe(f, v); fe_tobytes_words(pk.w + 8, f);
+        store_coord(o + 2, v, ok, 1u);
         load_coord_f64(u, src + 15);
         fe64_mul(v, u, zi); fe64_const_2d(u); fe64_mul(v, v, u);
-        fe64_to_fe(f, v); fe_tobytes_words(pk.w + 16, f);
-#pragma unroll
-        for (int q = 0; q < 24; q++) pk.w[q] = ok ? pk.w[q] : (q == 0 || q == 8 ? 1u : 0u);   // Z = 0: the identity (1, 1, 0)
-        uint4 *o = reinterpret_cast<uint4 *>(out + i);
-#pragma unroll
-        for (int q = 0; q < 6; q++) o[q] = make_uint4(pk.w[4 * q], pk.w[4 * q + 1], pk.w[4 * q + 2], pk.w[4 * q + 3]);
+        store_coord(o + 4, v, ok, 0u);
     }
 }
 
@@ -259,7 +355,16 @@ int msm_prepare_points_on(dalek_b200_ctx *ctx, cudaStream_t st, const void *d_in
     } else if (kind == PK_PNIELS) {
         k_prep_extended_pniels<<<cdiv(n, 128), 128, 0, st>>>((const uint64_t *)d_in, (ge_pniels_packed *)d_out, n);
     } else {
-        k_prep_extended<<<cdiv(n, PREP_GROUP), PREP_THREADS, 0, st>>>((const uint64_t *)d_in, (ge_niels_packed *)d_out, n);
+        // one workspace per context: the calls that prepare points (one per chunk of a host-buffer call) follow each
+        // other on one stream
+        const unsigned G = cdiv(n, PREP_GROUP);
+        int rc;
+        if ((rc = ws_reserve(ctx, ctx->prep_prod, 2 * (size_t)G * sizeof(fe64)))) return rc;
+        fe64 *prod = (fe64 *)ctx->prep_prod.p;
+        k_prep_zprod<<<G, PREP_THREADS, 0, st>>>((const uint64_t *)d_in, prod, n);
+        k_prep_invert<<<1, PREP_THREADS, 0, st>>>(prod, prod + G, G);
+        k_prep_finish<<<G, PREP_THREADS, 0, st>>>((const uint64_t *)d_in, prod, (ge_niels_packed *)d_out, n);
+        ctx->launches += 2;
     }
     ctx->launches++;
     CUDA_TRY(ctx, cudaGetLastError());

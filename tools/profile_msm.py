@@ -1,7 +1,10 @@
 """Per-kernel breakdown of ONE steady-state, device-resident MSM call over 2^20 extended points (the flagship
 workload of bench.py), captured with torch.profiler (CUDA activities).  Run on the H100:
 
-    python tools/profile_msm.py OUT.json [log2n]
+    python tools/profile_msm.py OUT.json [log2n] [--prep-alone]
+
+--prep-alone profiles the construction of a VartimeEdwardsPrecomputation over the same extended points instead: the
+point preparation then runs on the main stream with no sort kernels beside it (after the host-to-device copy).
 
 Prints and writes one JSON object: the card, and every kernel / memset / memcpy of the call with its stream, start
 offset from the first device activity of the call, and duration (microseconds).
@@ -18,16 +21,27 @@ from torch.profiler import ProfilerActivity, profile
 import curve25519_dalek_b200 as pkg
 import bench
 
-out_path = sys.argv[1]
-log2n = int(sys.argv[2]) if len(sys.argv) > 2 else 20
+args = [a for a in sys.argv[1:] if not a.startswith("--")]
+prep_alone = "--prep-alone" in sys.argv
+out_path = args[0]
+log2n = int(args[1]) if len(args) > 1 else 20
 n = 1 << log2n
 eng = pkg.Engine(0)
 wl = bench.MsmWorkload(eng, n, n, 0, torch)
+
+
+def step():
+    if prep_alone:
+        pkg.VartimeEdwardsPrecomputation((wl.h_points, n), engine=eng, fmt=pkg.POINTS_EXTENDED).close()
+    else:
+        wl.step_device_single()
+
+
 for _ in range(5):
-    wl.step_device_single()
+    step()
 torch.cuda.synchronize()
 with profile(activities=[ProfilerActivity.CUDA]) as prof:
-    wl.step_device_single()
+    step()
     torch.cuda.synchronize()
 
 rows = []
@@ -47,7 +61,10 @@ for r in rows:
     by_name[short] = round(by_name.get(short, 0.0) + r["dur_us"], 2)
 q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                    capture_output=True, text=True).stdout.strip()
-res = {"what": "one device-resident MSM call, 2^%d extended points (bench.MsmWorkload), after 5 warm-up calls" % log2n,
+what = ("the construction of a VartimeEdwardsPrecomputation over 2^%d extended points (bench.MsmWorkload's), after 5 "
+        "warm-up constructions" if prep_alone else "one device-resident MSM call, 2^%d extended points (bench.MsmWorkload), "
+        "after 5 warm-up calls") % log2n
+res = {"what": what,
        "timing": "torch.profiler, CUDA activities; start_us relative to the first device activity of the call",
        "device": q,
        "span_us": round(max(r["start_us"] + r["dur_us"] for r in rows), 2) if rows else 0,
