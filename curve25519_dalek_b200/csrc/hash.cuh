@@ -142,6 +142,45 @@ __device__ __forceinline__ void sha512_compress_regs(uint64_t h[8], uint64_t w[1
     h[0] += a; h[1] += b; h[2] += c; h[3] += d; h[4] += e; h[5] += f; h[6] += g; h[7] += hh;
 }
 
+// ---------------------------------------------------------------- SHA-256 (FIPS 180-4)
+static __device__ __constant__ uint32_t SHA256_K[64] = {
+    0x428a2f98u, 0x71374491u, 0xb5c0fbcfu, 0xe9b5dba5u, 0x3956c25bu, 0x59f111f1u, 0x923f82a4u, 0xab1c5ed5u,
+    0xd807aa98u, 0x12835b01u, 0x243185beu, 0x550c7dc3u, 0x72be5d74u, 0x80deb1feu, 0x9bdc06a7u, 0xc19bf174u,
+    0xe49b69c1u, 0xefbe4786u, 0x0fc19dc6u, 0x240ca1ccu, 0x2de92c6fu, 0x4a7484aau, 0x5cb0a9dcu, 0x76f988dau,
+    0x983e5152u, 0xa831c66du, 0xb00327c8u, 0xbf597fc7u, 0xc6e00bf3u, 0xd5a79147u, 0x06ca6351u, 0x14292967u,
+    0x27b70a85u, 0x2e1b2138u, 0x4d2c6dfcu, 0x53380d13u, 0x650a7354u, 0x766a0abbu, 0x81c2c92eu, 0x92722c85u,
+    0xa2bfe8a1u, 0xa81a664bu, 0xc24b8b70u, 0xc76c51a3u, 0xd192e819u, 0xd6990624u, 0xf40e3585u, 0x106aa070u,
+    0x19a4c116u, 0x1e376c08u, 0x2748774cu, 0x34b0bcb5u, 0x391c0cb3u, 0x4ed8aa4au, 0x5b9cca4fu, 0x682e6ff3u,
+    0x748f82eeu, 0x78a5636fu, 0x84c87814u, 0x8cc70208u, 0x90befffau, 0xa4506cebu, 0xbef9a3f7u, 0xc67178f2u};
+
+__device__ __forceinline__ uint32_t ror32(uint32_t x, int n) { return __funnelshift_r(x, x, n); }
+
+// One SHA-256 compression with the block in registers (16 big-endian words, static indices), as sha512_compress_regs.
+__device__ __forceinline__ void sha256_compress_regs(uint32_t h[8], uint32_t w[16])
+{
+    uint32_t a = h[0], b = h[1], c = h[2], d = h[3], e = h[4], f = h[5], g = h[6], hh = h[7];
+#pragma unroll 1
+    for (int r = 0; r < 64; r += 16) {
+#pragma unroll
+        for (int i = 0; i < 16; i++) {
+            if (r) {
+                uint32_t w15 = w[(i + 1) & 15], w2 = w[(i + 14) & 15];
+                uint32_t s0 = ror32(w15, 7) ^ ror32(w15, 18) ^ (w15 >> 3);
+                uint32_t s1 = ror32(w2, 17) ^ ror32(w2, 19) ^ (w2 >> 10);
+                w[i] = w[i] + s0 + w[(i + 9) & 15] + s1;
+            }
+            uint32_t S1 = ror32(e, 6) ^ ror32(e, 11) ^ ror32(e, 25);
+            uint32_t ch = (e & f) ^ (~e & g);
+            uint32_t t1 = hh + S1 + ch + SHA256_K[r + i] + w[i];
+            uint32_t S0 = ror32(a, 2) ^ ror32(a, 13) ^ ror32(a, 22);
+            uint32_t mj = (a & b) ^ (a & c) ^ (b & c);
+            uint32_t t2 = S0 + mj;
+            hh = g; g = f; f = e; e = d + t1; d = c; c = b; b = a; a = t1 + t2;
+        }
+    }
+    h[0] += a; h[1] += b; h[2] += c; h[3] += d; h[4] += e; h[5] += f; h[6] += g; h[7] += hh;
+}
+
 // A public prefix hashed before the register strings: Ed25519ph's dom2(1, C) = "SigEd25519 no Ed25519 collisions" || 1 ||
 // |C| || C (RFC 8032 5.1; ed25519-dalek signing.rs:945-951, verifying.rs:530-535), at most 34 + 255 bytes.  Travels as a
 // __grid_constant__ kernel parameter, like the DST of hash_to_curve.cu.

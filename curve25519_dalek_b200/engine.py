@@ -102,6 +102,10 @@ def load_library():
     lib.dalek_b200_ristretto_hash_from_bytes_batch.argtypes = [vp, vp, vp, sz, vp]
     lib.dalek_b200_edwards_hash_to_curve_batch.argtypes = [vp, vp, vp, sz, vp, sz, vp]
     lib.dalek_b200_edwards_encode_to_curve_batch.argtypes = [vp, vp, vp, sz, vp, sz, vp]
+    lib.dalek_b200_ristretto_map_to_curve_batch.argtypes = [vp, vp, sz, vp]
+    lib.dalek_b200_ristretto_lizard_encode_batch.argtypes = [vp, vp, sz, vp]
+    lib.dalek_b200_ristretto_lizard_decode_batch.argtypes = [vp, vp, C.c_int, sz, vp, vp]
+    lib.dalek_b200_ristretto_map_to_curve_inverse_batch.argtypes = [vp, vp, C.c_int, sz, vp, vp]
     _lib = lib
     return lib
 
@@ -398,6 +402,37 @@ class Engine:
     def edwards_encode_to_curve_batch(self, msgs_flat, offsets, n, dst):
         """EdwardsPoint::encode_to_curve::<Sha512> (RFC 9380 ..._NU_), same layout as edwards_hash_to_curve_batch."""
         return self._edwards_h2c(self.lib.dalek_b200_edwards_encode_to_curve_batch, msgs_flat, offsets, n, dst)
+
+    # ---- Lizard and the Elligator inverse ----
+    def ristretto_map_to_curve_batch(self, data, n):
+        """RistrettoPoint::map_to_curve for n x 32 B (bit 255 ignored) -> n x 32 B CompressedRistretto."""
+        out = (C.c_uint8 * (32 * max(n, 1)))()
+        self._check(self.lib.dalek_b200_ristretto_map_to_curve_batch(self.h, _ptr(data), n, C.addressof(out)))
+        return bytes(out)[:32 * n]
+
+    def ristretto_lizard_encode_batch(self, data, n):
+        """RistrettoPoint::lizard_encode::<Sha256> for n x 16 B -> n x 32 B CompressedRistretto."""
+        out = (C.c_uint8 * (32 * max(n, 1)))()
+        self._check(self.lib.dalek_b200_ristretto_lizard_encode_batch(self.h, _ptr(data), n, C.addressof(out)))
+        return bytes(out)[:32 * n]
+
+    def ristretto_lizard_decode_batch(self, points, n, point_fmt=POINTS_RISTRETTO):
+        """RistrettoPoint::lizard_decode::<Sha256> for n points (RISTRETTO or EXTENDED).  Returns (rc, n x 16 B payloads,
+        n status bytes: 0 Some, 1 None, 2 undecodable encoding); rc 1 (DALEK_NONE) unless every status is 0."""
+        out = (C.c_uint8 * (16 * max(n, 1)))()
+        st = (C.c_uint8 * max(n, 1))()
+        rc = self._check(self.lib.dalek_b200_ristretto_lizard_decode_batch(self.h, _ptr(points), point_fmt, n, C.addressof(out),
+                                                                           C.addressof(st)))
+        return rc, bytes(out)[:16 * n], bytes(st)[:n]
+
+    def ristretto_map_to_curve_inverse_batch(self, points, n, point_fmt=POINTS_RISTRETTO):
+        """RistrettoPoint::map_to_curve_inverse for n points.  Returns (rc, n x 16 x 32 B candidates, list of n u16 masks);
+        rc 1 (DALEK_NONE) when an encoding does not decode (its mask is 0)."""
+        out = (C.c_uint8 * (512 * max(n, 1)))()
+        mask = (C.c_uint16 * max(n, 1))()
+        rc = self._check(self.lib.dalek_b200_ristretto_map_to_curve_inverse_batch(self.h, _ptr(points), point_fmt, n,
+                                                                                  C.addressof(out), C.addressof(mask)))
+        return rc, bytes(out)[:512 * n], list(mask)[:n]
 
     # ---- ed25519 ----
     def verify_batch_raw(self, messages, sigs, pubkeys):
@@ -920,6 +955,56 @@ class RistrettoPoint:
         flat, offs, n = _flat_messages(messages)
         raw = eng.ristretto_hash_from_bytes_batch(flat, offs, n)
         return [raw[32 * i:32 * i + 32] for i in range(n)]
+
+    @staticmethod
+    def map_to_curve_batch(data, engine=None):
+        """RistrettoPoint::map_to_curve (ristretto/elligator.rs:62-67) for each 32-byte string (bit 255 ignored): the list of
+        32-byte CompressedRistretto encodings."""
+        _, items = _items(list(data), 32, "map_to_curve inputs")
+        if not items:
+            return []
+        eng = engine or default_engine()
+        raw = eng.ristretto_map_to_curve_batch(b"".join(items), len(items))
+        return [raw[32 * i:32 * i + 32] for i in range(len(items))]
+
+    @staticmethod
+    def lizard_encode_batch(data, engine=None):
+        """RistrettoPoint::lizard_encode::<Sha256> (lizard/lizard_ristretto.rs:25-39) for each 16-byte string: the list of
+        32-byte CompressedRistretto encodings."""
+        _, items = _items(list(data), 16, "Lizard payloads")
+        if not items:
+            return []
+        eng = engine or default_engine()
+        raw = eng.ristretto_lizard_encode_batch(b"".join(items), len(items))
+        return [raw[32 * i:32 * i + 32] for i in range(len(items))]
+
+    @staticmethod
+    def lizard_decode_batch(points, engine=None):
+        """RistrettoPoint::lizard_decode::<Sha256> (:43-71) for each 32-byte CompressedRistretto: the 16-byte payload, or
+        None when the point is not a Lizard encoding.  An encoding that does not decode raises ValueError."""
+        _, items = _items(list(points), 32, "points")
+        if not items:
+            return []
+        eng = engine or default_engine()
+        _, raw, st = eng.ristretto_lizard_decode_batch(b"".join(items), len(items))
+        if any(s == 2 for s in st):
+            raise ValueError("a point does not decode")
+        return [raw[16 * i:16 * i + 16] if st[i] == 0 else None for i in range(len(items))]
+
+    @staticmethod
+    def map_to_curve_inverse_batch(points, engine=None):
+        """RistrettoPoint::map_to_curve_inverse (:213-219) for each 32-byte CompressedRistretto: a list of 16 entries, each the
+        32 bytes that map_to_curve takes to the point, or None, in the reference's order.  The candidates depend on the
+        representative; a decoded encoding is the one with Z = 1.  An encoding that does not decode raises ValueError."""
+        _, items = _items(list(points), 32, "points")
+        if not items:
+            return []
+        eng = engine or default_engine()
+        rc, raw, masks = eng.ristretto_map_to_curve_inverse_batch(b"".join(items), len(items))
+        if rc == 1:
+            raise ValueError("a point does not decode")
+        return [[raw[512 * i + 32 * j:512 * i + 32 * j + 32] if masks[i] >> j & 1 else None for j in range(16)]
+                for i in range(len(items))]
 
 
 def verify_batch(messages, signatures, verifying_keys, engine=None):

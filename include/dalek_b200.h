@@ -85,7 +85,8 @@ int dalek_b200_last_kernel_ms(const dalek_b200_ctx *ctx, float *ms, int *launche
  * verify_batch call, the largest kernel of that path; summed over the pieces of a host-streamed call). */
 int dalek_b200_last_stage_ms(const dalek_b200_ctx *ctx, const char *stage, float *ms);
 /* Milliseconds between CUDA events recorded on the context's stream at entry of the last MSM / verify_batch /
- * precomputed-MSM / X25519 / to_montgomery_batch / hash-to-group / mul_batch call, or of the last ed25519_b200_verifying_keys /
+ * precomputed-MSM / X25519 / to_montgomery_batch / hash-to-group / Lizard / map_to_curve / map_to_curve_inverse / mul_batch
+ * call, or of the last ed25519_b200_verifying_keys /
  * sign_flat / sign_prehashed / verify_prehashed_each call, and after the last work it enqueued (all of the call's streams
  * joined): the device time of that call, copies of host-buffer calls included. */
 int dalek_b200_last_call_ms(const dalek_b200_ctx *ctx, float *ms);
@@ -295,6 +296,32 @@ int dalek_b200_edwards_hash_to_curve_batch(dalek_b200_ctx *ctx, const uint8_t *m
                                            size_t n, const uint8_t *dst, size_t dst_len, uint8_t *out);
 int dalek_b200_edwards_encode_to_curve_batch(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets,
                                              size_t n, const uint8_t *dst, size_t dst_len, uint8_t *out);
+
+/* -------- Lizard and the Elligator inverse ------------------------------------------------------
+ * Lizard (C/lizard/) is an injective map from 16-byte strings into ristretto255, for ElGamal encryption of short payloads.
+ * Host buffers; each call blocks and streams the batch in pieces like hash to group.  n = 0 is a successful no-op; with
+ * n > 0 a NULL buffer is DALEK_E_INVALID_ARG.  No option affects these calls.  The digest is fixed to SHA-256 (the
+ * reference is generic over any 32-byte Digest and says "Use SHA-256 if otherwise unsure").  Points are
+ * DALEK_POINTS_RISTRETTO (CompressedRistretto) or DALEK_POINTS_EXTENDED (20 radix-2^51 limbs, any Z, trusted to be a valid
+ * RistrettoPoint representative and used exactly as given: the candidate order of the inverse depends on the
+ * representative); any other point_fmt is DALEK_E_INVALID_ARG.  Constant time in the payloads, the points and the
+ * recovered payloads.  Every call clears the device copies of its staged inputs and outputs before it returns.
+ * map_to_curve_restricted is map_to_curve with a precondition assertion and has no entry point of its own.
+ *
+ * RistrettoPoint::map_to_curve (C/ristretto/elligator.rs:62-67): n x 32 B -> n x 32 B CompressedRistretto; bit 255 ignored. */
+int dalek_b200_ristretto_map_to_curve_batch(dalek_b200_ctx *ctx, const uint8_t *in, size_t n, uint8_t *out);
+/* RistrettoPoint::lizard_encode::<Sha256> (C/lizard/lizard_ristretto.rs:25-39): n x 16 B -> n x 32 B CompressedRistretto. */
+int dalek_b200_ristretto_lizard_encode_batch(dalek_b200_ctx *ctx, const uint8_t *data, size_t n, uint8_t *out);
+/* RistrettoPoint::lizard_decode::<Sha256> (:43-71).  data_out n x 16 B, status n bytes: 0 = Some (payload in data_out),
+ * 1 = None (a point, but not exactly one candidate passes), 2 = encoding does not decode.  Slots with status != 0 hold
+ * zeros.  Returns DALEK_OK if every status is 0, else DALEK_NONE. */
+int dalek_b200_ristretto_lizard_decode_batch(dalek_b200_ctx *ctx, const void *points, int point_fmt, size_t n,
+                                             uint8_t *data_out, uint8_t *status);
+/* RistrettoPoint::map_to_curve_inverse (:213-219).  out n x 16 x 32 B: candidate j of item i at out[512 i + 32 j], in the
+ * reference's order (jc0, dual(jc0), ..., jc3, dual(jc3), then their negations); zero bytes where None.  mask n x u16:
+ * bit j set iff candidate j is Some.  An undecodable encoding gives mask 0 and makes the call return DALEK_NONE. */
+int dalek_b200_ristretto_map_to_curve_inverse_batch(dalek_b200_ctx *ctx, const void *points, int point_fmt, size_t n,
+                                                    uint8_t *out, uint16_t *mask);
 
 /* -------- scalar batch helpers (SURVEY 8f rank 4) ---------------------------------------------
  * Scalar::from_bytes_mod_order_wide (C/scalar.rs:248-250) for n 64-byte strings -> n canonical 32-byte scalars. */
