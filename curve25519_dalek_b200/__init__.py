@@ -17,6 +17,8 @@ touches the CPU checker used by the tests.  Names follow the reference:
   EdwardsPoint.mul_batch / mul_clamped_batch / is_small_order_batch / is_torsion_free_batch and RistrettoPoint.mul_batch
       (src/edwards.rs:890-941, :1405-1437; src/ristretto.rs:917-926): constant-time s * P per item, one scalar or one
       point broadcast to the whole batch
+  EdwardsPoint / RistrettoPoint .optional_multiscalar_mul_batch / vartime_multiscalar_mul_batch / multiscalar_mul_batch
+      (traits.rs:78-262 once per item): many independent MSMs, each with its own scalars and points, in one call
   RistrettoPoint.map_to_curve_batch / lizard_encode_batch / lizard_decode_batch / map_to_curve_inverse_batch
       (src/ristretto/elligator.rs:62-67, src/lizard/lizard_ristretto.rs:25-71, :213-219): Lizard over SHA-256
 """

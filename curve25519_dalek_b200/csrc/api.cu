@@ -59,7 +59,7 @@ void dalek_b200_destroy(dalek_b200_ctx *ctx)
     DevBuf *bufs[] = {&ctx->scalars, &ctx->points_in, &ctx->points, &ctx->digits, &ctx->counts, &ctx->offsets,
                       &ctx->sorted, &ctx->buckets, &ctx->red_a, &ctx->red_b, &ctx->red_c, &ctx->red_d, &ctx->key_pts,
                       &ctx->result, &ctx->flags, &ctx->misc0, &ctx->misc1, &ctx->misc2, &ctx->misc3,
-                      &ctx->misc4, &ctx->misc5, &ctx->zs, &ctx->base_table, &ctx->ntasks, &ctx->task_off, &ctx->tasks, &ctx->task_sums, &ctx->msg_offs, &ctx->sum_desc, &ctx->sum_part, &ctx->key_table, &ctx->key_acc, &ctx->task_order, &ctx->sig_status, &ctx->misc6, &ctx->each_pow, &ctx->each_tab, &ctx->each_kstat, &ctx->comb_base_table, &ctx->prep_prod};
+                      &ctx->misc4, &ctx->misc5, &ctx->zs, &ctx->base_table, &ctx->ntasks, &ctx->task_off, &ctx->tasks, &ctx->task_sums, &ctx->msg_offs, &ctx->sum_desc, &ctx->sum_part, &ctx->key_table, &ctx->key_acc, &ctx->task_order, &ctx->sig_status, &ctx->misc6, &ctx->each_pow, &ctx->each_tab, &ctx->each_kstat, &ctx->comb_base_table, &ctx->prep_prod, &ctx->mb_ws[0], &ctx->mb_ws[1]};
     for (DevBuf *b : bufs) if (b->p) cudaFree(b->p);
     if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
     cudaEventDestroy(ctx->ev_a); cudaEventDestroy(ctx->ev_b); cudaEventDestroy(ctx->ev_fork); cudaEventDestroy(ctx->ev_join);
@@ -211,14 +211,11 @@ int msm_read_result(dalek_b200_ctx *ctx, const MsmResult *d_result, const int *d
     return *h_bad ? DALEK_NONE : DALEK_OK;
 }
 
-// One whole MSM, read back.  Ristretto points also give the Ristretto encoding of the result in out_compressed.  The
-// public entry points check the point format.
-static int msm_common(dalek_b200_ctx *ctx, const void *scalars, const void *points, bool on_device, int point_fmt,
-                      size_t n, uint8_t out_compressed[32], uint64_t out_limbs[20])
+// One whole MSM on the context's device, read back.  Ristretto points also give the Ristretto encoding of the result in
+// out_compressed.
+int msm_whole(dalek_b200_ctx *ctx, const void *scalars, const void *points, bool on_device, int point_fmt, size_t n,
+              uint8_t out_compressed[32], uint64_t out_limbs[20])
 {
-    if (!ctx || (n && (!scalars || !points)) || n >= (1ull << 31)) return DALEK_E_INVALID_ARG;
-    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    CallTimer timer(ctx);
     int rc;
     const int nwin = msm_window_count_for_bits(msm_choose_window_bits(ctx, n));
     if ((rc = ws_reserve(ctx, ctx->misc0, (size_t)nwin * sizeof(ge_p3_raw)))) return rc;
@@ -228,6 +225,16 @@ static int msm_common(dalek_b200_ctx *ctx, const void *scalars, const void *poin
     if ((rc = run_msm(ctx, scalars, points, on_device, point_fmt, n, n, (ge_p3_raw *)ctx->misc0.p, d_res))) return rc;
     if (d_enc && (rc = ristretto_encode_result(ctx, d_res, d_enc))) return rc;
     return msm_read_result(ctx, d_res, (const int *)ctx->flags.p, d_enc, out_compressed, out_limbs);
+}
+
+// The public entry points check the point format.
+static int msm_common(dalek_b200_ctx *ctx, const void *scalars, const void *points, bool on_device, int point_fmt,
+                      size_t n, uint8_t out_compressed[32], uint64_t out_limbs[20])
+{
+    if (!ctx || (n && (!scalars || !points)) || n >= (1ull << 31)) return DALEK_E_INVALID_ARG;
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    CallTimer timer(ctx);
+    return msm_whole(ctx, scalars, points, on_device, point_fmt, n, out_compressed, out_limbs);
 }
 
 static bool edwards_format(int point_fmt) { return point_fmt == DALEK_POINTS_COMPRESSED || point_fmt == DALEK_POINTS_EXTENDED; }

@@ -66,6 +66,7 @@ struct dalek_b200_ctx {
     bool comb_attr_set = false;     // cudaFuncAttributeMaxDynamicSharedMemorySize set for the comb kernel on this device
     DevBuf comb_base_table;         // comb table of the Ed25519 basepoint (comb.cuh) for X25519 public keys and signing, built once
     bool comb_base_table_ready = false;
+    DevBuf mb_ws[2];                // batched MSMs (msm_batch.cu): the workspace of the pieces on each of the two streams
     // pinned host staging
     void *h_pinned = nullptr;
     size_t h_pinned_cap = 0;
@@ -186,6 +187,11 @@ int msm_combine_windows(dalek_b200_ctx *ctx, const ge_p3_raw *d_windows, int ran
 // is set (a point did not decode), else DALEK_OK, or a negative engine code.
 int msm_read_result(dalek_b200_ctx *ctx, const MsmResult *d_result, const int *d_bad, const uint32_t *d_enc,
                     uint8_t out_compressed[32], uint64_t out_limbs[20]);
+
+// One whole vartime MSM (api.cu), host or device inputs, enqueued on ctx->stream and read back: what the single-MSM entry
+// points run after their argument checks.  Returns DALEK_OK, DALEK_NONE or a negative engine code.
+int msm_whole(dalek_b200_ctx *ctx, const void *scalars, const void *points, bool on_device, int point_fmt, size_t n,
+              uint8_t out_compressed[32], uint64_t out_limbs[20]);
 
 // ---- sharded MSM building blocks (api.cu), shared with the single-process multi-GPU entry points (multi.cu) ----
 // Enqueue the MSM of one shard on ctx's stream; its record (window accumulators + status word) is copied to

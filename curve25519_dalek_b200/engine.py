@@ -98,6 +98,8 @@ def load_library():
     lib.dalek_b200_mul_batch.argtypes = [vp, vp, sz, vp, C.c_int, sz, sz, C.c_int, vp, vp]
     lib.dalek_b200_mul_batch_dev.argtypes = [vp, vp, sz, vp, C.c_int, sz, sz, C.c_int, vp, vp]
     lib.dalek_b200_edwards_torsion_batch.argtypes = [vp, vp, C.c_int, sz, vp]
+    lib.dalek_b200_msm_batch.argtypes = [vp, vp, vp, C.c_int, vp, sz, C.c_int, vp, vp, vp]
+    lib.dalek_b200_msm_batch_dev.argtypes = [vp, vp, vp, C.c_int, vp, sz, C.c_int, vp, vp, vp]
     lib.dalek_b200_ristretto_from_uniform_bytes_batch.argtypes = [vp, vp, sz, vp]
     lib.dalek_b200_ristretto_hash_from_bytes_batch.argtypes = [vp, vp, vp, sz, vp]
     lib.dalek_b200_edwards_hash_to_curve_batch.argtypes = [vp, vp, vp, sz, vp, sz, vp]
@@ -368,6 +370,25 @@ class Engine:
                                                        _ptr(res), C.addressof(ok) if want_ok else None))
         return rc, (bytes(res)[:32 * n] if out is None else out), (bytes(ok)[:n] if want_ok else None)
 
+    # ---- many independent MSMs ----
+    def msm_batch(self, scalars, points, offsets, m, point_fmt=POINTS_COMPRESSED, constant_time=False, device_ptrs=False,
+                  want_limbs=False):
+        """m independent MSMs in one call (dalek_b200_msm_batch): MSM j is the sum of s_i * P_i over the terms
+        offsets[j] .. offsets[j+1] of the flat scalars (32 B each) and points; offsets are m + 1 uint64.  With device_ptrs
+        the three inputs are device buffers; the results always come back to the host.  Returns (rc, out, ok, limbs):
+        m x 32 bytes of encodings (CompressedRistretto for Ristretto points, else CompressedEdwardsY), m ok bytes and,
+        with want_limbs, m x 20 uint64.  rc 1 (DALEK_NONE): an MSM with ok 0 holds an undecodable point and its slot the
+        identity.  constant_time raises EngineError for an undecodable point or a scalar with bit 255 set."""
+        out = (C.c_uint8 * (32 * max(m, 1)))()
+        ok = (C.c_uint8 * max(m, 1))()
+        limbs = (C.c_uint64 * (20 * max(m, 1)))() if want_limbs else None
+        fn = self.lib.dalek_b200_msm_batch_dev if device_ptrs else self.lib.dalek_b200_msm_batch
+        keep = (scalars, points, offsets)
+        rc = self._check(fn(self.h, _ptr(scalars), _ptr(points), point_fmt, _ptr(offsets), m, 1 if constant_time else 0,
+                            C.addressof(out), C.addressof(limbs) if want_limbs else None, C.addressof(ok)))
+        del keep
+        return rc, bytes(out)[:32 * m], bytes(ok)[:m], (list(limbs)[:20 * m] if want_limbs else None)
+
     def torsion_batch(self, points, n, point_fmt=POINTS_COMPRESSED):
         """is_small_order | is_torsion_free << 1 | decoded << 2 per Edwards point (0 for an undecodable one), as bytes."""
         out = (C.c_uint8 * max(n, 1))()
@@ -595,6 +616,34 @@ def default_engine():
     return _default
 
 
+def _msm_batch(scalar_lists, point_lists, fmt, constant_time, engine):
+    import array
+    scalar_lists, point_lists = [list(s) for s in scalar_lists], [list(p) for p in point_lists]
+    assert len(scalar_lists) == len(point_lists), "one point list per scalar list"
+    for s, p in zip(scalar_lists, point_lists):
+        # both iterators must have equal, exact sizes (edwards.rs:982-988, :1013-1019 assert)
+        assert len(s) == len(p), "scalars and points must have the same length"
+    m = len(scalar_lists)
+    # a None among the points makes that MSM None; it is sent as an empty one
+    none = [any(q is None for q in p) for p in point_lists]
+    if constant_time and any(none):
+        raise ValueError("multiscalar_mul takes points, not Options")
+    offs = array.array("Q", [0])
+    for s, skip in zip(scalar_lists, none):
+        offs.append(offs[-1] + (0 if skip else len(s)))
+    flat_s = b"".join(b"".join(s) for s, skip in zip(scalar_lists, none) if not skip)
+    flat_p = b"".join(b"".join(p) for p, skip in zip(point_lists, none) if not skip)
+    eng = engine or default_engine()
+    rc, out, ok, _ = eng.msm_batch(flat_s, flat_p, offs.tobytes(), m, point_fmt=fmt, constant_time=constant_time)
+    return [None if (skip or not ok[j]) else out[32 * j:32 * j + 32] for j, skip in enumerate(none)]
+
+
+def _expect_all(results):
+    if any(r is None for r in results):
+        raise ValueError("should return some point")
+    return results
+
+
 class EdwardsPoint:
     """Mirror of the trait impls on curve25519_dalek::edwards::EdwardsPoint.  Points are handled in
     their 32-byte CompressedEdwardsY encoding; results are returned compressed."""
@@ -628,6 +677,24 @@ class EdwardsPoint:
         eng = engine or default_engine()
         rc, comp, _ = eng.edwards_ct_msm(b"".join(scalars), b"".join(points), len(scalars))
         return comp
+
+    @staticmethod
+    def optional_multiscalar_mul_batch(scalar_lists, point_lists, engine=None):
+        """optional_multiscalar_mul (traits.rs:196-262) for many independent MSMs in one call: item j is the MSM of
+        scalar_lists[j] over point_lists[j] (CompressedEdwardsY).  Returns the list of 32-byte encodings, None where a
+        point is None or does not decompress."""
+        return _msm_batch(scalar_lists, point_lists, POINTS_COMPRESSED, False, engine)
+
+    @staticmethod
+    def vartime_multiscalar_mul_batch(scalar_lists, point_lists, engine=None):
+        """traits.rs:249-262 for every item of optional_multiscalar_mul_batch: .expect() on each."""
+        return _expect_all(_msm_batch(scalar_lists, point_lists, POINTS_COMPRESSED, False, engine))
+
+    @staticmethod
+    def multiscalar_mul_batch(scalar_lists, point_lists, engine=None):
+        """MultiscalarMul::multiscalar_mul (traits.rs:78-134, edwards.rs:970-995) for many independent MSMs in one call,
+        constant time in the scalars.  An undecodable point or a scalar with bit 255 set raises EngineError."""
+        return _msm_batch(scalar_lists, point_lists, POINTS_COMPRESSED, True, engine)
 
     @staticmethod
     def to_montgomery_batch(limbs, n=None, engine=None):
@@ -919,6 +986,22 @@ class RistrettoPoint:
         if rc == 1:
             raise ValueError("should return some point")
         return comp
+
+    @staticmethod
+    def optional_multiscalar_mul_batch(scalar_lists, point_lists, engine=None):
+        """optional_multiscalar_mul (ristretto.rs:979-994) for many independent MSMs in one call over CompressedRistretto
+        points: the list of CompressedRistretto results, None where a point is None or does not decode."""
+        return _msm_batch(scalar_lists, point_lists, POINTS_RISTRETTO, False, engine)
+
+    @staticmethod
+    def vartime_multiscalar_mul_batch(scalar_lists, point_lists, engine=None):
+        return _expect_all(_msm_batch(scalar_lists, point_lists, POINTS_RISTRETTO, False, engine))
+
+    @staticmethod
+    def multiscalar_mul_batch(scalar_lists, point_lists, engine=None):
+        """RistrettoPoint::multiscalar_mul (ristretto.rs:964-977) for many independent MSMs in one call, constant time in
+        the scalars.  An undecodable point or a scalar with bit 255 set raises EngineError."""
+        return _msm_batch(scalar_lists, point_lists, POINTS_RISTRETTO, True, engine)
 
     @staticmethod
     def double_base_batch(a, b, G, H, engine=None):

@@ -274,6 +274,39 @@ int dalek_b200_mul_batch_dev(dalek_b200_ctx *ctx, const void *d_scalars, size_t 
  * out[i] = 0; the call still returns DALEK_OK.  Host buffers, streamed in pieces. */
 int dalek_b200_edwards_torsion_batch(dalek_b200_ctx *ctx, const void *points, int point_fmt, size_t n, uint8_t *out);
 
+/* -------- many independent MSMs in one call ----------------------------------------------------
+ * m multiscalar multiplications, each with its own scalars and its own points: MSM j is the sum of s_i * P_i over the
+ * terms offsets[j] <= i < offsets[j+1] of the flat arrays, and out holds one result per MSM.  Per MSM the semantics are
+ * those of the single calls on its segment:
+ *   constant_time = 0: VartimeMultiscalarMul::optional_multiscalar_mul (C/traits.rs:196-262, C/edwards.rs:1002-1030,
+ *     C/ristretto.rs:979-994).  An undecodable point makes that MSM None: ok[j] = 0, its slot holds the identity's
+ *     encoding (and limbs), every other MSM is unaffected and the call returns DALEK_NONE; otherwise DALEK_OK.
+ *   constant_time = 1: MultiscalarMul::multiscalar_mul (C/traits.rs:78-134, C/edwards.rs:970-995,
+ *     C/backend/serial/scalar_mul/straus.rs:103-144; for RISTRETTO C/ristretto.rs:964-977): no branch, loop bound or
+ *     address depends on a scalar; the segment sizes and the points are public.  An undecodable point is
+ *     DALEK_E_INVALID_ARG for the call (ok still says where), and so is a scalar with bit 255 set (Scalar invariant #1),
+ *     found before any device work.  The device copies of the scalars, their digits, the per-term tables and the
+ *     partial sums are cleared before the call returns.
+ *   offsets: m + 1 values, offsets[0] = 0, non-decreasing, offsets[m] = total < 2^31, else DALEK_E_INVALID_ARG before any
+ *     device work.  An empty segment gives the identity.  m = 0 is a successful no-op.  A NULL offsets or out with m > 0,
+ *     or NULL scalars or points with total > 0, is DALEK_E_INVALID_ARG; out_limbs and ok may be NULL.
+ *   Point formats: COMPRESSED and EXTENDED give CompressedEdwardsY results, RISTRETTO gives CompressedRistretto;
+ *     out_limbs are canonical radix-2^51 limbs (X | Y | Z | T) of an equal point.
+ *   Every result is the group element the single call returns for that segment.  Variable-time scalars are any 256-bit
+ *     values, as in dalek_b200_edwards_vartime_msm.  Variable-time segments of 2^15 terms or more run through the
+ *     single-MSM pipeline inside the call; the rest of the batch runs in pieces of whole MSMs of at most 2^18 terms on two
+ *     streams, about 1.3 KiB of workspace per term of a piece (a constant-time MSM larger than a piece is a piece of its
+ *     own).  No option affects these calls. */
+int dalek_b200_msm_batch(dalek_b200_ctx *ctx, const uint8_t *scalars /* total x 32 B */, const void *points, int point_fmt,
+                         const uint64_t *offsets /* m + 1 */, size_t m, int constant_time, uint8_t *out /* m x 32 B */,
+                         uint64_t *out_limbs /* nullable, m x 20 */, uint8_t *ok /* nullable, m bytes */);
+/* same with scalars, points and offsets in device memory; the results go to host memory.  The offsets are read back
+ * once (8 bytes per MSM) to check them and to size the pieces.  A scalar with bit 255 set in constant-time mode is
+ * reported after the batch ran: the call returns DALEK_E_INVALID_ARG and the outputs are unspecified.  The engine's digits,
+ * tables and partial sums are cleared as above; the input buffers are the caller's. */
+int dalek_b200_msm_batch_dev(dalek_b200_ctx *ctx, const void *d_scalars, const void *d_points, int point_fmt, const void *d_offsets,
+                             size_t m, int constant_time, uint8_t *out, uint64_t *out_limbs, uint8_t *ok);
+
 /* -------- hash to group ------------------------------------------------------------------------
  * Host buffers; each call blocks and streams the batch in pieces like the codecs.  The maps are total: these calls never
  * return DALEK_NONE.  n = 0 is a successful no-op; with n > 0 a NULL buffer other than msgs_flat is DALEK_E_INVALID_ARG.
