@@ -21,6 +21,8 @@ touches the CPU checker used by the tests.  Names follow the reference:
       (traits.rs:78-262 once per item): many independent MSMs, each with its own scalars and points, in one call
   RistrettoPoint.map_to_curve_batch / lizard_encode_batch / lizard_decode_batch / map_to_curve_inverse_batch
       (src/ristretto/elligator.rs:62-67, src/lizard/lizard_ristretto.rs:25-71, :213-219): Lizard over SHA-256
+  EdwardsPoint / RistrettoPoint .vartime_double_scalar_mul_basepoint_batch (src/edwards.rs:1078-1087,
+      src/ristretto.rs:1051-1063): a_i A_i + b_i B per item, variable time
 """
 from .engine import (Engine, MultiEngine, EngineError, EdwardsPoint, RistrettoPoint, SignatureError, verify_batch, default_engine,
                      library_path, load_library, POINTS_COMPRESSED, POINTS_EXTENDED, POINTS_RISTRETTO,

@@ -12,14 +12,16 @@
 //
 // Two paths, same results.  When the keys of a call repeat, the doublings are paid once per KEY (per-key comb tables,
 // k_each_key_* and k_verify_each_comb below: 128 mixed additions per signature, no doubling).  Otherwise (plain kernel,
-// k_verify_each): one thread per signature.  [s]B + [k](-A) is computed on the FP64 field with radix-16 signed digits
-// (scalar.rs:1019-1051): 63 x 4 doublings, 64 mixed additions from the shared 8-entry table of B and 64 additions
-// from the thread's own 8-entry table of -A (local memory).  The reference interleaves width-5 / width-8 NAFs;
-// fixed radix-16 keeps the lanes of a warp on the same schedule.  Same group element, hence the same encoding.
+// k_verify_each): one thread per signature.  [s]B + [k](-A) is computed on the FP64 field by double_base_eval
+// (double_base.cuh, shared with the double-base batch of double_base.cu): radix-16 signed digits (scalar.rs:1019-1051),
+// 63 x 4 doublings, 64 mixed additions from the shared 8-entry table of B and 64 additions from the thread's own 8-entry
+// table of -A (local memory).  The reference interleaves width-5 / width-8 NAFs; fixed radix-16 keeps the lanes of a
+// warp on the same schedule.  Same group element, hence the same encoding.
 #include <algorithm>
 #include <cstring>
 
 #include "../../include/dalek_b200.h"
+#include "double_base.cuh"
 #include "engine.h"
 #include "ge64.cuh"
 #include "hash.cuh"
@@ -27,17 +29,6 @@
 #include "sc.cuh"
 
 static inline unsigned cdiv(size_t a, unsigned b) { return (unsigned)((a + b - 1) / b); }
-
-__device__ __forceinline__ void radix16(int8_t d[64], const uint32_t w[8])
-{
-    int carry = 0;
-#pragma unroll 1
-    for (int pos = 0; pos < 64; pos++) {
-        int v = (int)((w[pos >> 3] >> (4 * (pos & 7))) & 15) + carry;
-        if (pos < 63) { carry = (v + 8) >> 4; v -= carry << 4; }
-        d[pos] = (int8_t)v;
-    }
-}
 
 // [8]P == identity  (EdwardsPoint::is_small_order, C/edwards.rs:1405-1407)
 __device__ __forceinline__ uint32_t is_small_order(const ge_p3 &p)
@@ -59,14 +50,7 @@ __device__ __forceinline__ void verify_each_body(const uint8_t *__restrict__ msg
                                                  const ge_niels_packed *__restrict__ base_row0, uint8_t *__restrict__ out)
 {
     __shared__ double s_B[8 * 15];                               // (j+1) B as balanced FP64 affine Niels, j = 0..7
-    if (threadIdx.x < 8) {
-        ge64_niels e; ge64_niels_unpack(e, base_row0[threadIdx.x]);
-        fe64 c;
-        double *dst = s_B + 15 * threadIdx.x;
-        fe64_carry(c, e.ypx);  for (int k = 0; k < 5; k++) dst[k] = c.v[k];
-        fe64_carry(c, e.ymx);  for (int k = 0; k < 5; k++) dst[5 + k] = c.v[k];
-        fe64_carry(c, e.xy2d); for (int k = 0; k < 5; k++) dst[10 + k] = c.v[k];
-    }
+    if (threadIdx.x < 8) double_base_stage_B(s_B + 15 * threadIdx.x, base_row0[threadIdx.x]);
     __syncthreads();
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -103,42 +87,13 @@ __device__ __forceinline__ void verify_each_body(const uint8_t *__restrict__ msg
 #pragma unroll
         for (int k = 0; k < 8; k++) s[k] = 0;
     }
-    // table of (j+1) * (-A), j = 0..7
-    ge64_pniels T[8];
-    {
-        ge_p3 nA = A, P;
-        fe_neg(nA.X, A.X); fe_carry(nA.X, nA.X);
-        fe_neg(nA.T, A.T); fe_carry(nA.T, nA.T);
-        ge_pniels pn1, pn; ge_p3_to_pniels(pn1, nA);
-        P = nA;
-#pragma unroll 1
-        for (int j = 0; j < 8; j++) {
-            if (j) ge_padd(P, P, pn1, 0);
-            ge_p3_to_pniels(pn, P);
-            fe64_from_fe(T[j].YpX, pn.YpX); fe64_from_fe(T[j].YmX, pn.YmX); fe64_from_fe(T[j].Z, pn.Z); fe64_from_fe(T[j].T2d, pn.T2d);
-        }
-    }
-    int8_t ds[64], dk[64];
-    radix16(ds, s);
-    radix16(dk, h);
-    ge64_p3 acc; ge64_identity(acc);
-#pragma unroll 1
-    for (int pos = 63; pos >= 0; pos--) {
-        if (pos != 63) { ge64_dbl(acc, acc); ge64_dbl(acc, acc); ge64_dbl(acc, acc); ge64_dbl(acc, acc); }
-        const int a = ds[pos], b = dk[pos];
-        if (a) {
-            const int m = a < 0 ? -a : a;
-            ge64_niels q;
-            const double *row = s_B + 15 * (m - 1);
-#pragma unroll
-            for (int k = 0; k < 5; k++) { q.ypx.v[k] = row[k]; q.ymx.v[k] = row[5 + k]; q.xy2d.v[k] = row[10 + k]; }
-            ge64_madd(acc, acc, q, (uint32_t)(a < 0));
-        }
-        if (b) {
-            const int m = b < 0 ? -b : b;
-            ge64_padd(acc, acc, T[m - 1], (uint32_t)(b < 0));
-        }
-    }
+    // [k](-A) + [s]B
+    ge_p3 nA = A;
+    fe_neg(nA.X, A.X); fe_carry(nA.X, nA.X);
+    fe_neg(nA.T, A.T); fe_carry(nA.T, nA.T);
+    ge64_p3 acc;
+    DoubleBaseLocal w;
+    double_base_eval(acc, nA, h, s, s_B, w);
     ge_p3 Rc; ge64_to_p3(Rc, acc);
     uint32_t enc[8];
     ge_compress<1>(enc, Rc);                                                  // RCompute::finish, verifying.rs:553-556

@@ -98,6 +98,8 @@ def load_library():
     lib.dalek_b200_mul_batch.argtypes = [vp, vp, sz, vp, C.c_int, sz, sz, C.c_int, vp, vp]
     lib.dalek_b200_mul_batch_dev.argtypes = [vp, vp, sz, vp, C.c_int, sz, sz, C.c_int, vp, vp]
     lib.dalek_b200_edwards_torsion_batch.argtypes = [vp, vp, C.c_int, sz, vp]
+    lib.dalek_b200_vartime_double_base_batch.argtypes = [vp, vp, vp, C.c_int, sz, vp, vp]
+    lib.dalek_b200_vartime_double_base_batch_dev.argtypes = [vp, vp, vp, C.c_int, sz, vp, vp]
     lib.dalek_b200_msm_batch.argtypes = [vp, vp, vp, C.c_int, vp, sz, C.c_int, vp, vp, vp]
     lib.dalek_b200_msm_batch_dev.argtypes = [vp, vp, vp, C.c_int, vp, sz, C.c_int, vp, vp, vp]
     lib.dalek_b200_ristretto_from_uniform_bytes_batch.argtypes = [vp, vp, sz, vp]
@@ -368,6 +370,31 @@ class Engine:
         ok = (C.c_uint8 * max(n, 1))() if want_ok else None
         rc = self._check(self.lib.dalek_b200_mul_batch(self.h, _ptr(scalars), n_scalars, _ptr(points), point_fmt, n_points, n, flags,
                                                        _ptr(res), C.addressof(ok) if want_ok else None))
+        return rc, (bytes(res)[:32 * n] if out is None else out), (bytes(ok)[:n] if want_ok else None)
+
+    # ---- variable-time double-base scalar multiplication ----
+    def vartime_double_base_batch(self, ab, points, n, point_fmt=POINTS_COMPRESSED, device_ptrs=False, out=None, want_ok=False):
+        """out[i] = a_i * A_i + b_i * B for n items (dalek_b200_vartime_double_base_batch): ab holds n pairs a_i || b_i of
+        32-byte scalars (bit 255 clear), points the A_i.  Returns (rc, out, ok or None) like mul_batch; rc 1 (DALEK_NONE)
+        when a point does not decode (its ok byte is 0 and its slot holds the identity).  With device_ptrs the inputs are
+        device buffers and the results go to `out` (32 n bytes) and, with want_ok, an n-byte ok buffer on the engine's
+        device, new uint8 tensors if not given."""
+        if device_ptrs:
+            ok = None
+            if out is None or want_ok:
+                import torch
+                dev = torch.device("cuda", self.device)
+                if out is None:
+                    out = torch.empty(32 * max(n, 1), dtype=torch.uint8, device=dev)
+                if want_ok:
+                    ok = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+            rc = self._check(self.lib.dalek_b200_vartime_double_base_batch_dev(self.h, _ptr(ab), _ptr(points), point_fmt, n, _ptr(out),
+                                                                               _ptr(ok)))
+            return rc, out, ok
+        res = (C.c_uint8 * (32 * max(n, 1)))() if out is None else out
+        ok = (C.c_uint8 * max(n, 1))() if want_ok else None
+        rc = self._check(self.lib.dalek_b200_vartime_double_base_batch(self.h, _ptr(ab), _ptr(points), point_fmt, n, _ptr(res),
+                                                                       C.addressof(ok) if want_ok else None))
         return rc, (bytes(res)[:32 * n] if out is None else out), (bytes(ok)[:n] if want_ok else None)
 
     # ---- many independent MSMs ----
@@ -718,6 +745,13 @@ class EdwardsPoint:
         return _mul_batch(bytes_list, points, POINTS_COMPRESSED, True, engine)
 
     @staticmethod
+    def vartime_double_scalar_mul_basepoint_batch(a_list, points, b_list, engine=None):
+        """EdwardsPoint::vartime_double_scalar_mul_basepoint (edwards.rs:1078-1087) for each item: a_i * A_i + b_i * B with
+        32-byte scalars (bit 255 clear, not reduced) and CompressedEdwardsY points A_i.  Returns the list of 32-byte
+        CompressedEdwardsY results.  An undecodable point raises ValueError.  Variable time."""
+        return _double_base_batch(a_list, points, b_list, POINTS_COMPRESSED, engine)
+
+    @staticmethod
     def is_small_order_batch(points, engine=None):
         """EdwardsPoint::is_small_order (edwards.rs:1405-1407) of each CompressedEdwardsY: a list of bool."""
         return [bool(f & 1) for f in _torsion_flags(points, engine)]
@@ -761,6 +795,24 @@ def _mul_batch(scalars, points, fmt, clamped, engine):
         raise ValueError("a point does not decode")
     outs = [raw[32 * i:32 * i + 32] for i in range(n)]
     return outs[0] if single_s and single_p else outs
+
+
+def _double_base_batch(a_list, points, b_list, fmt, engine):
+    _, as_ = _items(a_list, 32, "scalars")
+    _, bs = _items(b_list, 32, "scalars")
+    _, ps = _items(points, 32, "points")
+    if not len(as_) == len(bs) == len(ps):
+        raise ValueError("a_list, points and b_list must have the same length")
+    n = len(ps)
+    if n == 0:
+        return []
+    if any((a[31] | b[31]) & 0x80 for a, b in zip(as_, bs)):
+        raise ValueError("a scalar has bit 255 set")
+    eng = engine or default_engine()
+    rc, raw, _ = eng.vartime_double_base_batch(b"".join(a + b for a, b in zip(as_, bs)), b"".join(ps), n, fmt)
+    if rc == 1:
+        raise ValueError("a point does not decode")
+    return [raw[32 * i:32 * i + 32] for i in range(n)]
 
 
 def _torsion_flags(points, engine):
@@ -1018,6 +1070,13 @@ class RistrettoPoint:
         CompressedRistretto; a single scalar or a single point is used for every item.  Returns the CompressedRistretto
         of the product, or the list.  An undecodable point raises ValueError."""
         return _mul_batch(scalars, points, POINTS_RISTRETTO, False, engine)
+
+    @staticmethod
+    def vartime_double_scalar_mul_basepoint_batch(a_list, points, b_list, engine=None):
+        """RistrettoPoint::vartime_double_scalar_mul_basepoint (ristretto.rs:1051-1063) for each item: a_i * A_i + b_i * B
+        with 32-byte scalars (bit 255 clear) and CompressedRistretto points A_i.  Returns the list of 32-byte
+        CompressedRistretto results.  An undecodable point raises ValueError.  Variable time."""
+        return _double_base_batch(a_list, points, b_list, POINTS_RISTRETTO, engine)
 
     @staticmethod
     def from_uniform_bytes_batch(data, engine=None):

@@ -86,7 +86,7 @@ int dalek_b200_last_kernel_ms(const dalek_b200_ctx *ctx, float *ms, int *launche
 int dalek_b200_last_stage_ms(const dalek_b200_ctx *ctx, const char *stage, float *ms);
 /* Milliseconds between CUDA events recorded on the context's stream at entry of the last MSM / verify_batch /
  * precomputed-MSM / X25519 / to_montgomery_batch / hash-to-group / Lizard / map_to_curve / map_to_curve_inverse / mul_batch
- * call, or of the last ed25519_b200_verifying_keys /
+ * / vartime_double_base_batch call, or of the last ed25519_b200_verifying_keys /
  * sign_flat / sign_prehashed / verify_prehashed_each call, and after the last work it enqueued (all of the call's streams
  * joined): the device time of that call, copies of host-buffer calls included. */
 int dalek_b200_last_call_ms(const dalek_b200_ctx *ctx, float *ms);
@@ -273,6 +273,28 @@ int dalek_b200_mul_batch_dev(dalek_b200_ctx *ctx, const void *d_scalars, size_t 
  * is_small_order).  points: COMPRESSED or EXTENDED, anything else is DALEK_E_INVALID_ARG.  An undecodable point gives
  * out[i] = 0; the call still returns DALEK_OK.  Host buffers, streamed in pieces. */
 int dalek_b200_edwards_torsion_batch(dalek_b200_ctx *ctx, const void *points, int point_fmt, size_t n, uint8_t *out);
+
+/* -------- variable-time double-base scalar multiplication ----------------------------------------
+ * EdwardsPoint::vartime_double_scalar_mul_basepoint (C/edwards.rs:1078-1087 -> vartime_double_base.rs:23-72) and
+ * RistrettoPoint::vartime_double_scalar_mul_basepoint (C/ristretto.rs:1051-1063): out[i] = a_i A_i + b_i B, B the
+ * Ed25519 (= Ristretto) basepoint; the operation of every Schnorr-style verification, R' = [k](-A) + [s]B.
+ *   ab holds n pairs a_i || b_i of 32-byte little-endian scalars.  Each must have bit 255 clear (Scalar invariant #1),
+ *     else DALEK_E_INVALID_ARG, found before any device work.  Scalars in [l, 2^255) are used as given, not reduced: A_i
+ *     may carry a torsion component, and then a A_i != (a mod l) A_i.
+ *   Point formats as dalek_b200_mul_batch: COMPRESSED (CompressedEdwardsY in and out), EXTENDED (20 radix-2^51 limbs in,
+ *     any Z, limbs < 2^54; CompressedEdwardsY out), RISTRETTO (CompressedRistretto in and out); any other point_fmt is
+ *     DALEK_E_INVALID_ARG.  An undecodable point gives ok[i] = 0 and the identity's encoding in its slot, and the call
+ *     returns DALEK_NONE; every other slot is computed and its ok[i] is 1.
+ *   n = 0 is a successful no-op.  A NULL ab, points or out with n > 0 is DALEK_E_INVALID_ARG; ok may be NULL.
+ *   Variable time: scalars and points are public, so nothing is cleared.  Host buffers are streamed in pieces like the
+ *     codecs.  No option affects these calls. */
+int dalek_b200_vartime_double_base_batch(dalek_b200_ctx *ctx, const uint8_t *ab /* n x 64 B: a_i || b_i */,
+                                         const void *points, int point_fmt, size_t n,
+                                         uint8_t *out /* n x 32 B */, uint8_t *ok /* n bytes, nullable */);
+/* same, every buffer a device pointer; blocks until done.  A scalar with bit 255 set is reported after the batch ran:
+ * the call returns DALEK_E_INVALID_ARG and the outputs are unspecified. */
+int dalek_b200_vartime_double_base_batch_dev(dalek_b200_ctx *ctx, const void *d_ab, const void *d_points, int point_fmt,
+                                             size_t n, void *d_out, void *d_ok);
 
 /* -------- many independent MSMs in one call ----------------------------------------------------
  * m multiscalar multiplications, each with its own scalars and its own points: MSM j is the sum of s_i * P_i over the
