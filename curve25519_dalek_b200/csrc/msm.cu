@@ -211,8 +211,11 @@ __device__ __forceinline__ void block_inverse(fe64 &inv, const fe64 &acc, fe64 *
         fe64 x, b, a, t;
         if (lane < nw) x = s_warp[lane]; else fe64_1(x);
         warp_other_products(x, b, a, all);
-        if (INVERT) {   // on the integer field: the temporaries of the FP64 chain (fe64_pow22501) would spill
-            fe q; fe64_to_fe(q, all); fe_invert(q, q); fe64_from_fe_limbs(t, q);
+        if (INVERT) {   // limb-parallel on warp 0's lanes (warp4_f64.cuh): one lone thread's chain is latency-bound
+            const w20_role r = w20_roles();
+            const double inv = w20_invert(w20_limb(all, r.i), r);
+#pragma unroll
+            for (uint32_t k = 0; k < 5; k++) t.v[k] = w20_shfl(inv, k);
         } else {
             t = *tot_inv;
         }
@@ -1002,8 +1005,9 @@ k_bucket_accumulate(const ge_niels_packed *__restrict__ points, const uint32_t *
     for (int q = 0; q < 10; q++) o[q] = make_uint4(r.w[4 * q], r.w[4 * q + 1], r.w[4 * q + 2], r.w[4 * q + 3]);
 }
 
-// Everything below is latency-bound tree work on few points: it runs on groups of four lanes
-// (warp4.cuh), one point operation per group at a time.
+// Everything below is latency-bound tree work on few points: k_heavy_fixup and k_plain_sum run on groups of four
+// lanes (warp4.cuh), one point operation per group at a time; k_chunk_reduce and k_finish_windows spread the limbs of
+// one point over 20 lanes of a warp (warp4_f64.cuh).
 
 // One warp per heavy bucket (grid-stride over the heavy list): the 8 groups of the warp take
 // strided task sums, then a 3-level shuffle tree across groups.
@@ -1078,35 +1082,32 @@ k_chunk_reduce_f64(const ge_p3_raw *__restrict__ S_in, uint32_t n_in, uint32_t m
 //   level l   chunks of m items of S^{l-1}: S^l_q, W^l_q = sum_r r S^{l-1}_{qm+r}      (0-based weights)
 //   then      target = A_1 + m_1 (A_2 + m_2 (A_3 + ...)),  A_l = plain sum of the W^l array
 // Doublings happen once per level in the final per-window Horner, not inside every level.
-// One 4-lane group per chunk; n_in is a power of two and m divides it, so every chunk has m items.
+// One warp per chunk, the limbs of each point spread over 20 lanes (warp4_f64.cuh); n_in is a power of two and m
+// divides it, so every chunk has m items.
 __global__ void __launch_bounds__(128)
 k_chunk_reduce(const ge_p3_raw *__restrict__ S_in, uint32_t n_in, uint32_t m, uint32_t one_based, uint32_t n_out,
                uint32_t nwin, ge_p3_raw *__restrict__ S_out, ge_p3_raw *__restrict__ W_out)
 {
-    const uint32_t role = threadIdx.x & 3;
-    const uint32_t total = n_out * nwin;
-    uint32_t t = (blockIdx.x * blockDim.x + threadIdx.x) >> 2;
-    if (((blockIdx.x * blockDim.x + (threadIdx.x & ~31u)) >> 2) >= total) return;    // whole warp out of range
-    const bool live = t < total;
-    if (!live) t = total - 1;                                                       // keep the warp converged
+    const uint32_t t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (t >= n_out * nwin) return;                                                  // whole warps
+    const w20_role rl = w20_roles();
+    const double d2 = w20_const_2d(rl);
     const uint32_t w = t / n_out, q = t % n_out;
     const ge_p3_raw *S = S_in + (size_t)w * n_in + (size_t)q * m;
-    w4_point run, acc, x;
-    w4_load(run, S + (m - 1));
-    acc = run;
+    double run = w20_load(S + (m - 1), rl), acc = run;
+#pragma unroll 1
     for (uint32_t r = m - 1; r-- > 1;) {
-        w4_load(x, S + r);
-        w4_add(run, x, role);
-        w4_add(acc, run, role);
+        w20_add(run, w20_load(S + r, rl), d2, rl);
+        w20_add(acc, run, d2, rl);
     }
     if (m > 1) {
-        w4_load(x, S);
-        w4_add(run, x, role);
-        if (one_based) w4_add(acc, run, role);
+        w20_add(run, w20_load(S, rl), d2, rl);
+        if (one_based) w20_add(acc, run, d2, rl);
     } else if (!one_based) {
-        w4_identity(acc);
+        acc = w20_identity(rl);
     }
-    if (live) { w4_store(S_out + t, run, role); w4_store(W_out + t, acc, role); }
+    w20_store(S_out + t, run);
+    w20_store(W_out + t, acc);
 }
 
 // plain sum of one array per CTA (blockIdx.x = array id): 32 groups take strided items, then a
@@ -1150,37 +1151,35 @@ __global__ void __launch_bounds__(128)
 k_finish_windows(const ge_p3_raw *__restrict__ S_top, const ge_p3_raw *__restrict__ A, LevelInfo li, uint32_t nwin,
                  ge_p3_raw *__restrict__ out)
 {
-    const uint32_t role = threadIdx.x & 3;
-    uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 2;
-    if (((blockIdx.x * blockDim.x + (threadIdx.x & ~31u)) >> 2) >= nwin) return;
-    const bool live = w < nwin;
-    if (!live) w = nwin - 1;
-    w4_point t, x;
+    const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;               // one warp per window, 20 lanes
+    if (w >= nwin) return;
+    const w20_role rl = w20_roles();
+    double t;
     if (li.nlevels > 0) {
-        w4_load(t, A + (size_t)(li.nlevels - 1) * nwin + w);
+        const double d2 = w20_const_2d(rl);
+        t = w20_load(A + (size_t)(li.nlevels - 1) * nwin + w, rl);
+#pragma unroll 1
         for (int l = li.nlevels - 2; l >= 0; l--) {
-            for (int k = 0; k < li.log2m[l]; k++) w4_dbl(t, role, k == li.log2m[l] - 1);
-            w4_load(x, A + (size_t)l * nwin + w);
-            w4_add(t, x, role);
+#pragma unroll 1
+            for (int k = 0; k < li.log2m[l]; k++) w20_dbl(t, rl);
+            w20_add(t, w20_load(A + (size_t)l * nwin + w, rl), d2, rl);
         }
     } else {
-        w4_load(t, S_top + w);            // a single bucket of weight 1
+        t = w20_load(S_top + w, rl);      // a single bucket of weight 1
     }
-    if (live) w4_store(out + w, t, role);
+    w20_store(out + w, t);
 }
 
-// Final Horner over windows (pippenger.rs:159): total = total * 2^c + window, ~250 sequential
-// doublings on one 4-lane group over the FP64 field (warp4_f64.cuh), then encode.
+// Final Horner over windows (pippenger.rs:159): total = total * 2^c + window, ~250 sequential doublings with the
+// limbs of the total spread over 20 lanes (warp4_f64.cuh), then the encoding's inversion on the same lanes.
 __global__ void __launch_bounds__(32)
 k_combine(const ge_p3_raw *__restrict__ windows, int ranks, int nwin, int c, MsmResult *__restrict__ res)
 {
-    const uint32_t role = threadIdx.x & 3;
-    w4f_point tot;
-    w4f_horner(tot, windows, ranks, nwin, c, role);
-    if (threadIdx.x != 0) return;
-    ge_p3 total; w4f_to_p3(total, tot);
+    const w20_role r = w20_roles();
     uint32_t s[8];
-    ge_compress(s, total);
+    ge_p3 total;
+    w20_encode(s, total, w20_horner(windows, ranks, nwin, c, r), r);
+    if (threadIdx.x != 0) return;
 #pragma unroll
     for (int i = 0; i < 8; i++) res->compressed[i] = s[i];
     fe_to_limbs51(res->limbs, total.X); fe_to_limbs51(res->limbs + 5, total.Y);
@@ -1341,7 +1340,7 @@ int msm_reduce_finish(dalek_b200_ctx *ctx, int c, ge_p3_raw *d_windows, MsmResul
         if (l == 0 && ctx->opt_field_f64 && n_in % m == 0)
             k_chunk_reduce_f64<<<cdiv((size_t)n_out * nwin, 32), 32, 0, st>>>(S_in, n_in, m, n_out, nwin, S_out, W_out);   // small CTAs: 1024 warps spread evenly over the SMs
         else
-            k_chunk_reduce<<<cdiv((size_t)n_out * nwin * 4, 128), 128, 0, st>>>(S_in, n_in, m, l == 0 ? 1u : 0u, n_out, nwin, S_out, W_out);
+            k_chunk_reduce<<<cdiv((size_t)n_out * nwin * 32, 128), 128, 0, st>>>(S_in, n_in, m, l == 0 ? 1u : 0u, n_out, nwin, S_out, W_out);
         ctx->launches++;
         w_arrays.push_back({pos + (size_t)n_out * nwin, n_out});
         S_in = S_out; n_in = n_out; pos += 2 * (size_t)n_out * nwin;
@@ -1370,7 +1369,7 @@ int msm_reduce_finish(dalek_b200_ctx *ctx, int c, ge_p3_raw *d_windows, MsmResul
         k_plain_sum<<<(unsigned)n2, 128, 0, st>>>(parts, dd2, A);
         ctx->launches += 2;
     }
-    k_finish_windows<<<cdiv((size_t)nwin * 4, 128), 128, 0, st>>>(S_in, A, li, nwin, d_windows);
+    k_finish_windows<<<cdiv((size_t)nwin * 32, 128), 128, 0, st>>>(S_in, A, li, nwin, d_windows);
     ctx->launches++;
     if (d_result) {
         k_combine<<<1, 32, 0, st>>>(d_windows, 1, nwin, c, d_result);

@@ -270,6 +270,48 @@ W4_DEV double w20_mul(double a_own, double b_own, const w20_role &r)
 #endif
 }
 
+// limb i of A^2.  A squaring is w20_mul(a, a): a form that spreads the 15 distinct limb products three per lane (two
+// operand shuffles and three splits instead of five each) needs lane-dependent x19 wraps for its partial columns, and
+// 254 of them in a chain took 48 us against 39 us for w20_mul on an H100 80GB HBM3 (700 W, 1980 MHz).
+W4_DEV double w20_sq(double a, const w20_role &r) { return w20_mul(a, a, r); }
+
+W4_DEV double w20_sqn(double a, int n, const w20_role &r)
+{
+#if FE64_DEV
+#pragma unroll 1
+#endif
+    for (int k = 0; k < n; k++) a = w20_sq(a, r);
+    return a;
+}
+
+// limb i of z^(p-2): the fixed chain of fe_invert / fe64_pow22501 (C/field.rs:176-210, :283-292), 254 squarings and
+// 11 multiplications; 0 -> 0.  Every group inverts its own element; the instruction stream does not depend on the data.
+// z: scale < 2; output scale 1.
+W4_DEV double w20_invert(double z, const w20_role &r)
+{
+    const double t0 = w20_sq(z, r);
+    const double t2 = w20_mul(z, w20_sqn(t0, 2, r), r);
+    const double t3 = w20_mul(t0, t2, r);
+    const double t5 = w20_mul(t2, w20_sq(t3, r), r);
+    const double t7 = w20_mul(w20_sqn(t5, 5, r), t5, r);
+    const double t9 = w20_mul(w20_sqn(t7, 10, r), t7, r);
+    const double t11 = w20_mul(w20_sqn(t9, 20, r), t9, r);
+    const double t13 = w20_mul(w20_sqn(t11, 10, r), t7, r);
+    const double t15 = w20_mul(w20_sqn(t13, 50, r), t13, r);
+    const double t17 = w20_mul(w20_sqn(t15, 100, r), t15, r);
+    const double t19 = w20_mul(w20_sqn(t17, 50, r), t13, r);   // z^(2^250 - 1)
+    return w20_mul(w20_sqn(t19, 5, r), t3, r);
+}
+
+// limb i of a replicated element (i uniform or not: a select, not an indexed load)
+W4_DEV double w20_limb(const fe64 &a, uint32_t i)
+{
+    double v = 0.0;
+#pragma unroll
+    for (uint32_t k = 0; k < 5; k++) if (i == k) v = a.v[k];
+    return v;
+}
+
 // own limb of the replicated point / back (c = limb i of coordinate g)
 W4_DEV double w20_take(const w4f_point &p, const w20_role &r)
 {
@@ -317,13 +359,71 @@ W4_DEV void w20_dbl_n(w4f_point &p, int k)
     w20_give(p, c);
 }
 
-// Horner over windows (pippenger.rs:159): total = total * 2^c + sum over ranks of window w, from the top window down.
-// windows: rank-major (ranks x nwin raw points).  The result is replicated in the four lanes of every group.
-W4_DEV void w4f_horner(w4f_point &tot, const ge_p3_raw *windows, int ranks, int nwin, int c, uint32_t role)
+// c <- limb of P + Q, both limb-distributed extended points (the formulas and scales of w4f_add); d2 = limb i of 2d.
+// The multiplication Q.T 2d does not depend on P: it leaves the dependent chain, which is two w20_mul.
+W4_DEV void w20_add(double &c, double q, double d2, const w20_role &r)
 {
-    fe64 d2; fe64_const_2d(d2);
-    w4f_point x;
-    w4f_identity(tot);
+    const double qT2d = w20_mul(w20_shfl(q, 15u + r.i), d2, r);     // as_projective_niels, in every group
+    const double qx = w20_shfl(q, r.i), qy = w20_shfl(q, 5u + r.i);
+    const double x = w20_shfl(c, r.i), y = w20_shfl(c, 5u + r.i);
+    // a = (Y - X)(qY - qX), b = (Y + X)(qY + qX), zz = Z qZ, cc = T qT2d in groups 0..3      <= 2 x 2
+    const double f = r.g == 0 ? y - x : r.g == 1 ? y + x : c;
+    const double g = r.g == 0 ? qy - qx : r.g == 1 ? qy + qx : r.g == 2 ? q : qT2d;
+    const double m = w20_mul(f, g, r);
+    const double a = w20_shfl(m, r.i), b = w20_shfl(m, 5u + r.i), zz = w20_shfl(m, 10u + r.i), cc = w20_shfl(m, 15u + r.i);
+    const double D = zz + zz;                                           // 2
+    const double E = b - a, H = b + a;                                  // 2, 2
+    const double DpC = D + cc;                                          // 3
+    const double DmC = w20_carry(D - cc, r);                            // 3 -> 1
+    const double f2 = r.g == 1 ? DpC : r.g == 3 ? E : DmC;              // X3 = DmC E, Y3 = DpC H, Z3 = DmC DpC, T3 = E H
+    const double g2 = r.g == 0 ? E : r.g == 2 ? DpC : H;
+    c = w20_mul(f2, g2, r);                                             // <= 3 x 2
+}
+
+// own limb of a raw point (fe64_from_fe_limbs on one limb, then the carry round)
+W4_DEV double w20_load(const ge_p3_raw *src, const w20_role &r)
+{
+    const uint32_t *w = src->w + 10u * r.g + 2u * r.i;
+    const uint64_t l = (uint64_t)w[0] + ((uint64_t)w[1] << 26);      // < 2^51 + 2^26: exact in a double
+#if FE64_DEV
+    const double t = __longlong_as_double((long long)l | FE64_E52) - FE64_TWO52;
+#else
+    const double t = (double)l;
+#endif
+    return w20_carry(t, r);
+}
+
+// store a limb-distributed point as a raw point: lane l < 4 gathers coordinate l and writes its 40 bytes
+W4_DEV void w20_store(ge_p3_raw *dst, double c)
+{
+    const uint32_t g = w4_lane() & 3u;
+    fe64 v;
+#pragma unroll
+    for (uint32_t k = 0; k < 5; k++) v.v[k] = w20_shfl(c, 5u * g + k);
+    if (w4_lane() >= 4u) return;
+    fe o; fe64_to_fe(o, v);
+    uint32_t *d = dst->w + 10u * g;
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+    for (int k = 0; k < 10; k += 2) *reinterpret_cast<uint2 *>(d + k) = make_uint2(o.v[k], o.v[k + 1]);
+#else
+    for (int k = 0; k < 10; k++) d[k] = o.v[k];
+#endif
+}
+
+// limb i of 2d
+W4_DEV double w20_const_2d(const w20_role &r) { fe64 d2; fe64_const_2d(d2); return w20_limb(d2, r.i); }
+
+// limb of the identity (0, 1, 1, 0)
+W4_DEV double w20_identity(const w20_role &r) { return (r.g == 1 || r.g == 2) && r.i == 0 ? 1.0 : 0.0; }
+
+// Horner over windows (pippenger.rs:159): total = total * 2^c + sum over ranks of window w, from the top window down.
+// windows: rank-major (ranks x nwin raw points).  Returns this lane's limb of the total: the whole pass, doublings and
+// additions, stays limb-distributed.
+W4_DEV double w20_horner(const ge_p3_raw *windows, int ranks, int nwin, int c, const w20_role &rl)
+{
+    const double d2 = w20_const_2d(rl);
+    double tot = w20_identity(rl);
     // Leading windows that are empty contribute nothing and doubling the identity is wasted latency: the top window of
     // every MSM over canonical scalars (< 2^253) is the carry window of the signed recoding, always empty; short scalars
     // (verify_batch's 128-bit z_i) leave more.  `started` is uniform over the warp (every lane loads the same points).
@@ -331,7 +431,8 @@ W4_DEV void w4f_horner(w4f_point &tot, const ge_p3_raw *windows, int ranks, int 
 #pragma unroll 1
     for (int w = nwin - 1; w >= 0; w--) {
         if (started) {
-            w20_dbl_n(tot, c);
+#pragma unroll 1
+            for (int t = 0; t < c; t++) w20_dbl(tot, rl);
         } else {
             bool any = false;
 #pragma unroll 1
@@ -351,6 +452,29 @@ W4_DEV void w4f_horner(w4f_point &tot, const ge_p3_raw *windows, int ranks, int 
             started = true;
         }
 #pragma unroll 1
-        for (int r = 0; r < ranks; r++) { w4f_load(x, windows + (size_t)r * nwin + w); w4f_add(tot, x, d2, role); }
+        for (int r = 0; r < ranks; r++) w20_add(tot, w20_load(windows + (size_t)r * nwin + w, rl), d2, rl);
     }
+    return tot;
+}
+
+// w20_horner with the total replicated in the four lanes of every group (the 4-lane interface; role is not needed)
+W4_DEV void w4f_horner(w4f_point &tot, const ge_p3_raw *windows, int ranks, int nwin, int c, uint32_t /* role */)
+{
+    w20_give(tot, w20_horner(windows, ranks, nwin, c, w20_roles()));
+}
+
+// EdwardsPoint::compress (C/edwards.rs:564-617) of a limb-distributed point: Z^-1 in every group, X Z^-1 and Y Z^-1 in
+// one multiplication, then the final limbs gathered.  Every lane gets the encoding s and the point itself.
+W4_DEV void w20_encode(uint32_t s[8], ge_p3 &P, double c, const w20_role &r)
+{
+    const double zinv = w20_invert(w20_shfl(c, 10u + r.i), r);
+    const double aff = w20_mul(c, zinv, r);                           // groups 0, 1: x, y
+    w4f_point p; w20_give(p, c);
+    fe64 x64, y64;
+#pragma unroll
+    for (uint32_t k = 0; k < 5; k++) { x64.v[k] = w20_shfl(aff, k); y64.v[k] = w20_shfl(aff, 5u + k); }
+    w4f_to_p3(P, p);
+    fe x, y; fe64_to_fe(x, x64); fe64_to_fe(y, y64);
+    fe_tobytes_words(s, y);
+    s[7] ^= (uint32_t)fe_isnegative(x) << 31;
 }
