@@ -61,14 +61,13 @@ FE_HD void straus_table5(ge_pniels_packed tab[8], const ge64_p3 &A)
 
 // One warp, eight points (group g handles point 8 * warp + g): for i from the top non-zero digit down to 0
 //   Q <- 2Q;  Q <- Q +/- table[|naf_i| / 2] when naf_i != 0          (straus.rs:181-197, window.rs:187-192)
-// then the eight accumulators of the warp are added.  The sum is replicated in the lanes of group 0 on return.
-W4_DEV void straus_warp(w4f_point &Q, const int8_t *nafs, const ge_pniels_packed *tables, size_t n, size_t warp, uint32_t role, uint32_t grp)
+// Each group is left with its own accumulator s_j P_j (the identity for groups past n), a complete extended point.
+W4_DEV void straus_warp_accumulate(w4f_point &Q, const int8_t *nafs, const ge_pniels_packed *tables, size_t n, size_t warp, uint32_t role, uint32_t grp)
 {
     const size_t j = warp * 8 + grp;
     const bool live = j < n;
     const int8_t *naf = nafs + NAF_LEN * (live ? j : 0);
     const ge_pniels_packed *tab = tables + 8 * (live ? j : 0);
-    fe64 d2; fe64_const_2d(d2);
     w4f_identity(Q);
     // leading zero digits: doubling the identity changes nothing (straus.rs:181-190 starts from the identity)
     int top = -1;
@@ -82,7 +81,7 @@ W4_DEV void straus_warp(w4f_point &Q, const int8_t *nafs, const ge_pniels_packed
     for (int i = top; i >= 0; i--) {
         const int d = live ? naf[i] : 0;
         const bool any = w4_any(d != 0);
-        if (i != top) w4f_dbl(Q, role, any);
+        if (i != top) w4f_dbl(Q, role, any || i == 0);             // T after the last step: the warp sum reads it
         if (any) {                                                 // uniform per warp: full-mask shuffles inside
             const uint32_t neg = d < 0, e = (uint32_t)(neg ? -d : d) >> 1;      // window.rs:187-192: entry |x| / 2
             ge_pniels_packed pk;
@@ -98,8 +97,20 @@ W4_DEV void straus_warp(w4f_point &Q, const int8_t *nafs, const ge_pniels_packed
             if (d != 0) Q = R;                                     // groups with a zero digit keep Q
         }
     }
-    for (int delta = 16; delta >= 4; delta >>= 1) {                // the warp's eight accumulators -> one point
+}
+
+// The eight accumulators of the warp are added (this reads their T).  The sum is replicated in the lanes of group 0.
+W4_DEV void straus_warp_sum(w4f_point &Q, uint32_t role)
+{
+    fe64 d2; fe64_const_2d(d2);
+    for (int delta = 16; delta >= 4; delta >>= 1) {
         w4f_point X; w4f_shfl_down(X, Q, delta);
         w4f_add(Q, X, d2, role);
     }
+}
+
+W4_DEV void straus_warp(w4f_point &Q, const int8_t *nafs, const ge_pniels_packed *tables, size_t n, size_t warp, uint32_t role, uint32_t grp)
+{
+    straus_warp_accumulate(Q, nafs, tables, n, warp, role, grp);
+    straus_warp_sum(Q, role);
 }

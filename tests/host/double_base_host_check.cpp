@@ -10,6 +10,9 @@
 #include "../../curve25519_dalek_b200/csrc/double_base.cuh"
 #include <string.h>
 
+// 1 if T = XY / Z: the point handed to the next stage is a complete extended point (the next addition reads T)
+static int t_consistent(const ge_p3 &q) { fe a, b; fe_mul(a, q.X, q.Y); fe_mul(b, q.Z, q.T); return fe_eq(a, b); }
+
 // fmt: 0 CompressedEdwardsY, 1 extended radix-2^51 limbs (160 B), 2 CompressedRistretto; 1 if the point decodes
 static uint32_t load_point(ge_p3 &p, const uint8_t *in, int fmt)
 {
@@ -52,7 +55,8 @@ static void stage_B(double s_B[8 * 15])
 }
 
 extern "C" {
-// out = encode(a P + b B), ab = a || b (bit 255 clear).  Returns 1 if P decodes (else out = the identity's encoding).
+// out = encode(a P + b B), ab = a || b (bit 255 clear).  Returns 1 if P decodes (else out = the identity's encoding), -2
+// if a P + b B has T != XY / Z.
 int h_double_base(uint8_t *out, const uint8_t *ab, const uint8_t *point, int fmt)
 {
     static double s_B[8 * 15];
@@ -73,6 +77,6 @@ int h_double_base(uint8_t *out, const uint8_t *ab, const uint8_t *point, int fmt
     if (fmt == 2) ristretto_compress<1>(w, q);
     else ge_compress<1>(w, q);
     memcpy(out, w, 32);
-    return (int)good;
+    return t_consistent(q) ? (int)good : -2;
 }
 }

@@ -10,11 +10,15 @@
 #include <string.h>
 #include <vector>
 
+// 1 if T = XY / Z: the point handed to the next stage is a complete extended point (the next addition reads T)
+static int t_consistent(const ge_p3 &q) { fe a, b; fe_mul(a, q.X, q.Y); fe_mul(b, q.Z, q.T); return fe_eq(a, b); }
+
 extern "C" {
 int h_mb_chunk_max(void) { return MB_CHUNK; }
 
 // out = CompressedEdwardsY of sum s_t P_t over one chunk of len <= MB_CHUNK terms (32-byte scalars, CompressedEdwardsY
-// points); ct: the constant-time loop.  Returns 1 if every point decodes (an undecodable one counts as the identity).
+// points); ct: the constant-time loop.  Returns 1 if every point decodes (an undecodable one counts as the identity), 0 if
+// not, -2 if the chunk's sum (which the per-MSM sum of the chunks adds) has T != XY / Z.
 int h_mb_chunk(uint8_t *out, const uint8_t *scalars, const uint8_t *points, int len, int ct)
 {
     std::vector<int8_t> digits((size_t)len * NAF_LEN + 4);
@@ -42,7 +46,7 @@ int h_mb_chunk(uint8_t *out, const uint8_t *scalars, const uint8_t *points, int 
     uint32_t w[8];
     ge_compress<1>(w, q);
     memcpy(out, w, 32);
-    return all;
+    return t_consistent(q) ? all : -2;
 }
 
 // The cut of nseg MSMs (nseg + 1 offsets) into chunks: chunk_base gets nseg + 1 slots; seg / first / len get one entry

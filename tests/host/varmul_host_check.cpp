@@ -9,6 +9,9 @@
 #include "../../curve25519_dalek_b200/csrc/varmul.cuh"
 #include <string.h>
 
+// 1 if T = XY / Z: the point handed to the next stage is a complete extended point (the next addition reads T)
+static int t_consistent(const ge_p3 &q) { fe a, b; fe_mul(a, q.X, q.Y); fe_mul(b, q.Z, q.T); return fe_eq(a, b); }
+
 // fmt: 0 CompressedEdwardsY, 1 extended radix-2^51 limbs (160 B), 2 CompressedRistretto; 1 if the point decodes
 static uint32_t load_point(ge_p3 &p, const uint8_t *in, int fmt)
 {
@@ -33,7 +36,8 @@ static uint32_t load_point(ge_p3 &p, const uint8_t *in, int fmt)
 }
 
 extern "C" {
-// out = encode(s P); clamp: clamp_integer first.  Returns 1 if P decodes (else out = the identity's encoding).
+// out = encode(s P); clamp: clamp_integer first.  Returns 1 if P decodes (else out = the identity's encoding), -2 if
+// s P has T != XY / Z.
 int h_mul(uint8_t *out, const uint8_t *scalar, const uint8_t *point, int fmt, int clamp)
 {
     uint32_t s[8];
@@ -51,7 +55,7 @@ int h_mul(uint8_t *out, const uint8_t *scalar, const uint8_t *point, int fmt, in
     if (fmt == 2) ristretto_compress<1>(w, q);
     else ge_compress<1>(w, q);
     memcpy(out, w, 32);
-    return (int)good;
+    return t_consistent(q) ? (int)good : -2;
 }
 
 // is_small_order | is_torsion_free << 1 | decoded << 2, or 0 for an undecodable point (fmt 0 or 1)

@@ -89,8 +89,18 @@ int h_w4f_horner(uint8_t *out, const uint8_t *windows, int ranks, int nwin, int 
     return 1;
 }
 
-// the vartime Straus path of straus_vt.cu for n <= 8 * warps points: NAF, tables, per-warp loop, sum of the warps
-int h_straus_vartime(uint8_t *out, const uint8_t *scalars, const uint8_t *points, int n)
+static int fe_is_xy_zt(const ge_p3 &p) { fe a, b; fe_mul(a, p.X, p.Y); fe_mul(b, p.Z, p.T); return fe_eq(a, b); }
+static void store_coords(uint8_t *o, const ge_p3 &p)                    // canonical X | Y | Z | T, 32 bytes each
+{
+    const fe *c[4] = {&p.X, &p.Y, &p.Z, &p.T};
+    for (int k = 0; k < 4; k++) { uint32_t w[8]; fe_tobytes_words(w, *c[k]); memcpy(o + 32 * k, w, 32); }
+}
+
+// The vartime Straus path of straus_vt.cu on ceil(n / 8) emulated warps: NAF, tables, per-warp loop, sum of the warps
+// -> out (compressed).  groups (nullable): 8 * ceil(n / 8) records of 128 bytes, the accumulator of each group as
+// straus_warp_accumulate leaves it, before the warp sum.  Returns 0 on an undecodable point, -1 if the lanes of a group
+// disagree, -2 if a warp's sum (which the sum of the warps adds) has T != XY / Z.
+int h_straus_groups(uint8_t *groups, uint8_t *out, const uint8_t *scalars, const uint8_t *points, int n)
 {
     std::vector<int8_t> nafs((size_t)NAF_LEN * (n ? n : 1));
     std::vector<ge_pniels_packed> tables((size_t)8 * (n ? n : 1));
@@ -108,18 +118,28 @@ int h_straus_vartime(uint8_t *out, const uint8_t *scalars, const uint8_t *points
     }
     const int warps = (n + 7) / 8;
     ge_p3 total; ge_p3_identity(total);
+    int rc = 1;
     for (int w = 0; w < warps; w++) {
         ge_p3 part;
+        std::vector<uint8_t> acc(32 * 128);
         run_warp([&](uint32_t lane) {
             w4f_point Q;
-            straus_warp(Q, nafs.data(), tables.data(), (size_t)n, (size_t)w, lane & 3, lane >> 2);
+            straus_warp_accumulate(Q, nafs.data(), tables.data(), (size_t)n, (size_t)w, lane & 3, lane >> 2);
+            ge_p3 g; w4f_to_p3(g, Q);
+            store_coords(&acc[128 * lane], g);
+            straus_warp_sum(Q, lane & 3);
             if (lane == 0) w4f_to_p3(part, Q);
         });
+        for (int l = 0; l < 32; l++) if (memcmp(&acc[128 * l], &acc[128 * (l & ~3)], 128)) rc = -1;
+        if (groups) for (int g = 0; g < 8; g++) memcpy(groups + 128 * (8 * w + g), &acc[128 * 4 * g], 128);
+        if (rc == 1 && !fe_is_xy_zt(part)) rc = -2;
         ge_add(total, total, part);
     }
     store_point(out, total);
-    return 1;
+    return rc;
 }
+
+int h_straus_vartime(uint8_t *out, const uint8_t *scalars, const uint8_t *points, int n) { return h_straus_groups(nullptr, out, scalars, points, n); }
 
 // The 20-lane field multiplication (w20_mul: one limb per lane, transpose-sum by shuffles, one parallel round of carries)
 // against the single-thread host model fe64_mul, compared as canonical bytes.  a, b: 4 x 5 limbs each (one element per lane

@@ -252,3 +252,16 @@ def test_double_base_kernels_sass():
     assert len(blocks) == 3
     for b in blocks:
         assert "DFMA" in "\n".join(b)                  # the FP64 field
+
+
+@pytest.mark.parametrize("pattern", ["even", "pow2_2", "pow2_5", "pow2_6", "pow2_64", "pow2_200", "pow2_250"])
+def test_scalars_with_trailing_zero_bits(host, orc, pattern):
+    """a and b both even, or both multiples of 2^k: the evaluation ends on doublings with no addition, and its result
+    (which callers add to) must still carry T = XY / Z (h_double_base returns -2 otherwise)."""
+    import straus_patterns as sp
+    rnd = random.Random(pattern)
+    P = orc.scalarmul(b32(rnd.randrange(L)), orc.basepoint())
+    enc = orc.compress(P)
+    a_s, b_s = sp.pattern_scalars(pattern, rnd, 4), sp.pattern_scalars(pattern, rnd, 4)
+    for a, b in zip(a_s, b_s):
+        assert dbl(host, b32(a), enc, b32(b)) == (orc.compress(want(orc, b32(a), P, b32(b))), 1), (hex(a), hex(b))

@@ -196,3 +196,18 @@ def test_chunk_kernels_resource_usage():
     assert re.search(r"STACK:64\b", seen["0"]) and re.search(r"LOCAL:0\b", seen["0"])
     for usage in seen.values():
         assert int(re.search(r"REG:(\d+)", usage).group(1)) <= 192
+
+
+@pytest.mark.parametrize("ct", [False, True])
+@pytest.mark.parametrize("pattern", ["even", "ones", "small_odd"] + ["pow2_%d" % k for k in (2, 5, 6, 64, 200, 250)])
+def test_chunk_scalar_patterns_shared_by_every_term(host, orc, pattern, ct):
+    """Every scalar of the chunk even, a multiple of 2^k, or odd with one digit: no term adds in the last digit
+    positions (or none ever doubles).  The chunk's sum is added to the other chunks of its MSM, so its T must be
+    XY / Z (h_mb_chunk returns -2 otherwise)."""
+    import straus_patterns as sp
+    rnd = random.Random("%s-%d" % (pattern, ct))
+    B = orc.basepoint()
+    for n in (5, 16):
+        pts = [orc.scalarmul(b32(rnd.randrange(L)), B) for _ in range(n)]
+        scalars = [b32(v) for v in sp.pattern_scalars(pattern, rnd, n)]
+        assert chunk(host, scalars, [orc.compress(p) for p in pts], ct) == (want(orc, scalars, pts, ct), 1), n

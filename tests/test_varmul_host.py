@@ -214,3 +214,14 @@ def test_kernels_resource_usage():
             assert re.search(r"REG:\d+", lines[i + 1])
             found += 1
     assert found == 8
+
+
+@pytest.mark.parametrize("pattern", ["even", "pow2_2", "pow2_5", "pow2_6", "pow2_64", "pow2_200", "pow2_250"])
+def test_scalars_with_trailing_zero_bits(host, orc, pattern):
+    """Even scalars and multiples of 2^k end on doublings with no addition: the result must still carry T = XY / Z
+    (h_mul returns -2 otherwise)."""
+    import straus_patterns as sp
+    rnd = random.Random(pattern)
+    P = orc.scalarmul(b32(rnd.randrange(L)), orc.basepoint())
+    for s in sp.pattern_scalars(pattern, rnd, 6):
+        assert mul(host, b32(s), orc.compress(P)) == (orc.compress(orc.scalarmul(b32(s), P)), 1), hex(s)
