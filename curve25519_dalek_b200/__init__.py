@@ -23,15 +23,21 @@ touches the CPU checker used by the tests.  Names follow the reference:
       (src/ristretto/elligator.rs:62-67, src/lizard/lizard_ristretto.rs:25-71, :213-219): Lizard over SHA-256
   EdwardsPoint / RistrettoPoint .vartime_double_scalar_mul_basepoint_batch (src/edwards.rs:1078-1087,
       src/ristretto.rs:1051-1063): a_i A_i + b_i B per item, variable time
+  MontgomeryPoint.mul_batch / mul_bits_be_batch / to_edwards_batch / mul_base_batch / mul_clamped_batch /
+      mul_base_clamped_batch (src/montgomery.rs:143-268, :484-505): Scalar * MontgomeryPoint, the ladder over any bit
+      string of up to 512 bits, Montgomery -> Edwards, and fixed-base u(s B)
+  EdwardsPoint.mul_base_batch / mul_base_clamped_batch and RistrettoPoint.mul_base_batch (src/edwards.rs:918-957,
+      src/ristretto.rs:939): constant-time s B at every batch size
+  ed25519_to_montgomery (ed25519-dalek/src/verifying.rs:476): VerifyingKey::to_montgomery
 """
-from .engine import (Engine, MultiEngine, EngineError, EdwardsPoint, RistrettoPoint, SignatureError, verify_batch, default_engine,
-                     library_path, load_library, POINTS_COMPRESSED, POINTS_EXTENDED, POINTS_RISTRETTO,
+from .engine import (Engine, MultiEngine, EngineError, EdwardsPoint, RistrettoPoint, MontgomeryPoint, SignatureError, verify_batch, default_engine,
+                     library_path, load_library, POINTS_COMPRESSED, POINTS_EXTENDED, POINTS_RISTRETTO, POINTS_MONTGOMERY,
                      VartimeEdwardsPrecomputation, VartimeRistrettoPrecomputation, x25519, x25519_public_keys,
                      X25519_BASEPOINT_BYTES, ed25519_verifying_keys, ed25519_sign, ed25519_sign_prehashed,
-                     ed25519_verify_prehashed)
+                     ed25519_verify_prehashed, ed25519_to_montgomery)
 
-__all__ = ["Engine", "MultiEngine", "EngineError", "EdwardsPoint", "RistrettoPoint", "SignatureError", "verify_batch", "default_engine",
-           "library_path", "load_library", "POINTS_COMPRESSED", "POINTS_EXTENDED", "POINTS_RISTRETTO",
+__all__ = ["Engine", "MultiEngine", "EngineError", "EdwardsPoint", "RistrettoPoint", "MontgomeryPoint", "SignatureError", "verify_batch", "default_engine",
+           "library_path", "load_library", "POINTS_COMPRESSED", "POINTS_EXTENDED", "POINTS_RISTRETTO", "POINTS_MONTGOMERY",
            "VartimeEdwardsPrecomputation", "VartimeRistrettoPrecomputation", "x25519", "x25519_public_keys",
            "X25519_BASEPOINT_BYTES", "ed25519_verifying_keys", "ed25519_sign", "ed25519_sign_prehashed",
-           "ed25519_verify_prehashed"]
+           "ed25519_verify_prehashed", "ed25519_to_montgomery"]

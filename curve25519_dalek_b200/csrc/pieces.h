@@ -67,3 +67,13 @@ static int run_pieces(dalek_b200_ctx *ctx, const uint8_t *msgs, const uint64_t *
     ctx->last_kernel_launches = (int)k;
     return 0;
 }
+
+// clear the staged inputs (ctx->points_in) and results (ctx->points) of a call that handled secrets (zeroize on drop),
+// then wait for the stream
+static inline int wipe_staging(dalek_b200_ctx *ctx, size_t in_bytes, size_t out_bytes)
+{
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->points_in.p, 0, in_bytes, ctx->stream));
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->points.p, 0, out_bytes, ctx->stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    return 0;
+}

@@ -3,6 +3,9 @@
 //                                                                                         of x25519.cuh on the FP64 field
 //   PublicKey::from(&secret) x25519.rs:105-110 -> C/montgomery.rs:164-174   k_x25519_base  mul_base_clamped(k).to_montgomery()
 //                            -> C/edwards.rs:580-590                                       as a constant-time fixed-base comb
+//   EdwardsPoint::mul_base / mul_base_clamped   C/edwards.rs:918-957         k_x25519_base  the same comb, other encoders:
+//   RistrettoPoint::mul_base                    C/ristretto.rs:939                          CompressedEdwardsY, CompressedRistretto
+//   MontgomeryPoint::mul_base / mul_base_clamped C/montgomery.rs:143-174                    or Montgomery u; clamped or not
 // Both are constant time in k and u: no branch, loop bound or address depends on them (x25519.cuh; comb.cuh scans
 // every entry of a table row).  The comb table of the Ed25519 basepoint B (64 x 8 entries (j+1) 16^i B, 60 KiB) is
 // built once per context.  Unlike base.cu's mul_base, which indexes its table by the digit, the comb never reads a
@@ -17,6 +20,8 @@
 #include "engine.h"
 #include "pieces.h"
 #include "x25519.cuh"
+
+static_assert(DALEK_POINTS_MONTGOMERY != DALEK_POINTS_COMPRESSED && DALEK_POINTS_MONTGOMERY != DALEK_POINTS_RISTRETTO, "formats");
 
 static inline unsigned cdiv(size_t a, unsigned b) { return (unsigned)((a + b - 1) / b); }
 
@@ -47,8 +52,12 @@ __global__ void __launch_bounds__(128) k_x25519_base_table(double *__restrict__ 
     comb_entry(table + (size_t)t * COMB_ENTRY, B, t >> 3, t & 7);
 }
 
-// u(clamp(k) B): 64 mixed additions over the radix-16 signed digits of the clamped, unreduced k (< 2^255, so the
-// recoding of scalar.rs:1019-1051 holds), then u = (Z + Y) / (Z - Y) (C/edwards.rs:580-590).
+// s B for the scalar s of item i, encoded as OUT (DALEK_POINTS_COMPRESSED, _RISTRETTO or _MONTGOMERY): 64 mixed additions
+// over the radix-16 signed digits of s, read as it is (CLAMP = 0, bit 255 clear: the value is not reduced, and since B
+// has order l the point is (s mod l) B) or clamped (CLAMP = 1, clamp_integer, C/scalar.rs:1407-1412, not reduced).  Both
+// keep s < 2^255, so the recoding of scalar.rs:1019-1051 holds.  Montgomery u = (Z + Y) / (Z - Y) (C/edwards.rs:580-590);
+// the identity (s = 0 mod l) gives u = 0 like the reference's to_montgomery.
+template <int OUT, int CLAMP>
 __global__ void __launch_bounds__(X25519_COMB_THREADS, 1)
 k_x25519_base(const uint32_t *__restrict__ scalars, const double *__restrict__ table, size_t n, uint32_t *__restrict__ out)
 {
@@ -62,32 +71,50 @@ k_x25519_base(const uint32_t *__restrict__ scalars, const double *__restrict__ t
     comb_mul_base_nibbles(acc, s_tab, [&](int pos) {
         if ((pos & 7) == 0) {                                     // one scalar word per 8 digits, clamped as it is read
             w = scalars[8 * i + (pos >> 3)];
-            w &= pos == 0 ? 0xfffffff8u : 0xffffffffu;
-            w = pos == 56 ? ((w & 0x7fffffffu) | 0x40000000u) : w;
+            if (CLAMP) {
+                w &= pos == 0 ? 0xfffffff8u : 0xffffffffu;
+                w = pos == 56 ? ((w & 0x7fffffffu) | 0x40000000u) : w;
+            }
         }
         const uint32_t v = w & 15;
         w >>= 4;
         return v;
     });
-    fe64 num, den, inv, u;
-    fe64_add(num, acc.Z, acc.Y);                                  // 2
-    fe64_sub(den, acc.Z, acc.Y); fe64_carry(den, den);            // 1
-    x25519_invert(inv, den);
-    fe64_mul(u, num, inv);                                        // 2 x 1
     uint32_t r[8];
-    x25519_encode(r, u);
+    if (OUT == DALEK_POINTS_MONTGOMERY) {
+        fe64 num, den, inv, u;
+        fe64_add(num, acc.Z, acc.Y);                              // 2
+        fe64_sub(den, acc.Z, acc.Y); fe64_carry(den, den);        // 1
+        x25519_invert(inv, den);
+        fe64_mul(u, num, inv);                                    // 2 x 1
+        x25519_encode(r, u);
+    } else {
+        ge_p3 q; ge64_to_p3(q, acc);
+        if (OUT == DALEK_POINTS_RISTRETTO) ristretto_compress<1>(r, q);
+        else ge_compress<1>(r, q);
+    }
 #pragma unroll
     for (int j = 0; j < 8; j++) out[8 * i + j] = r[j];
 }
 
-// the comb table of B, built once per context (with the dynamic shared-memory limit of k_x25519_base)
+template <int OUT, int CLAMP>
+static int x25519_base_smem_attr(dalek_b200_ctx *ctx)
+{
+    CUDA_TRY(ctx, cudaFuncSetAttribute(k_x25519_base<OUT, CLAMP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)(X25519_COMB_DOUBLES * sizeof(double))));
+    return 0;
+}
+
+// the comb table of B, built once per context (with the dynamic shared-memory limit of every k_x25519_base instance)
 int comb_base_table_ensure(dalek_b200_ctx *ctx)
 {
     if (ctx->comb_base_table_ready) return 0;
     int rc;
     if ((rc = ws_reserve(ctx, ctx->comb_base_table, X25519_COMB_DOUBLES * sizeof(double)))) return rc;
-    CUDA_TRY(ctx, cudaFuncSetAttribute(k_x25519_base, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)(X25519_COMB_DOUBLES * sizeof(double))));
+    if ((rc = x25519_base_smem_attr<DALEK_POINTS_MONTGOMERY, 1>(ctx)) || (rc = x25519_base_smem_attr<DALEK_POINTS_MONTGOMERY, 0>(ctx)) ||
+        (rc = x25519_base_smem_attr<DALEK_POINTS_COMPRESSED, 1>(ctx)) || (rc = x25519_base_smem_attr<DALEK_POINTS_COMPRESSED, 0>(ctx)) ||
+        (rc = x25519_base_smem_attr<DALEK_POINTS_RISTRETTO, 0>(ctx)))
+        return rc;
     k_x25519_base_table<<<4, 128, 0, ctx->stream>>>((double *)ctx->comb_base_table.p);
     ctx->launches++;
     CUDA_TRY(ctx, cudaGetLastError());
@@ -101,13 +128,34 @@ static void launch_x25519(const void *d_k, const void *d_u, size_t m, void *d_ou
                                                                (uint32_t *)d_out, (uint8_t *)d_contrib);
 }
 
-// clear the staged scalars / points and the staged results (zeroize on drop), then wait for the stream
-static int wipe_staging(dalek_b200_ctx *ctx, size_t in_bytes, size_t out_bytes)
+// one piece of the fixed-base comb: m scalars at d_k -> m encodings at d_out
+static void launch_x25519_base(int out_fmt, bool clamp, const double *table, const void *d_k, size_t m, void *d_out, cudaStream_t st)
 {
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->points_in.p, 0, in_bytes, ctx->stream));
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->points.p, 0, out_bytes, ctx->stream));
-    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    return 0;
+    const unsigned grid = cdiv(m, X25519_COMB_THREADS);
+    const size_t smem = X25519_COMB_DOUBLES * sizeof(double);
+    const uint32_t *k = (const uint32_t *)d_k;
+    uint32_t *o = (uint32_t *)d_out;
+    if (out_fmt == DALEK_POINTS_MONTGOMERY && clamp) k_x25519_base<DALEK_POINTS_MONTGOMERY, 1><<<grid, X25519_COMB_THREADS, smem, st>>>(k, table, m, o);
+    else if (out_fmt == DALEK_POINTS_MONTGOMERY) k_x25519_base<DALEK_POINTS_MONTGOMERY, 0><<<grid, X25519_COMB_THREADS, smem, st>>>(k, table, m, o);
+    else if (out_fmt == DALEK_POINTS_COMPRESSED && clamp) k_x25519_base<DALEK_POINTS_COMPRESSED, 1><<<grid, X25519_COMB_THREADS, smem, st>>>(k, table, m, o);
+    else if (out_fmt == DALEK_POINTS_COMPRESSED) k_x25519_base<DALEK_POINTS_COMPRESSED, 0><<<grid, X25519_COMB_THREADS, smem, st>>>(k, table, m, o);
+    else k_x25519_base<DALEK_POINTS_RISTRETTO, 0><<<grid, X25519_COMB_THREADS, smem, st>>>(k, table, m, o);
+}
+
+// the fixed-base comb over host buffers: the cached table of B, the batch streamed in pieces, the staging cleared
+static int x25519_base_batch(dalek_b200_ctx *ctx, const uint8_t *scalars, size_t n, int out_fmt, bool clamp, uint8_t *out)
+{
+    int rc;
+    if ((rc = comb_base_table_ensure(ctx))) return rc;
+    const double *table = (const double *)ctx->comb_base_table.p;
+    rc = run_pieces(ctx, nullptr, nullptr, scalars, 32, nullptr, 0, out, 32, nullptr, 0, n,
+                    [&](const uint8_t *, const uint64_t *, const uint8_t *dk, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *,
+                        cudaStream_t st) {
+                        launch_x25519_base(out_fmt, clamp, table, dk, m, d_o, st);
+                        return 0;
+                    });
+    if (rc) return rc;
+    return wipe_staging(ctx, n * 32, n * 32);
 }
 
 extern "C" {
@@ -155,19 +203,28 @@ int dalek_b200_x25519_public_keys(dalek_b200_ctx *ctx, const uint8_t *scalars, s
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     if (!n) return DALEK_OK;
     CallTimer timer(ctx);
-    int rc;
-    if ((rc = comb_base_table_ensure(ctx))) return rc;
-    const double *table = (const double *)ctx->comb_base_table.p;
-    const size_t smem = X25519_COMB_DOUBLES * sizeof(double);
-    rc = run_pieces(ctx, nullptr, nullptr, scalars, 32, nullptr, 0, out, 32, nullptr, 0, n,
-                    [&](const uint8_t *, const uint64_t *, const uint8_t *dk, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *,
-                        cudaStream_t st) {
-                        k_x25519_base<<<cdiv(m, X25519_COMB_THREADS), X25519_COMB_THREADS, smem, st>>>((const uint32_t *)dk, table, m,
-                                                                                                    (uint32_t *)d_o);
-                        return 0;
-                    });
-    if (rc) return rc;
-    return wipe_staging(ctx, n * 32, n * 32);
+    return x25519_base_batch(ctx, scalars, n, DALEK_POINTS_MONTGOMERY, true, out);
+}
+
+int dalek_b200_mul_base_ct_batch(dalek_b200_ctx *ctx, const uint8_t *scalars, size_t n, int out_fmt, int flags, uint8_t *out)
+{
+    if (!ctx || (n && (!scalars || !out))) return DALEK_E_INVALID_ARG;
+    if (out_fmt != DALEK_POINTS_COMPRESSED && out_fmt != DALEK_POINTS_RISTRETTO && out_fmt != DALEK_POINTS_MONTGOMERY) return DALEK_E_INVALID_ARG;
+    if (flags & ~DALEK_MUL_CLAMPED) return DALEK_E_INVALID_ARG;
+    const bool clamp = (flags & DALEK_MUL_CLAMPED) != 0;
+    if (clamp && out_fmt == DALEK_POINTS_RISTRETTO) {
+        ctx->last_error = "clamped multiplication is defined for Edwards and Montgomery points only";
+        return DALEK_E_INVALID_ARG;
+    }
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    if (!n) return DALEK_OK;
+    if (!clamp) {                                                  // Scalar invariant #1 (scalar.rs:214-230): bit 255 clear
+        uint8_t top = 0;
+        for (size_t i = 0; i < n; i++) top |= scalars[32 * i + 31];
+        if (top & 0x80) { ctx->last_error = "scalar with bit 255 set (Scalar invariant #1)"; return DALEK_E_INVALID_ARG; }
+    }
+    CallTimer timer(ctx);
+    return x25519_base_batch(ctx, scalars, n, out_fmt, clamp, out);
 }
 
 }  // extern "C"

@@ -1,12 +1,18 @@
-// x25519.cuh -- the X25519 Montgomery ladder on the FP64 field (fe64.cuh), host-compilable.
+// x25519.cuh -- the Montgomery ladder on the FP64 field (fe64.cuh), host-compilable.
 //
-// x25519(k, u) of x25519-dalek (x25519.rs:390-392) is MontgomeryPoint::mul_clamped (C/montgomery.rs:150-161):
-//   * k is clamped (clamp_integer, C/scalar.rs:1407-1412) and NOT reduced;
-//   * u is read with FieldElement::from_bytes: bit 255 ignored, values in [p, 2^255) accepted as they are;
-//   * Costello-Smith algorithm 8 over bits 254..0 of k, then the final swap on bit 0 (montgomery.rs:183-211);
-//   * as_affine: U * W^(p-2), so W = 0 gives u = 0 (montgomery.rs:409-412).
-// Constant time: the 255 steps run whatever k and u are, the swaps are XOR masks, scalar words are picked by
-// masks over all eight words (no address depends on k), and the canonical encoding is branch-free.
+// mont_ladder<NW> is MontgomeryPoint::mul_bits_be (C/montgomery.rs:176-211) over bits nbits-1..0 of an integer of NW
+// little-endian 32-bit words (NW = 8 or 16, so up to 512 bits):
+//   * u is read with FieldElement::from_bytes: bit 255 ignored, values in [p, 2^255) accepted as they are, twist
+//     points accepted;
+//   * x0 = identity, x1 = (u : 1), prev = 0; one Costello-Smith algorithm 8 step per bit, then the final swap on
+//     the last bit (bit 0);
+//   * as_affine: U * W^(p-2), so W = 0 gives u = 0 (montgomery.rs:409-412); nbits = 0 runs no step and gives u = 0.
+// x25519(k, u) of x25519-dalek (x25519.rs:390-392) is MontgomeryPoint::mul_clamped (C/montgomery.rs:150-161): the
+// 8-word instance over bits 254..0 of the clamped (clamp_integer, C/scalar.rs:1407-1412), NOT reduced k.  Scalar *
+// MontgomeryPoint (montgomery.rs:484-492) is the same instance over the unclamped Scalar (bit 255 clear).
+// Constant time: nbits is public and uniform per call; the steps run whatever k and u are, the swaps are XOR masks,
+// words of k are picked by masks over all NW words (no address depends on k), and the canonical encoding is
+// branch-free.
 //
 // Scale bookkeeping (fe64.cuh:20-22): ladder coordinates have scale 1 between steps; the sums t0, t1, t9, t10 of
 // differential_add_and_double have scale 2 and are carried before they are squared (fe64_sq needs scale < 2).
@@ -51,12 +57,13 @@ FE_HD void x25519_clamp(uint32_t k[8])
     k[7] |= 0x40000000u;
 }
 
-// k[w] selected by masks over all eight words: the word index never becomes a register-array address
-FE_HD uint32_t x25519_word(const uint32_t k[8], int w)
+// k[w] selected by masks over all NW words: the word index never becomes a register-array address
+template <int NW = 8>
+FE_HD uint32_t x25519_word(const uint32_t k[NW], int w)
 {
     uint32_t r = 0;
 #pragma unroll
-    for (int j = 0; j < 8; j++) r |= k[j] & (0u - (uint32_t)(j == w));
+    for (int j = 0; j < NW; j++) r |= k[j] & (0u - (uint32_t)(j == w));
     return r;
 }
 
@@ -113,13 +120,11 @@ FE_HD void x25519_ladder_step(fe64 &U0, fe64 &W0, fe64 &U1, fe64 &W1, const fe64
     fe64_mul(W1, u, t10);                              // t17: W of P + Q
 }
 
-// out = x25519(k, u) as eight canonical little-endian words (montgomery.rs:150-211, :409-412)
-FE_HD void x25519_ladder(uint32_t out[8], const uint32_t k_in[8], const uint32_t u_in[8])
+// out = u([n] P) for u = u(P) (u_in: eight little-endian words) and n = bits nbits-1..0 of k (NW words, nbits <= 32 NW),
+// as eight canonical little-endian words (montgomery.rs:176-211, :409-412)
+template <int NW>
+FE_HD void mont_ladder(uint32_t out[8], const uint32_t k[NW], int nbits, const uint32_t u_in[8])
 {
-    uint32_t k[8];
-#pragma unroll
-    for (int j = 0; j < 8; j++) k[j] = k_in[j];
-    x25519_clamp(k);
     fe64 u, U0, W0, U1, W1;
     fe64_frombytes_words(u, u_in);                     // bit 255 ignored, [p, 2^255) accepted (montgomery.rs:598-605)
     fe64_carry(u, u);                                  // scale 1
@@ -129,18 +134,28 @@ FE_HD void x25519_ladder(uint32_t out[8], const uint32_t k_in[8], const uint32_t
 #if FE64_DEV
 #pragma unroll 1
 #endif
-    for (int i = 254; i >= 0; i--) {
-        const uint32_t bit = (x25519_word(k, i >> 5) >> (i & 31)) & 1u;
+    for (int i = nbits - 1; i >= 0; i--) {
+        const uint32_t bit = (x25519_word<NW>(k, i >> 5) >> (i & 31)) & 1u;
         const uint32_t swap = prev ^ bit;
         fe64_cswap(U0, U1, swap);
         fe64_cswap(W0, W1, swap);
         x25519_ladder_step(U0, W0, U1, W1, u);
         prev = bit;
     }
-    fe64_cswap(U0, U1, prev);                          // prev = bit 0 of the clamped k
+    fe64_cswap(U0, U1, prev);                          // prev = bit 0 of n (0 when nbits = 0)
     fe64_cswap(W0, W1, prev);
     fe64 wi, r;
     x25519_invert(wi, W0);
     fe64_mul(r, U0, wi);
     x25519_encode(out, r);
+}
+
+// out = x25519(k, u) as eight canonical little-endian words (montgomery.rs:150-211, :409-412)
+FE_HD void x25519_ladder(uint32_t out[8], const uint32_t k_in[8], const uint32_t u_in[8])
+{
+    uint32_t k[8];
+#pragma unroll
+    for (int j = 0; j < 8; j++) k[j] = k_in[j];
+    x25519_clamp(k);
+    mont_ladder<8>(out, k, 255, u_in);
 }

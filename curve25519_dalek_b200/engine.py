@@ -6,6 +6,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 POINTS_RISTRETTO = 2
 POINTS_COMPRESSED = 0
 POINTS_EXTENDED = 1
+POINTS_MONTGOMERY = 3        # Montgomery u (an output format of Engine.mul_base_ct_batch)
 
 _lib = None
 
@@ -95,6 +96,11 @@ def load_library():
     lib.dalek_b200_x25519_batch.argtypes = [vp, vp, vp, sz, vp, vp]
     lib.dalek_b200_x25519_batch_dev.argtypes = [vp, vp, vp, sz, vp, vp]
     lib.dalek_b200_x25519_public_keys.argtypes = [vp, vp, sz, vp]
+    lib.dalek_b200_montgomery_mul_batch.argtypes = [vp, vp, sz, vp, sz, sz, vp]
+    lib.dalek_b200_montgomery_mul_batch_dev.argtypes = [vp, vp, sz, vp, sz, sz, vp]
+    lib.dalek_b200_montgomery_mul_bits_be_batch.argtypes = [vp, vp, sz, sz, sz, vp, sz, sz, vp]
+    lib.dalek_b200_montgomery_to_edwards_batch.argtypes = [vp, vp, vp, sz, vp, vp]
+    lib.dalek_b200_mul_base_ct_batch.argtypes = [vp, vp, sz, C.c_int, C.c_int, vp]
     lib.dalek_b200_mul_batch.argtypes = [vp, vp, sz, vp, C.c_int, sz, sz, C.c_int, vp, vp]
     lib.dalek_b200_mul_batch_dev.argtypes = [vp, vp, sz, vp, C.c_int, sz, sz, C.c_int, vp, vp]
     lib.dalek_b200_edwards_torsion_batch.argtypes = [vp, vp, C.c_int, sz, vp]
@@ -345,6 +351,51 @@ class Engine:
         out = (C.c_uint8 * (32 * max(n, 1)))()
         self._check(self.lib.dalek_b200_x25519_public_keys(self.h, _ptr(scalars), n, C.addressof(out)))
         return bytes(out)[:32 * n]
+
+    # ---- MontgomeryPoint ----
+    def montgomery_mul_batch(self, scalars, n_scalars, us, n_points, n, device_ptrs=False, out=None):
+        """Scalar * MontgomeryPoint (dalek_b200_montgomery_mul_batch): out[i] = u([s_i] P_i) for 32-byte scalars (bit 255
+        clear, not clamped) and 32-byte u coordinates; n_scalars and n_points are each 1 (broadcast) or n.  Host buffers
+        give bytes.  With device_ptrs the inputs are device buffers and the results go to `out` (32 n bytes), a new uint8
+        tensor on the engine's device if not given, which is returned."""
+        if device_ptrs:
+            if out is None:
+                import torch
+                out = torch.empty(32 * max(n, 1), dtype=torch.uint8, device=torch.device("cuda", self.device))
+            self._check(self.lib.dalek_b200_montgomery_mul_batch_dev(self.h, _ptr(scalars), n_scalars, _ptr(us), n_points, n,
+                                                                     _ptr(out)))
+            return out
+        res = (C.c_uint8 * (32 * max(n, 1)))()
+        self._check(self.lib.dalek_b200_montgomery_mul_batch(self.h, _ptr(scalars), n_scalars, _ptr(us), n_points, n,
+                                                             C.addressof(res)))
+        return bytes(res)[:32 * n]
+
+    def montgomery_mul_bits_be_batch(self, ints, int_bytes, n_ints, nbits, us, n_points, n):
+        """MontgomeryPoint::mul_bits_be (dalek_b200_montgomery_mul_bits_be_batch): out[i] = u([b_i] P_i), b_i = bits
+        nbits-1..0 of an int_bytes-byte little-endian integer (1 <= int_bytes <= 64, nbits <= 8 int_bytes); n_ints and
+        n_points are each 1 (broadcast) or n.  Host buffers -> n x 32 B."""
+        res = (C.c_uint8 * (32 * max(n, 1)))()
+        self._check(self.lib.dalek_b200_montgomery_mul_bits_be_batch(self.h, _ptr(ints), int_bytes, n_ints, nbits, _ptr(us),
+                                                                     n_points, n, C.addressof(res)))
+        return bytes(res)[:32 * n]
+
+    def montgomery_to_edwards_batch(self, us, signs, n):
+        """MontgomeryPoint::to_edwards (dalek_b200_montgomery_to_edwards_batch) for n u coordinates and n sign bytes:
+        (rc, n x 32 B CompressedEdwardsY, n ok bytes); rc 1 (DALEK_NONE) when some item is None (ok 0, the identity's
+        encoding in its slot)."""
+        res = (C.c_uint8 * (32 * max(n, 1)))()
+        ok = (C.c_uint8 * max(n, 1))()
+        rc = self._check(self.lib.dalek_b200_montgomery_to_edwards_batch(self.h, _ptr(us), _ptr(signs), n, C.addressof(res),
+                                                                         C.addressof(ok)))
+        return rc, bytes(res)[:32 * n], bytes(ok)[:n]
+
+    def mul_base_ct_batch(self, scalars, n, out_fmt=POINTS_COMPRESSED, clamped=False):
+        """s_i B, constant time (dalek_b200_mul_base_ct_batch): out_fmt POINTS_COMPRESSED, POINTS_RISTRETTO or
+        POINTS_MONTGOMERY; scalars with bit 255 clear, or any 32 bytes clamped (not with POINTS_RISTRETTO).  -> n x 32 B"""
+        res = (C.c_uint8 * (32 * max(n, 1)))()
+        self._check(self.lib.dalek_b200_mul_base_ct_batch(self.h, _ptr(scalars), n, out_fmt, 1 if clamped else 0,
+                                                          C.addressof(res)))
+        return bytes(res)[:32 * n]
 
     # ---- variable-base scalar multiplication ----
     def mul_batch(self, scalars, n_scalars, points, n_points, n, point_fmt=POINTS_COMPRESSED, clamped=False, device_ptrs=False,
@@ -745,6 +796,17 @@ class EdwardsPoint:
         return _mul_batch(bytes_list, points, POINTS_COMPRESSED, True, engine)
 
     @staticmethod
+    def mul_base_batch(scalars, engine=None):
+        """EdwardsPoint::mul_base (edwards.rs:918-928) for each 32-byte scalar (bit 255 clear, not reduced: the point is
+        (s mod l) B), constant time at every batch size.  Returns the CompressedEdwardsY, or the list."""
+        return _mul_base_batch(scalars, POINTS_COMPRESSED, False, engine)
+
+    @staticmethod
+    def mul_base_clamped_batch(bytes_list, engine=None):
+        """EdwardsPoint::mul_base_clamped (edwards.rs:944-957): any 32 bytes, clamped and not reduced; like mul_base_batch."""
+        return _mul_base_batch(bytes_list, POINTS_COMPRESSED, True, engine)
+
+    @staticmethod
     def vartime_double_scalar_mul_basepoint_batch(a_list, points, b_list, engine=None):
         """EdwardsPoint::vartime_double_scalar_mul_basepoint (edwards.rs:1078-1087) for each item: a_i * A_i + b_i * B with
         32-byte scalars (bit 255 clear, not reduced) and CompressedEdwardsY points A_i.  Returns the list of 32-byte
@@ -795,6 +857,108 @@ def _mul_batch(scalars, points, fmt, clamped, engine):
         raise ValueError("a point does not decode")
     outs = [raw[32 * i:32 * i + 32] for i in range(n)]
     return outs[0] if single_s and single_p else outs
+
+
+def _mul_base_batch(scalars, fmt, clamped, engine):
+    single, ss = _items(scalars, 32, "scalars")
+    if not ss:
+        return []
+    if not clamped and any(s[31] & 0x80 for s in ss):
+        raise ValueError("a scalar has bit 255 set")
+    eng = engine or default_engine()
+    raw = eng.mul_base_ct_batch(b"".join(ss), len(ss), fmt, clamped=clamped)
+    outs = [raw[32 * i:32 * i + 32] for i in range(len(ss))]
+    return outs[0] if single else outs
+
+
+class MontgomeryPoint:
+    """Mirror of curve25519_dalek::montgomery::MontgomeryPoint (montgomery.rs).  Points are their 32-byte u coordinates,
+    read like FieldElement::from_bytes (bit 255 ignored, values in [p, 2^255) accepted, twist points accepted); results
+    are canonical.  One item gives one result, a list gives the list; a single scalar or point is used for every item."""
+
+    @staticmethod
+    def mul_batch(scalars, points, engine=None):
+        """Scalar * MontgomeryPoint (montgomery.rs:484-505): u([s] P) for 32-byte scalars with bit 255 clear (not clamped,
+        not reduced), constant time."""
+        single_s, ss = _items(scalars, 32, "scalars")
+        single_p, ps = _items(points, 32, "points")
+        n = _broadcast_len(single_s, ss, single_p, ps)
+        if n == 0:
+            return []
+        if any(s[31] & 0x80 for s in ss):
+            raise ValueError("a scalar has bit 255 set")
+        eng = engine or default_engine()
+        raw = eng.montgomery_mul_batch(b"".join(ss), len(ss), b"".join(ps), len(ps), n)
+        outs = [raw[32 * i:32 * i + 32] for i in range(n)]
+        return outs[0] if single_s and single_p else outs
+
+    @staticmethod
+    def mul_bits_be_batch(ints, nbits, points, engine=None):
+        """MontgomeryPoint::mul_bits_be (montgomery.rs:176-211) over bits nbits-1..0 of little-endian integers of one
+        common length of 1..64 bytes (nbits <= 8 x that length), constant time in the bits."""
+        single_i = isinstance(ints, (bytes, bytearray))
+        items = [bytes(ints)] if single_i else [bytes(x) for x in ints]
+        int_bytes = len(items[0]) if items else 1
+        if any(len(x) != int_bytes for x in items) or not 1 <= int_bytes <= 64:
+            raise ValueError("the integers are 1..64 bytes each, all of one length")
+        if not 0 <= nbits <= 8 * int_bytes:
+            raise ValueError("nbits must be between 0 and 8 x the integers' length")
+        single_p, ps = _items(points, 32, "points")
+        n = _broadcast_len(single_i, items, single_p, ps)
+        if n == 0:
+            return []
+        eng = engine or default_engine()
+        raw = eng.montgomery_mul_bits_be_batch(b"".join(items), int_bytes, len(items), nbits, b"".join(ps), len(ps), n)
+        outs = [raw[32 * i:32 * i + 32] for i in range(n)]
+        return outs[0] if single_i and single_p else outs
+
+    @staticmethod
+    def to_edwards_batch(points, signs, engine=None):
+        """MontgomeryPoint::to_edwards (montgomery.rs:223-268) for each u coordinate with its sign (a u8: only bit 0
+        counts; one int is used for every item): the CompressedEdwardsY of the point, or None for u = -1 and for u of the
+        twist.  Returns a list."""
+        _, ps = _items(points, 32, "points")
+        sg = [signs] * len(ps) if isinstance(signs, int) else [int(x) for x in signs]
+        if len(sg) != len(ps):
+            raise ValueError("one sign per point")
+        if any(not 0 <= x <= 255 for x in sg):
+            raise ValueError("signs are u8 values")
+        if not ps:
+            return []
+        eng = engine or default_engine()
+        _, raw, ok = eng.montgomery_to_edwards_batch(b"".join(ps), bytes(sg), len(ps))
+        return [raw[32 * i:32 * i + 32] if ok[i] else None for i in range(len(ps))]
+
+    @staticmethod
+    def mul_base_batch(scalars, engine=None):
+        """MontgomeryPoint::mul_base (montgomery.rs:143-146): u(s B) for 32-byte scalars with bit 255 clear, constant time."""
+        return _mul_base_batch(scalars, POINTS_MONTGOMERY, False, engine)
+
+    @staticmethod
+    def mul_clamped_batch(bytes_list, points, engine=None):
+        """MontgomeryPoint::mul_clamped (montgomery.rs:150-161): x25519(bytes, u), through the X25519 batch."""
+        single_s, ss = _items(bytes_list, 32, "scalars")
+        single_p, ps = _items(points, 32, "points")
+        n = _broadcast_len(single_s, ss, single_p, ps)
+        if n == 0:
+            return []
+        outs = x25519(ss * n if len(ss) == 1 else ss, ps * n if len(ps) == 1 else ps, engine=engine)
+        return outs[0] if single_s and single_p else outs
+
+    @staticmethod
+    def mul_base_clamped_batch(bytes_list, engine=None):
+        """MontgomeryPoint::mul_base_clamped (montgomery.rs:164-174): the X25519 public key of each 32-byte secret."""
+        single, ss = _items(bytes_list, 32, "scalars")
+        if not ss:
+            return []
+        outs = x25519_public_keys(ss, engine=engine)
+        return outs[0] if single else outs
+
+
+def _broadcast_len(single_a, a, single_b, b):
+    if not single_a and not single_b and len(a) != len(b):
+        raise ValueError("the inputs must have the same length (or one of them be a single item)")
+    return len(b) if single_a else len(a)
 
 
 def _double_base_batch(a_list, points, b_list, fmt, engine):
@@ -889,6 +1053,19 @@ def ed25519_verifying_keys(seeds, engine=None):
     eng = engine or default_engine()
     raw = eng.verifying_keys(b"".join(ks), len(ks))
     outs = [raw[32 * i:32 * i + 32] for i in range(len(ks))]
+    return outs[0] if single else outs
+
+
+def ed25519_to_montgomery(verifying_keys, engine=None):
+    """VerifyingKey::to_montgomery (ed25519-dalek verifying.rs:476): the Montgomery u of each 32-byte verifying key, None
+    for a key that does not decompress.  One key gives one result, a list gives the list."""
+    single, ks = _items(verifying_keys, 32, "verifying keys")
+    if not ks:
+        return []
+    eng = engine or default_engine()
+    _, limbs, ok = eng.decompress_batch(b"".join(ks), len(ks))
+    raw = eng.edwards_to_montgomery_batch(limbs, len(ks))
+    outs = [raw[32 * i:32 * i + 32] if ok[i] else None for i in range(len(ks))]
     return outs[0] if single else outs
 
 
@@ -1070,6 +1247,12 @@ class RistrettoPoint:
         CompressedRistretto; a single scalar or a single point is used for every item.  Returns the CompressedRistretto
         of the product, or the list.  An undecodable point raises ValueError."""
         return _mul_batch(scalars, points, POINTS_RISTRETTO, False, engine)
+
+    @staticmethod
+    def mul_base_batch(scalars, engine=None):
+        """RistrettoPoint::mul_base (ristretto.rs:939) for each 32-byte scalar (bit 255 clear), constant time at every batch
+        size.  Returns the CompressedRistretto, or the list."""
+        return _mul_base_batch(scalars, POINTS_RISTRETTO, False, engine)
 
     @staticmethod
     def vartime_double_scalar_mul_basepoint_batch(a_list, points, b_list, engine=None):

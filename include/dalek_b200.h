@@ -52,6 +52,7 @@ typedef struct dalek_b200_ctx dalek_b200_ctx;
 #define DALEK_POINTS_COMPRESSED 0         /* n x 32 B CompressedEdwardsY */
 #define DALEK_POINTS_EXTENDED 1           /* n x 20 x u64 radix-2^51 limbs */
 #define DALEK_POINTS_RISTRETTO 2          /* n x 32 B CompressedRistretto (precomputation API and variable-base multiplication) */
+#define DALEK_POINTS_MONTGOMERY 3         /* n x 32 B MontgomeryPoint u, canonical (output of dalek_b200_mul_base_ct_batch only) */
 
 /* -------- context ---------------------------------------------------------------------- */
 /* Create an engine context on CUDA device `device`.  Fails (no CPU fallback) if the device
@@ -86,7 +87,7 @@ int dalek_b200_last_kernel_ms(const dalek_b200_ctx *ctx, float *ms, int *launche
 int dalek_b200_last_stage_ms(const dalek_b200_ctx *ctx, const char *stage, float *ms);
 /* Milliseconds between CUDA events recorded on the context's stream at entry of the last MSM / verify_batch /
  * precomputed-MSM / X25519 / to_montgomery_batch / hash-to-group / Lizard / map_to_curve / map_to_curve_inverse / mul_batch
- * / vartime_double_base_batch call, or of the last ed25519_b200_verifying_keys /
+ * / vartime_double_base_batch / MontgomeryPoint / mul_base_ct_batch call, or of the last ed25519_b200_verifying_keys /
  * sign_flat / sign_prehashed / verify_prehashed_each call, and after the last work it enqueued (all of the call's streams
  * joined): the device time of that call, copies of host-buffer calls included. */
 int dalek_b200_last_call_ms(const dalek_b200_ctx *ctx, float *ms);
@@ -243,6 +244,53 @@ int dalek_b200_x25519_batch_dev(dalek_b200_ctx *ctx, const void *d_scalars, cons
                                 void *d_out, void *d_contributory);
 /* PublicKey::from(&StaticSecret) = mul_base_clamped(k).to_montgomery(); out: n x 32 B */
 int dalek_b200_x25519_public_keys(dalek_b200_ctx *ctx, const uint8_t *scalars, size_t n, uint8_t *out);
+
+/* -------- MontgomeryPoint (C/montgomery.rs) -------------------------------------------------------
+ * u coordinates are 32 bytes read like FieldElement::from_bytes (bit 255 ignored, values in [p, 2^255) accepted, points
+ * of the twist accepted); results are canonical.  Broadcast: n_scalars / n_ints and n_points are each 1 or n; 1 uses
+ * that input for every item, any other value is DALEK_E_INVALID_ARG.  n = 0 is a successful no-op; a NULL buffer with
+ * n > 0 is DALEK_E_INVALID_ARG, except ok.  The ladders are constant time in the scalars / integers and in u: nbits is
+ * public, the swaps are XOR masks and no address depends on a bit.  Host-buffer calls stream the batch in pieces like
+ * the codecs and clear the device copies of the scalars and results before they return.
+ *
+ * Scalar * MontgomeryPoint (C/montgomery.rs:484-505): out[i] = u([s_i] P_i), the ladder over bits 254..0 of the
+ * unclamped, unreduced Scalar s_i.  A scalar with bit 255 set (Scalar invariant #1) is DALEK_E_INVALID_ARG before any
+ * device work.  mul_clamped (montgomery.rs:150-161) is dalek_b200_x25519_batch. */
+int dalek_b200_montgomery_mul_batch(dalek_b200_ctx *ctx, const uint8_t *scalars, size_t n_scalars, const uint8_t *us,
+                                    size_t n_points, size_t n, uint8_t *out /* n x 32 B */);
+/* same, every buffer a device pointer; blocks until done.  A scalar with bit 255 set is reported after the batch ran:
+ * the call returns DALEK_E_INVALID_ARG and the outputs are unspecified. */
+int dalek_b200_montgomery_mul_batch_dev(dalek_b200_ctx *ctx, const void *d_scalars, size_t n_scalars, const void *d_us,
+                                        size_t n_points, size_t n, void *d_out);
+/* MontgomeryPoint::mul_bits_be (C/montgomery.rs:176-211): out[i] = u([b_i] P_i) for the integer b_i given by bits
+ * nbits-1..0 of ints[i], an int_bytes-byte little-endian integer (1 <= int_bytes <= 64, 0 <= nbits <= 8 int_bytes;
+ * otherwise DALEK_E_INVALID_ARG).  The ladder runs one step per bit from bit nbits-1 down, whatever the bits are;
+ * nbits = 0 gives u = 0 (as_affine of the identity, montgomery.rs:409-412).  Any bit values are accepted. */
+int dalek_b200_montgomery_mul_bits_be_batch(dalek_b200_ctx *ctx, const uint8_t *ints, size_t int_bytes, size_t n_ints,
+                                            size_t nbits, const uint8_t *us, size_t n_points, size_t n,
+                                            uint8_t *out /* n x 32 B */);
+/* MontgomeryPoint::to_edwards (C/montgomery.rs:223-268): y = (u - 1) / (u + 1), bit 7 of its last byte flipped by bit 0
+ * of signs[i] (the u8 shift of the reference), then CompressedEdwardsY::decompress (C/edwards.rs:211-257).  out[i] is
+ * the CompressedEdwardsY of the point.  u = -1 (either encoding) and u of the twist are None: ok[i] = 0, the identity's
+ * encoding in the slot and the call returns DALEK_NONE; every other ok[i] is 1.  Host buffers, streamed in pieces. */
+int dalek_b200_montgomery_to_edwards_batch(dalek_b200_ctx *ctx, const uint8_t *us, const uint8_t *signs /* n bytes */,
+                                           size_t n, uint8_t *out /* n x 32 B */, uint8_t *ok /* n bytes, nullable */);
+
+/* -------- constant-time fixed-base scalar multiplication ------------------------------------------
+ * out[i] = s_i B, B the Ed25519 basepoint: EdwardsPoint::mul_base / mul_base_clamped (C/edwards.rs:918-957),
+ * RistrettoPoint::mul_base (C/ristretto.rs:939) and MontgomeryPoint::mul_base / mul_base_clamped (C/montgomery.rs:143-174,
+ * EdwardsPoint::mul_base(s).to_montgomery()).  out_fmt: DALEK_POINTS_COMPRESSED (CompressedEdwardsY),
+ * DALEK_POINTS_RISTRETTO (CompressedRistretto) or DALEK_POINTS_MONTGOMERY (u), 32 B each; anything else is
+ * DALEK_E_INVALID_ARG.  flags = 0: scalars with bit 255 clear (else DALEK_E_INVALID_ARG), not reduced; as B has order l the
+ * point is (s mod l) B.  flags = DALEK_MUL_CLAMPED: any 32 bytes, clamped (clamp_integer, C/scalar.rs:1407-1412); the
+ * reference has no RistrettoPoint::mul_base_clamped, so the flag with RISTRETTO is DALEK_E_INVALID_ARG.  Other flag bits
+ * are DALEK_E_INVALID_ARG.  n = 0 is a successful no-op; a NULL buffer with n > 0 is DALEK_E_INVALID_ARG.
+ * Constant time in the scalars at every batch size: the comb of dalek_b200_x25519_public_keys over the context's cached
+ * table of B, every table row scanned in full.  Host buffers, streamed in pieces; the device copies of the scalars and
+ * results are cleared before the call returns.  (dalek_b200_edwards_mul_base_batch indexes its table by the digit and is
+ * for public scalars only.) */
+int dalek_b200_mul_base_ct_batch(dalek_b200_ctx *ctx, const uint8_t *scalars, size_t n, int out_fmt, int flags,
+                                 uint8_t *out /* n x 32 B */);
 
 /* -------- variable-base scalar multiplication -------------------------------------------------
  * out[i] = s_i * P_i: EdwardsPoint * Scalar (C/edwards.rs:890-899 -> C/backend/serial/scalar_mul/variable_base.rs:11-48),
