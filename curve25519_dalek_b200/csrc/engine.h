@@ -64,6 +64,7 @@ struct dalek_b200_ctx {
     bool base_table_ready = false;
     bool each_attr_set = false;     // the same for k_verify_each_comb
     bool comb_attr_set = false;     // cudaFuncAttributeMaxDynamicSharedMemorySize set for the comb kernel on this device
+    bool sort_attr_set = false;     // the same for the two digit-sort kernels of msm.cu, at their call-independent bounds
     DevBuf comb_base_table;         // comb table of the Ed25519 basepoint (comb.cuh) for X25519 public keys and signing, built once
     bool comb_base_table_ready = false;
     DevBuf mb_ws[2];                // batched MSMs (msm_batch.cu): the workspace of the pieces on each of the two streams

@@ -47,7 +47,11 @@ int ws_reserve(dalek_b200_ctx *ctx, DevBuf &b, size_t bytes)
     if (b.p) { cudaFree(b.p); b.p = nullptr; b.cap = 0; }
     size_t want = bytes + bytes / 8 + 256;
     cudaError_t e = cudaMalloc(&b.p, want);
-    if (e != cudaSuccess) { ctx->last_error = std::string("cudaMalloc: ") + cudaGetErrorString(e); return DALEK_E_NOMEM; }
+    if (e != cudaSuccess) {
+        ctx->last_error = std::string("cudaMalloc: ") + cudaGetErrorString(e);
+        (void)cudaGetLastError();        // else the next CUDA_TRY(cudaGetLastError()) of this host thread reports it
+        return DALEK_E_NOMEM;
+    }
     b.cap = want;
     return 0;
 }
@@ -58,7 +62,11 @@ int pinned_reserve(dalek_b200_ctx *ctx, size_t bytes)
     if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
     ctx->h_pinned = nullptr; ctx->h_pinned_cap = 0;
     cudaError_t e = cudaMallocHost(&ctx->h_pinned, bytes + 4096);
-    if (e != cudaSuccess) { ctx->last_error = std::string("cudaMallocHost: ") + cudaGetErrorString(e); return DALEK_E_NOMEM; }
+    if (e != cudaSuccess) {
+        ctx->last_error = std::string("cudaMallocHost: ") + cudaGetErrorString(e);
+        (void)cudaGetLastError();
+        return DALEK_E_NOMEM;
+    }
     ctx->h_pinned_cap = bytes + 4096;
     return 0;
 }
@@ -432,6 +440,12 @@ int msm_choose_window_bits_mixed(const dalek_b200_ctx *ctx, size_t n_short, int 
 #define SORT_FINE_MAX 12          // fine bits
 #define SORT_BIN_MEAN 4096u       // coarse bins are added while their mean size on uniform digits is above this
 #define SORT_FINE_CAP 8192u       // records of a coarse bin (or of a slice of a bigger one) k_sort_fine holds in shared memory
+// Dynamic shared memory of the two sort kernels at the largest nc and F msm_sort_fine_bits can pick (49284 B and
+// 114820 B).  The limit a launch is checked against belongs to the kernel on the device, not to a context: a per-call
+// value set by one context would lower the limit under a concurrent call of another context with a larger nc or F.
+// So every context sets these call-independent bounds once, and each launch passes its own, smaller size.
+#define SORT_PART_SMEM_MAX (SORT_TILE * 8 + (2 * SORT_NC_MAX + 33) * 4)
+#define SORT_FINE_SMEM_MAX (SORT_FINE_CAP * 12 + ((1u << SORT_FINE_MAX) + 33) * 4)
 
 // Digit of the lowest remaining window of s (tests/msm_digit_cases.py): s is shifted right by c, carry in and out.
 __device__ __forceinline__ int32_t next_digit(uint32_t s[8], uint32_t &carry, int c)
@@ -1254,8 +1268,15 @@ int msm_accumulate_chunk(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const g
 
     const size_t part_smem = SORT_TILE * 8 + (2 * (size_t)nc + 33) * 4;
     const size_t fine_smem = SORT_FINE_CAP * 12 + ((1u << F) + 33) * 4;
-    CUDA_TRY(ctx, cudaFuncSetAttribute(k_sort_partition, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)part_smem));
-    CUDA_TRY(ctx, cudaFuncSetAttribute(k_sort_fine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fine_smem));
+    if (part_smem > SORT_PART_SMEM_MAX || fine_smem > SORT_FINE_SMEM_MAX) {   // msm_sort_fine_bits keeps nc and F in bounds
+        ctx->last_error = "msm_accumulate_chunk: digit sort needs more shared memory than its bound";
+        return DALEK_E_CUDA;
+    }
+    if (!ctx->sort_attr_set) {
+        CUDA_TRY(ctx, cudaFuncSetAttribute(k_sort_partition, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SORT_PART_SMEM_MAX));
+        CUDA_TRY(ctx, cudaFuncSetAttribute(k_sort_fine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SORT_FINE_SMEM_MAX));
+        ctx->sort_attr_set = true;
+    }
     CUDA_TRY(ctx, cudaMemsetAsync(ccount, 0, ((size_t)nwin * nc + 1) * 4, st));
     CUDA_TRY(ctx, cudaMemsetAsync(t_hist, 0, 2 * TASK_BINS * 4, st));
     if (n) {
@@ -1268,10 +1289,12 @@ int msm_accumulate_chunk(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const g
         k_sort_partition<<<cdiv(n, SORT_TILE), SORT_THREADS, part_smem, st>>>((const uint4 *)d_scalars, n, c, nact, F, nc, nb, flat,
                                                                               ccount, ccursor, records, counts);
         ctx->launches++;
+        CUDA_TRY(ctx, cudaGetLastError());     // a lost sort launch leaves records unwritten: enqueue nothing that reads them
     }
     const size_t extra = n * (size_t)nact / SORT_FINE_CAP;          // bounds the extra slices of all big bins
     k_sort_fine<<<(unsigned)(nwin * nc + extra), SORT_THREADS, fine_smem, st>>>(records, ccount, ccursor, xpre, xtot, n, F, nc, nb,
                                                                                (uint32_t)nwin, flat ? 1 : 0, counts, offsets, sorted, ntasks);
+    CUDA_TRY(ctx, cudaGetLastError());
     k_task_count<<<cdiv(total_buckets, 256), 256, 0, st>>>(counts, (uint32_t)total_buckets, task_len, ntasks, heavy);
     k_scan_partial<<<nwin * parts, 1024, 0, st>>>(ntasks, nb, parts, part_sums);
     k_scan_bases<<<nwin, 32, 0, st>>>(part_sums, parts);

@@ -152,6 +152,7 @@ static int verify_each_dev(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const uin
 #define EACH_K 4                        // signatures per thread of the comb kernel: one shared inversion
 #define EACH_ENT 16                     // doubles per table entry: y+x | y-x | 2dxy as balanced limbs, padded to 128 bytes
 #define EACH_KEY_DOUBLES (64 * 8 * EACH_ENT)
+#define EACH_COMB_SMEM (COMB_BASE_DOUBLES * sizeof(double))   // k_verify_each_comb: the 64 x 8 x 15 table of B (60 KiB)
 
 // one thread per distinct key: decompress, 16^i A for i = 0..63 (63 x 4 doublings), small-order mark
 __global__ void __launch_bounds__(64)
@@ -352,12 +353,11 @@ static int verify_each_comb(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const ui
     if ((rc = ws_reserve(ctx, ctx->each_kstat, f.nkeys))) return rc;
     k_each_key_pow16<<<cdiv(f.nkeys, 64), 64, 0, st>>>(d_keys, f.uniq, f.nkeys, (ge_p3_raw *)ctx->each_pow.p, (uint8_t *)ctx->each_kstat.p);
     k_each_key_rows<<<cdiv(f.nkeys * 512, 128), 128, 0, st>>>((const ge_p3_raw *)ctx->each_pow.p, f.nkeys, (double *)ctx->each_tab.p);
-    const size_t smem = 512 * 15 * sizeof(double);
     if (!ctx->each_attr_set) {
-        CUDA_TRY(ctx, cudaFuncSetAttribute(k_verify_each_comb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(ctx, cudaFuncSetAttribute(k_verify_each_comb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EACH_COMB_SMEM));
         ctx->each_attr_set = true;
     }
-    k_verify_each_comb<<<cdiv((n + EACH_K - 1) / EACH_K, 128), 128, smem, st>>>(d_sigs, f.hs, f.bad_s, f.rep, f.dense, (const uint8_t *)ctx->each_kstat.p,
+    k_verify_each_comb<<<cdiv((n + EACH_K - 1) / EACH_K, 128), 128, EACH_COMB_SMEM, st>>>(d_sigs, f.hs, f.bad_s, f.rep, f.dense, (const uint8_t *)ctx->each_kstat.p,
                                                        (const double *)ctx->each_tab.p, (const ge_niels_packed *)ctx->base_table.p, 0, n, strict, d_out);
     ctx->launches += 3;
     CUDA_TRY(ctx, cudaGetLastError());

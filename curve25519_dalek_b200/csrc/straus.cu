@@ -221,6 +221,7 @@ k_double_base(const uint32_t *__restrict__ a, const uint32_t *__restrict__ b, co
 // lookup scans all 8 entries of a row at warp-uniform addresses with arithmetic masks (window.rs:54-76),
 // and the digit's sign is applied by masked swap / negate inside the addition (comb.cuh).
 #define COMB_ROWS 128          // 2 bases x 64 digit positions
+#define COMB_GH_BYTES ((size_t)COMB_ROWS * 8 * COMB_ENTRY * sizeof(double))   // both tables (120 KiB): device copy and shared memory
 
 __global__ void __launch_bounds__(128)
 k_comb_tables(const uint32_t *__restrict__ GH, double *__restrict__ table, int *__restrict__ status)
@@ -277,9 +278,8 @@ static int double_base_setup(dalek_b200_ctx *ctx, const uint8_t G[32], const uin
 {
     int rc;
     cudaStream_t st = ctx->stream;
-    const size_t comb_bytes = (size_t)COMB_ROWS * 8 * COMB_ENTRY * sizeof(double);
     const size_t head = 64 + 2 * 8 * 40 * 4 + 64;
-    if ((rc = ws_reserve(ctx, ctx->misc0, head + comb_bytes))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->misc0, head + COMB_GH_BYTES))) return rc;
     uint32_t *d_gh = (uint32_t *)ctx->misc0.p;
     uint32_t *d_tables = d_gh + 16;
     plan.d_status = (int *)(d_tables + 640);
@@ -291,11 +291,11 @@ static int double_base_setup(dalek_b200_ctx *ctx, const uint8_t G[32], const uin
     const bool comb = ctx->opt_double_base_comb && n >= 4096;     // the table build only pays off for a real batch
     if (comb) {
         if (!ctx->comb_attr_set) {                               // per context: the attribute is per device
-            CUDA_TRY(ctx, cudaFuncSetAttribute(k_double_base_comb<384>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)comb_bytes));
+            CUDA_TRY(ctx, cudaFuncSetAttribute(k_double_base_comb<384>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)COMB_GH_BYTES));
             ctx->comb_attr_set = true;
         }
         k_comb_tables<<<8, 128, 0, st>>>(d_gh, d_comb, plan.d_status);
-        plan.table = d_comb; plan.variant = 1; plan.smem = comb_bytes;
+        plan.table = d_comb; plan.variant = 1; plan.smem = COMB_GH_BYTES;
     } else {
         k_double_base_tables<<<1, 32, 0, st>>>(d_gh, d_tables, plan.d_status);
         plan.table = d_tables; plan.variant = 0; plan.smem = 0;
