@@ -93,6 +93,20 @@ int dalek_b200_set_option(dalek_b200_ctx *ctx, const char *name, long value)
     return DALEK_E_INVALID_ARG;
 }
 
+int dalek_b200_get_option(const dalek_b200_ctx *ctx, const char *name, long *value)
+{
+    if (!ctx || !name || !value) return DALEK_E_INVALID_ARG;
+    const struct { const char *name; long v; } opts[] = {
+        {"window_bits", ctx->opt_window_bits}, {"host_chunks", ctx->opt_host_chunks}, {"decompress_f64", ctx->opt_decompress_f64},
+        {"trace", ctx->opt_trace}, {"precomp_tables", ctx->opt_precomp_tables}, {"double_base_comb", ctx->opt_double_base_comb},
+        {"dedupe_keys", ctx->opt_dedupe_keys}, {"verify_pieces", ctx->opt_verify_pieces}, {"transcript_warp", ctx->opt_transcript_warp},
+        {"transcript_blocks", ctx->opt_transcript_blocks}, {"each_comb", ctx->opt_each_comb}, {"small_straus", ctx->opt_small_straus},
+        {"acc_tma", ctx->opt_acc_tma}, {"field_f64", ctx->opt_field_f64}, {"verify_chunk", ctx->opt_verify_chunk}};
+    for (const auto &o : opts)
+        if (!strcmp(name, o.name)) { *value = o.v; return 0; }
+    return DALEK_E_INVALID_ARG;
+}
+
 uint64_t dalek_b200_launch_count(const dalek_b200_ctx *ctx) { return ctx ? ctx->launches : 0; }
 
 int dalek_b200_last_kernel_ms(const dalek_b200_ctx *ctx, float *ms, int *launches)

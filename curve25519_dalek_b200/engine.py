@@ -33,6 +33,7 @@ def load_library():
     lib.dalek_b200_last_error.argtypes = [vp]
     lib.dalek_b200_last_error.restype = C.c_char_p
     lib.dalek_b200_set_option.argtypes = [vp, C.c_char_p, C.c_long]
+    lib.dalek_b200_get_option.argtypes = [vp, C.c_char_p, C.POINTER(C.c_long)]
     lib.dalek_b200_launch_count.argtypes = [vp]
     lib.dalek_b200_launch_count.restype = C.c_uint64
     lib.dalek_b200_last_kernel_ms.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]
@@ -185,6 +186,11 @@ class Engine:
 
     def set_option(self, name, value):
         self._check(self.lib.dalek_b200_set_option(self.h, name.encode(), int(value)))
+
+    def get_option(self, name):
+        v = C.c_long()
+        self._check(self.lib.dalek_b200_get_option(self.h, name.encode(), C.byref(v)))
+        return int(v.value)
 
     def launch_count(self):
         return int(self.lib.dalek_b200_launch_count(self.h))

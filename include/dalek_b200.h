@@ -77,6 +77,8 @@ const char *dalek_b200_last_error(const dalek_b200_ctx *ctx);
  * device timeline of verify_batch on stderr).
  * Returns 0 or DALEK_E_INVALID_ARG. */
 int dalek_b200_set_option(dalek_b200_ctx *ctx, const char *name, long value);
+/* The current value of a tunable named as for dalek_b200_set_option, in *value.  Returns 0 or DALEK_E_INVALID_ARG. */
+int dalek_b200_get_option(const dalek_b200_ctx *ctx, const char *name, long *value);
 /* Number of kernels launched by this context since creation (bench.py's gpu_launches). */
 uint64_t dalek_b200_launch_count(const dalek_b200_ctx *ctx);
 /* Milliseconds (CUDA events on the context's stream) spent in the dominant kernel of the last

@@ -16,7 +16,9 @@ pytestmark = pytest.mark.gpu
 def eng():
     import curve25519_dalek_b200 as pkg
     e = pkg.Engine(0)
+    tables = e.get_option("precomp_tables")
     yield e
+    assert e.get_option("precomp_tables") == tables        # no test leaves the option changed
     e.close()
 
 
@@ -166,11 +168,12 @@ def test_precomputed_window_tables(eng, oracle, tables):
     tv = [int.from_bytes(t[i].tobytes(), "little") for i in range(n)]
     uv = [int.from_bytes(u[i].tobytes(), "little") for i in range(nd)]
     B = oracle.basepoint()
+    found = eng.get_option("precomp_tables")
     eng.set_option("precomp_tables", tables)
     try:
         pre = pkg.VartimeEdwardsPrecomputation((limbs, n), engine=eng, fmt=pkg.POINTS_EXTENDED)
     finally:
-        eng.set_option("precomp_tables", 1)
+        eng.set_option("precomp_tables", found)
     for ns in (n, 4097, 1):
         b = rng.integers(0, 256, size=(ns, 32), dtype=np.uint8); b[:, 31] &= 0x1F
         b[0] = 255; b[0, 31] = 0x7F                                   # 2^255 - 1
