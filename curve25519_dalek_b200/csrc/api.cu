@@ -56,11 +56,7 @@ void dalek_b200_destroy(dalek_b200_ctx *ctx)
     cudaStreamSynchronize(ctx->stream2);
     cudaStreamSynchronize(ctx->stream3);
     cudaStreamSynchronize(ctx->stream_hash);
-    DevBuf *bufs[] = {&ctx->scalars, &ctx->points_in, &ctx->points, &ctx->digits, &ctx->counts, &ctx->offsets,
-                      &ctx->sorted, &ctx->buckets, &ctx->red_a, &ctx->red_b, &ctx->red_c, &ctx->red_d, &ctx->key_pts,
-                      &ctx->result, &ctx->flags, &ctx->misc0, &ctx->misc1, &ctx->misc2, &ctx->misc3,
-                      &ctx->misc4, &ctx->misc5, &ctx->zs, &ctx->base_table, &ctx->ntasks, &ctx->task_off, &ctx->tasks, &ctx->task_sums, &ctx->msg_offs, &ctx->sum_desc, &ctx->sum_part, &ctx->key_table, &ctx->key_acc, &ctx->task_order, &ctx->sig_status, &ctx->misc6, &ctx->each_pow, &ctx->each_tab, &ctx->each_kstat, &ctx->comb_base_table, &ctx->prep_prod, &ctx->mb_ws[0], &ctx->mb_ws[1]};
-    for (DevBuf *b : bufs) if (b->p) cudaFree(b->p);
+    for (DevBuf &b : ctx->ws) if (b.p) cudaFree(b.p);
     if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
     cudaEventDestroy(ctx->ev_a); cudaEventDestroy(ctx->ev_b); cudaEventDestroy(ctx->ev_fork); cudaEventDestroy(ctx->ev_join);
     cudaEventDestroy(ctx->ev_join2); cudaEventDestroy(ctx->ev_call0); cudaEventDestroy(ctx->ev_call1);
@@ -135,8 +131,16 @@ int dalek_b200_last_call_ms(const dalek_b200_ctx *ctx, float *ms)
 }  // extern "C"
 
 // ------------------------------------------------------------------------------------------
-// Inputs (host or device) -> bucket sums -> window accumulators (-> result if d_result); ctx->flags[0] is set if a
-// point does not decode.
+int msm_driver_ws_reserve(dalek_b200_ctx *ctx)
+{
+    int rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_WINDOWS], MSM_WINDOWS_MAX * sizeof(ge_p3_raw)))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_RESULT], 3 * sizeof(MsmResult) + 64))) return rc;
+    return ws_reserve(ctx, ctx->ws[WS_FLAGS], FLAG_WORDS * sizeof(int));
+}
+
+// Inputs (host or device) -> bucket sums -> window accumulators (-> result if d_result); the FLAG_STATUS word is set if
+// a point does not decode.
 // Host inputs are streamed in chunks on a dedicated copy stream: while chunk k+1 crosses PCIe,
 // chunk k is converted, sorted and added into the (persistent) bucket sums.
 static int run_msm(dalek_b200_ctx *ctx, const void *scalars, const void *points_in, bool on_device, int point_fmt, size_t n,
@@ -154,24 +158,24 @@ static int run_msm(dalek_b200_ctx *ctx, const void *scalars, const void *points_
     // inversion would only lengthen its latency-bound path
     const int kind = msm_prepared_kind(point_fmt, straus ? PK_PNIELS : PK_NIELS);
     const size_t psz = kind == PK_NIELS ? sizeof(ge_niels_packed) : sizeof(ge_pniels_packed);
-    if ((rc = ws_reserve(ctx, ctx->points, std::max<size_t>(1, n) * psz))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->flags, 64))) return rc;
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->flags.p, 0, 64, st));
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_OUT], std::max<size_t>(1, n) * psz))) return rc;
+    int *d_bad = (int *)ctx->ws[WS_FLAGS].p + FLAG_STATUS;
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->ws[WS_FLAGS].p, 0, FLAG_WORDS * sizeof(int), st));
     if (on_device) {
         if (straus) {
-            if ((rc = msm_prepare_points(ctx, points_in, point_fmt, n, ctx->points.p, (int *)ctx->flags.p, kind))) return rc;
-            if ((rc = straus_vartime_msm(ctx, (const uint32_t *)scalars, ctx->points.p, kind, n, d_result))) return rc;
+            if ((rc = msm_prepare_points(ctx, points_in, point_fmt, n, ctx->ws[WS_STAGING_OUT].p, d_bad, kind))) return rc;
+            if ((rc = straus_vartime_msm(ctx, (const uint32_t *)scalars, ctx->ws[WS_STAGING_OUT].p, kind, n, d_result))) return rc;
         } else {
             // the point conversion (or decompression) runs on the second stream under the digit / sort passes of the main one
             CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, st));
             CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->ev_fork, 0));
-            if ((rc = msm_prepare_points_on(ctx, ctx->stream2, points_in, point_fmt, n, ctx->points.p, (int *)ctx->flags.p))) return rc;
+            if ((rc = msm_prepare_points_on(ctx, ctx->stream2, points_in, point_fmt, n, ctx->ws[WS_STAGING_OUT].p, d_bad))) return rc;
             CUDA_TRY(ctx, cudaEventRecord(ctx->ev_join, ctx->stream2));
-            if ((rc = msm_accumulate_chunk(ctx, (const uint32_t *)scalars, (const ge_niels_packed *)ctx->points.p, n, c, true, 0, 0, ctx->ev_join))) return rc;
+            if ((rc = msm_accumulate_chunk(ctx, (const uint32_t *)scalars, (const ge_niels_packed *)ctx->ws[WS_STAGING_OUT].p, n, c, true, 0, 0, ctx->ev_join))) return rc;
         }
     } else {
-        if ((rc = ws_reserve(ctx, ctx->scalars, std::max<size_t>(1, n) * 32))) return rc;
-        if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * pin))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_SCALARS], std::max<size_t>(1, n) * 32))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_IN], std::max<size_t>(1, n) * pin))) return rc;
         int K = n >= (1u << 18) ? (int)std::min<long>(8, std::max<long>(1, ctx->opt_host_chunks)) : 1;
         CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, st));
         CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream_copy, ctx->ev_fork, 0));
@@ -180,22 +184,22 @@ static int run_msm(dalek_b200_ctx *ctx, const void *scalars, const void *points_
         // in exchange for more copy / compute overlap (tools/sweep_msm_options.py times 1, 2, 4 and 8 chunks)
         for (int k = 0; k < K; k++) {
             const size_t i0 = n * k / K, i1 = n * (k + 1) / K, cnt = i1 - i0;
-            char *ds = (char *)ctx->scalars.p + i0 * 32, *dp = (char *)ctx->points_in.p + i0 * pin;
+            char *ds = (char *)ctx->ws[WS_SCALARS].p + i0 * 32, *dp = (char *)ctx->ws[WS_STAGING_IN].p + i0 * pin;
             if (cnt) {
                 CUDA_TRY(ctx, cudaMemcpyAsync(ds, (const char *)scalars + i0 * 32, cnt * 32, cudaMemcpyHostToDevice, ctx->stream_copy));
                 CUDA_TRY(ctx, cudaMemcpyAsync(dp, (const char *)points_in + i0 * pin, cnt * pin, cudaMemcpyHostToDevice, ctx->stream_copy));
             }
             CUDA_TRY(ctx, cudaEventRecord(ctx->ev_grp[k], ctx->stream_copy));
             CUDA_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_grp[k], 0));
-            char *dq = (char *)ctx->points.p + i0 * psz;
+            char *dq = (char *)ctx->ws[WS_STAGING_OUT].p + i0 * psz;
             if (straus) {                                            // K = 1 for small inputs
-                if ((rc = msm_prepare_points(ctx, dp, point_fmt, cnt, dq, (int *)ctx->flags.p, kind))) return rc;
+                if ((rc = msm_prepare_points(ctx, dp, point_fmt, cnt, dq, d_bad, kind))) return rc;
                 if ((rc = straus_vartime_msm(ctx, (const uint32_t *)ds, dq, kind, cnt, d_result))) return rc;
             } else {
                 // as for device inputs: the chunk's points are converted on the second stream while its digit / sort
                 // passes run on the main one (the normalisation's inversions would otherwise sit on the critical path)
                 CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->ev_grp[k], 0));
-                if ((rc = msm_prepare_points_on(ctx, ctx->stream2, dp, point_fmt, cnt, dq, (int *)ctx->flags.p))) return rc;
+                if ((rc = msm_prepare_points_on(ctx, ctx->stream2, dp, point_fmt, cnt, dq, d_bad))) return rc;
                 CUDA_TRY(ctx, cudaEventRecord(ctx->ev_join, ctx->stream2));
                 if ((rc = msm_accumulate_chunk(ctx, (const uint32_t *)ds, (const ge_niels_packed *)dq, cnt, c, k == 0, 0, 0, ctx->ev_join))) return rc;
             }
@@ -231,14 +235,12 @@ int msm_whole(dalek_b200_ctx *ctx, const void *scalars, const void *points, bool
               uint8_t out_compressed[32], uint64_t out_limbs[20])
 {
     int rc;
-    const int nwin = msm_window_count_for_bits(msm_choose_window_bits(ctx, n));
-    if ((rc = ws_reserve(ctx, ctx->misc0, (size_t)nwin * sizeof(ge_p3_raw)))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->result, sizeof(MsmResult) + 32))) return rc;
-    MsmResult *d_res = (MsmResult *)ctx->result.p;
+    if ((rc = msm_driver_ws_reserve(ctx))) return rc;
+    MsmResult *d_res = (MsmResult *)ctx->ws[WS_MSM_RESULT].p;
     uint32_t *d_enc = point_fmt == DALEK_POINTS_RISTRETTO ? (uint32_t *)(d_res + 1) : nullptr;
-    if ((rc = run_msm(ctx, scalars, points, on_device, point_fmt, n, n, (ge_p3_raw *)ctx->misc0.p, d_res))) return rc;
+    if ((rc = run_msm(ctx, scalars, points, on_device, point_fmt, n, n, (ge_p3_raw *)ctx->ws[WS_MSM_WINDOWS].p, d_res))) return rc;
     if (d_enc && (rc = ristretto_encode_result(ctx, d_res, d_enc))) return rc;
-    return msm_read_result(ctx, d_res, (const int *)ctx->flags.p, d_enc, out_compressed, out_limbs);
+    return msm_read_result(ctx, d_res, (const int *)ctx->ws[WS_FLAGS].p + FLAG_STATUS, d_enc, out_compressed, out_limbs);
 }
 
 // The public entry points check the point format.
@@ -319,7 +321,7 @@ __global__ void k_records_to_windows(const uint64_t *__restrict__ in, int ranks,
 }
 
 // Enqueue the partial MSM of one shard on the context's stream and leave its record (window accumulators +
-// status word) in ctx->misc1; nothing is synchronised.  ev_a .. ev_b bracket the bucket accumulation.
+// status word) in WS_SHARD_RECORD, where ..._partial_async copies it out; nothing is synchronised.  ev_a .. ev_b bracket the bucket accumulation.
 static int partial_enqueue(dalek_b200_ctx *ctx, const void *scalars, const void *points, bool on_device, int point_fmt,
                            size_t n_local, size_t n_shard, int *nwin_out)
 {
@@ -329,11 +331,11 @@ static int partial_enqueue(dalek_b200_ctx *ctx, const void *scalars, const void 
     int rc;
     const int c = msm_choose_window_bits(ctx, n_shard);
     const int nwin = msm_window_count_for_bits(c);
-    if ((rc = ws_reserve(ctx, ctx->misc0, (size_t)nwin * sizeof(ge_p3_raw)))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->misc1, (size_t)nwin * 160 + 8))) return rc;
-    if ((rc = run_msm(ctx, scalars, points, on_device, point_fmt, n_local, n_shard, (ge_p3_raw *)ctx->misc0.p, nullptr))) return rc;
-    k_windows_to_record<<<(nwin + 1 + 63) / 64, 64, 0, ctx->stream>>>((const ge_p3_raw *)ctx->misc0.p, nwin, (const int *)ctx->flags.p,
-                                                                     (uint64_t *)ctx->misc1.p);
+    if ((rc = msm_driver_ws_reserve(ctx))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_SHARD_RECORD], (size_t)nwin * 160 + 8))) return rc;
+    if ((rc = run_msm(ctx, scalars, points, on_device, point_fmt, n_local, n_shard, (ge_p3_raw *)ctx->ws[WS_MSM_WINDOWS].p, nullptr))) return rc;
+    k_windows_to_record<<<(nwin + 1 + 63) / 64, 64, 0, ctx->stream>>>((const ge_p3_raw *)ctx->ws[WS_MSM_WINDOWS].p, nwin, (const int *)ctx->ws[WS_FLAGS].p + FLAG_STATUS,
+                                                                     (uint64_t *)ctx->ws[WS_SHARD_RECORD].p);
     ctx->launches++;
     CUDA_TRY(ctx, cudaGetLastError());
     *nwin_out = nwin;
@@ -355,7 +357,7 @@ static int partial_common(dalek_b200_ctx *ctx, const void *scalars, const void *
     if ((rc = partial_enqueue(ctx, scalars, points, on_device, point_fmt, n_local, n_shard, &nwin))) return rc;
     const size_t bytes = (size_t)nwin * 160 + 8;
     if ((rc = pinned_reserve(ctx, bytes))) return rc;
-    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_pinned, ctx->misc1.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_pinned, ctx->ws[WS_SHARD_RECORD].p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     read_kernel_ms(ctx);
     memcpy(out_windows, ctx->h_pinned, (size_t)nwin * 160);
@@ -374,9 +376,9 @@ int msm_partial_enqueue_record(dalek_b200_ctx *ctx, const void *scalars, const v
     int rc, nwin = 0;
     if ((rc = partial_enqueue(ctx, scalars, points, on_device, point_fmt, n_local, n_shard, &nwin))) return rc;
     if (dst_device >= 0 && dst_device != ctx->device)
-        CUDA_TRY(ctx, cudaMemcpyPeerAsync(d_out_record, dst_device, ctx->misc1.p, ctx->device, (size_t)nwin * 160 + 8, ctx->stream));
+        CUDA_TRY(ctx, cudaMemcpyPeerAsync(d_out_record, dst_device, ctx->ws[WS_SHARD_RECORD].p, ctx->device, (size_t)nwin * 160 + 8, ctx->stream));
     else
-        CUDA_TRY(ctx, cudaMemcpyAsync(d_out_record, ctx->misc1.p, (size_t)nwin * 160 + 8, cudaMemcpyDeviceToDevice, ctx->stream));
+        CUDA_TRY(ctx, cudaMemcpyAsync(d_out_record, ctx->ws[WS_SHARD_RECORD].p, (size_t)nwin * 160 + 8, cudaMemcpyDeviceToDevice, ctx->stream));
     return DALEK_OK;
 }
 
@@ -391,26 +393,25 @@ int msm_combine_records(dalek_b200_ctx *ctx, const void *records, bool on_device
     const int c = msm_choose_window_bits(ctx, n_shard);
     const int nwin = msm_window_count_for_bits(c);
     const size_t cnt = (size_t)ranks * nwin;
-    if ((rc = ws_reserve(ctx, ctx->red_c, cnt * sizeof(ge_p3_raw)))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->flags, 64))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->result, sizeof(MsmResult)))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_COMBINE_WINDOWS], cnt * sizeof(ge_p3_raw)))) return rc;
+    if ((rc = msm_driver_ws_reserve(ctx))) return rc;
     if ((rc = pinned_reserve(ctx, sizeof(MsmResult) + 64))) return rc;
     cudaStream_t st = ctx->stream;
     const void *d_rec = records;
     if (!on_device) {
-        if ((rc = ws_reserve(ctx, ctx->red_d, (size_t)ranks * rec_bytes))) return rc;
-        CUDA_TRY(ctx, cudaMemcpyAsync(ctx->red_d.p, records, (size_t)ranks * rec_bytes, cudaMemcpyHostToDevice, st));
-        d_rec = ctx->red_d.p;
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_COMBINE_RECORDS], (size_t)ranks * rec_bytes))) return rc;
+        CUDA_TRY(ctx, cudaMemcpyAsync(ctx->ws[WS_COMBINE_RECORDS].p, records, (size_t)ranks * rec_bytes, cudaMemcpyHostToDevice, st));
+        d_rec = ctx->ws[WS_COMBINE_RECORDS].p;
     }
-    int *d_bad = (int *)ctx->flags.p + 8;                       // flags[0] belongs to a partial call still in flight
+    int *d_bad = (int *)ctx->ws[WS_FLAGS].p + FLAG_COMBINE;
     CUDA_TRY(ctx, cudaMemsetAsync(d_bad, 0, 4, st));
     k_records_to_windows<<<(unsigned)((cnt + 63) / 64), 64, 0, st>>>((const uint64_t *)d_rec, ranks, nwin, rec_bytes / 8,
-                                                                      (ge_p3_raw *)ctx->red_c.p, d_bad);
+                                                                      (ge_p3_raw *)ctx->ws[WS_COMBINE_WINDOWS].p, d_bad);
     ctx->launches++;
-    if ((rc = msm_combine_windows(ctx, (const ge_p3_raw *)ctx->red_c.p, ranks, nwin, c, (MsmResult *)ctx->result.p))) return rc;
+    if ((rc = msm_combine_windows(ctx, (const ge_p3_raw *)ctx->ws[WS_COMBINE_WINDOWS].p, ranks, nwin, c, (MsmResult *)ctx->ws[WS_MSM_RESULT].p))) return rc;
     MsmResult *h = (MsmResult *)ctx->h_pinned;
     int *h_bad = (int *)((char *)ctx->h_pinned + sizeof(MsmResult));
-    CUDA_TRY(ctx, cudaMemcpyAsync(h, ctx->result.p, sizeof(MsmResult), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(h, ctx->ws[WS_MSM_RESULT].p, sizeof(MsmResult), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(ctx, cudaMemcpyAsync(h_bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
     if (ctx->async_open) CUDA_TRY(ctx, cudaEventRecord(ctx->ev_call1, st));
     CUDA_TRY(ctx, cudaStreamSynchronize(st));

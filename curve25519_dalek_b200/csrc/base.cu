@@ -82,8 +82,8 @@ int base_table_ensure(dalek_b200_ctx *ctx)
 {
     if (ctx->base_table_ready) return 0;
     int rc;
-    if ((rc = ws_reserve(ctx, ctx->base_table, 512 * sizeof(ge_niels_packed)))) return rc;
-    k_build_base_table<<<8, 64, 0, ctx->stream>>>((ge_niels_packed *)ctx->base_table.p);
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_BASE_TABLE], 512 * sizeof(ge_niels_packed)))) return rc;
+    k_build_base_table<<<8, 64, 0, ctx->stream>>>((ge_niels_packed *)ctx->ws[WS_BASE_TABLE].p);
     ctx->launches++;
     CUDA_TRY(ctx, cudaGetLastError());
     ctx->base_table_ready = true;
@@ -101,16 +101,16 @@ int dalek_b200_edwards_mul_base_batch(dalek_b200_ctx *ctx, const uint8_t *scalar
     cudaStream_t st = ctx->stream;
     if ((rc = base_table_ensure(ctx))) return rc;
     if (!n) return 0;
-    if ((rc = ws_reserve(ctx, ctx->scalars, n * 32))) return rc;
-    if (out_limbs && (rc = ws_reserve(ctx, ctx->points_in, n * 160))) return rc;
-    if (out_compressed && (rc = ws_reserve(ctx, ctx->misc1, n * 32))) return rc;
-    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->scalars.p, scalars, n * 32, cudaMemcpyHostToDevice, st));
-    k_mul_base<<<cdiv(n, 128), 128, 0, st>>>((const uint32_t *)ctx->scalars.p, n, (const ge_niels_packed *)ctx->base_table.p,
-                                             out_limbs ? (uint64_t *)ctx->points_in.p : nullptr,
-                                             out_compressed ? (uint32_t *)ctx->misc1.p : nullptr);
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_SCALARS], n * 32))) return rc;
+    if (out_limbs && (rc = ws_reserve(ctx, ctx->ws[WS_STAGING_IN], n * 160))) return rc;
+    if (out_compressed && (rc = ws_reserve(ctx, ctx->ws[WS_STAGING_MSGS], n * 32))) return rc;
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->ws[WS_SCALARS].p, scalars, n * 32, cudaMemcpyHostToDevice, st));
+    k_mul_base<<<cdiv(n, 128), 128, 0, st>>>((const uint32_t *)ctx->ws[WS_SCALARS].p, n, (const ge_niels_packed *)ctx->ws[WS_BASE_TABLE].p,
+                                             out_limbs ? (uint64_t *)ctx->ws[WS_STAGING_IN].p : nullptr,
+                                             out_compressed ? (uint32_t *)ctx->ws[WS_STAGING_MSGS].p : nullptr);
     ctx->launches++;
-    if (out_limbs) CUDA_TRY(ctx, cudaMemcpyAsync(out_limbs, ctx->points_in.p, n * 160, cudaMemcpyDeviceToHost, st));
-    if (out_compressed) CUDA_TRY(ctx, cudaMemcpyAsync(out_compressed, ctx->misc1.p, n * 32, cudaMemcpyDeviceToHost, st));
+    if (out_limbs) CUDA_TRY(ctx, cudaMemcpyAsync(out_limbs, ctx->ws[WS_STAGING_IN].p, n * 160, cudaMemcpyDeviceToHost, st));
+    if (out_compressed) CUDA_TRY(ctx, cudaMemcpyAsync(out_compressed, ctx->ws[WS_STAGING_MSGS].p, n * 32, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(ctx, cudaStreamSynchronize(st));
     return 0;
 }

@@ -27,8 +27,6 @@
 
 static inline unsigned cdiv(size_t a, unsigned b) { return (unsigned)((a + b - 1) / b); }
 
-enum { FLAG_BAD_A = 0, FLAG_BAD_S = 1, FLAG_BAD_R = 2 };
-
 __global__ void __launch_bounds__(128)
 k_hram(const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ offs, const uint32_t *__restrict__ sigs,
        const uint32_t *__restrict__ keys, size_t n, uint32_t *__restrict__ hrams, uint32_t *__restrict__ hs,
@@ -634,30 +632,30 @@ static int verify_reserve(dalek_b200_ctx *ctx, size_t n, VerifyBufs &b)
     int rc;
     const size_t m = 2 * n + 1;
     if (m >= (1ull << 31)) return DALEK_E_INVALID_ARG;
-    if ((rc = ws_reserve(ctx, ctx->misc2, std::max<size_t>(1, n) * 64))) return rc;   // hrams
-    if ((rc = ws_reserve(ctx, ctx->misc3, std::max<size_t>(1, n) * 32))) return rc;   // h_i
-    if ((rc = ws_reserve(ctx, ctx->misc4, std::max<size_t>(1, n) * 32))) return rc;   // z_i s_i
-    if ((rc = ws_reserve(ctx, ctx->zs, std::max<size_t>(1, n) * 16))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->scalars, m * 32))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points, m * sizeof(ge_niels_packed)))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->flags, 64))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->misc5, (size_t)32768 * 9 * 4))) return rc;
-    b.hrams = (uint32_t *)ctx->misc2.p; b.hs = (uint32_t *)ctx->misc3.p; b.zsprod = (uint32_t *)ctx->misc4.p;
-    b.zs = (uint32_t *)ctx->zs.p; b.scalars = (uint32_t *)ctx->scalars.p; b.points = (ge_niels_packed *)ctx->points.p;
-    b.flags = (int *)ctx->flags.p;
+    if ((rc = msm_driver_ws_reserve(ctx))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_VERIFY_HRAM], std::max<size_t>(1, n) * 64))) return rc;   // hrams
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_VERIFY_H], std::max<size_t>(1, n) * 32))) return rc;   // h_i
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_VERIFY_ZS_PROD], std::max<size_t>(1, n) * 32))) return rc;   // z_i s_i
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_VERIFY_Z], std::max<size_t>(1, n) * 16))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_SCALARS], m * 32))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_OUT], m * sizeof(ge_niels_packed)))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_VERIFY_SUMS], (size_t)32768 * 9 * 4))) return rc;
+    b.hrams = (uint32_t *)ctx->ws[WS_VERIFY_HRAM].p; b.hs = (uint32_t *)ctx->ws[WS_VERIFY_H].p; b.zsprod = (uint32_t *)ctx->ws[WS_VERIFY_ZS_PROD].p;
+    b.zs = (uint32_t *)ctx->ws[WS_VERIFY_Z].p; b.scalars = (uint32_t *)ctx->ws[WS_SCALARS].p; b.points = (ge_niels_packed *)ctx->ws[WS_STAGING_OUT].p;
+    b.flags = (int *)ctx->ws[WS_FLAGS].p;
     // key de-duplication table: power of two >= 2n slots, plus rep[n], uniq[n], dense[n] and 16 counters
     size_t tsize = 1024;
     while (tsize < 2 * n) tsize <<= 1;
     const size_t n1 = std::max<size_t>(1, n);
-    if ((rc = ws_reserve(ctx, ctx->key_table, (tsize + 3 * n1 + 16) * 4))) return rc;
-    b.table = (uint32_t *)ctx->key_table.p; b.tmask = (uint32_t)(tsize - 1);
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_VERIFY_KEY_TABLE], (tsize + 3 * n1 + 16) * 4))) return rc;
+    b.table = (uint32_t *)ctx->ws[WS_VERIFY_KEY_TABLE].p; b.tmask = (uint32_t)(tsize - 1);
     b.rep = b.table + tsize; b.uniq = b.rep + n1; b.dense = b.uniq + n1; b.counters = b.dense + n1;
     if (ctx->opt_dedupe_keys) {
         CUDA_TRY(ctx, cudaMemsetAsync(b.table, 0xff, tsize * 4, ctx->stream));
         CUDA_TRY(ctx, cudaMemsetAsync(b.counters, 0, 64, ctx->stream));
     }
-    if ((rc = ws_reserve(ctx, ctx->sig_status, 3 * n1))) return rc;          // per-signature / per-key failure marks
-    b.bad_s = (uint8_t *)ctx->sig_status.p; b.bad_r = b.bad_s + n1; b.bad_key = b.bad_r + n1;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_VERIFY_MARKS], 3 * n1))) return rc;          // per-signature / per-key failure marks
+    b.bad_s = (uint8_t *)ctx->ws[WS_VERIFY_MARKS].p; b.bad_r = b.bad_s + n1; b.bad_key = b.bad_r + n1;
     CUDA_TRY(ctx, cudaMemsetAsync(b.bad_s, 0, 3 * n1, ctx->stream));
     return 0;
 }
@@ -786,8 +784,8 @@ static int verify_equation(dalek_b200_ctx *ctx, const VerifyBufs &b, size_t n, s
     cudaStream_t st = ctx->stream;
     const size_t cnt = hi - lo;
     const uint32_t nsum = (uint32_t)std::min<size_t>(32768, std::max<size_t>(1, cnt));
-    k_sum_partial<<<cdiv(nsum, 128), 128, 0, st>>>(b.zsprod + 8 * lo, cnt, nsum, (uint32_t *)ctx->misc5.p);
-    k_sum_final<<<1, 256, 0, st>>>((const uint32_t *)ctx->misc5.p, nsum, b.scalars);
+    k_sum_partial<<<cdiv(nsum, 128), 128, 0, st>>>(b.zsprod + 8 * lo, cnt, nsum, (uint32_t *)ctx->ws[WS_VERIFY_SUMS].p);
+    k_sum_final<<<1, 256, 0, st>>>((const uint32_t *)ctx->ws[WS_VERIFY_SUMS].p, nsum, b.scalars);
     ctx->launches += 2;
     const bool merged = ctx->opt_dedupe_keys && n;
     if (merged) {
@@ -795,8 +793,8 @@ static int verify_equation(dalek_b200_ctx *ctx, const VerifyBufs &b, size_t n, s
             k_key_gather<<<cdiv(n, 256), 256, 0, st>>>(b.hs, b.uniq, n, b.scalars + 8);
             ctx->launches++;
         } else {
-            if ((rc = ws_reserve(ctx, ctx->key_acc, nkeys * 64))) return rc;
-            unsigned long long *acc = (unsigned long long *)ctx->key_acc.p;
+            if ((rc = ws_reserve(ctx, ctx->ws[WS_VERIFY_KEY_ACC], nkeys * 64))) return rc;
+            unsigned long long *acc = (unsigned long long *)ctx->ws[WS_VERIFY_KEY_ACC].p;
             CUDA_TRY(ctx, cudaMemsetAsync(acc, 0, nkeys * 64, st));
             if (cnt) k_key_accumulate<<<cdiv(cnt, 256), 256, 0, st>>>(b.hs + 8 * lo, b.rep + lo, b.dense, cnt, acc);
             k_key_finalize<<<cdiv(nkeys, 128), 128, 0, st>>>(acc, nkeys, b.scalars + 8);
@@ -807,9 +805,6 @@ static int verify_equation(dalek_b200_ctx *ctx, const VerifyBufs &b, size_t n, s
     // the z_i are 128-bit (batch.rs:224-229): their terms only populate the low windows
     const size_t nlong = merged ? nkeys + 1 : cnt + 1;
     const int c = msm_choose_window_bits_mixed(ctx, cnt, 128, nlong);
-    const int nwin = msm_window_count_for_bits(c);
-    if ((rc = ws_reserve(ctx, ctx->misc0, (size_t)nwin * sizeof(ge_p3_raw)))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->result, sizeof(MsmResult)))) return rc;
     if (merged || cnt == n) {
         if ((rc = msm_accumulate_chunk(ctx, b.scalars, b.points, nlong, c, true))) return rc;
     } else {           // one term per signature, sub-range: the basepoint term, then the keys of the range
@@ -819,10 +814,10 @@ static int verify_equation(dalek_b200_ctx *ctx, const VerifyBufs &b, size_t n, s
     trace_mark(ctx, "key chunk accumulated", st);
     if (cnt && (rc = msm_accumulate_chunk(ctx, b.scalars + 8 * (1 + n + lo), b.points + 1 + n + lo, cnt, c, false, (128 + c) / c))) return rc;
     trace_mark(ctx, "R chunk accumulated", st);
-    if ((rc = msm_reduce_finish(ctx, c, (ge_p3_raw *)ctx->misc0.p, (MsmResult *)ctx->result.p))) return rc;
+    if ((rc = msm_reduce_finish(ctx, c, (ge_p3_raw *)ctx->ws[WS_MSM_WINDOWS].p, (MsmResult *)ctx->ws[WS_MSM_RESULT].p))) return rc;
     trace_mark(ctx, "reduced and combined", st);
     MsmResult *h = (MsmResult *)ctx->h_pinned;
-    CUDA_TRY(ctx, cudaMemcpyAsync(h, ctx->result.p, sizeof(MsmResult), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(h, ctx->ws[WS_MSM_RESULT].p, sizeof(MsmResult), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(ctx, cudaStreamSynchronize(st));
     *is_identity = h->is_identity != 0;
     return 0;
@@ -875,7 +870,7 @@ static int verify_batches_tail(dalek_b200_ctx *ctx, const VerifyCall &call, cons
     const size_t nb = (n + batch - 1) / batch;
     if ((rc = verify_join(ctx, b, n, pieces, &nkeys))) return rc;
     if (nb == 0) return DALEK_OK;
-    if ((rc = ws_reserve(ctx, ctx->misc6, nb))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_ITEM_STATUS], nb))) return rc;
     const int merged = ctx->opt_dedupe_keys ? 1 : 0;
     uint32_t *zh = merged ? b.hs : b.scalars + 8;            // where k_coeffs left z_i h_i
     // The per-batch status (malformed input, small-order defect) is computed on the decompression stream, idle by now, WHILE
@@ -886,14 +881,14 @@ static int verify_batches_tail(dalek_b200_ctx *ctx, const VerifyCall &call, cons
     cudaStream_t ss = ctx->stream2;
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, ctx->stream));
     CUDA_TRY(ctx, cudaStreamWaitEvent(ss, ctx->ev_fork, 0));
-    k_batch_status<<<cdiv(nb, 128), 128, 0, ss>>>(b.bad_s, b.bad_r, b.bad_key, b.rep, b.dense, merged, n, batch, nb, (uint8_t *)ctx->misc6.p);
+    k_batch_status<<<cdiv(nb, 128), 128, 0, ss>>>(b.bad_s, b.bad_r, b.bad_key, b.rep, b.dense, merged, n, batch, nb, (uint8_t *)ctx->ws[WS_ITEM_STATUS].p);
     {   // lanes per batch: enough groups to fill the machine, at least ~8 signatures per lane
         uint32_t G = 1;
         while (G < 32 && (size_t)G * 8 <= batch && nb * G < (size_t)ctx->sm_count * 512) G <<= 1;
-        if ((rc = ws_reserve(ctx, ctx->red_c, nb * sizeof(ge_p3_raw)))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_BATCH_TORSION], nb * sizeof(ge_p3_raw)))) return rc;
         k_batch_torsion<<<cdiv(nb * G, 128), 128, 0, ss>>>(b.zs, zh, b.points + 1 + n, b.points + 1, b.rep, b.dense, merged, n, batch,
-                                                           nb, G, (ge_p3_raw *)ctx->red_c.p);
-        k_batch_torsion_test<<<cdiv(nb, 64), 64, 0, ss>>>((const ge_p3_raw *)ctx->red_c.p, nb, (uint8_t *)ctx->misc6.p);
+                                                           nb, G, (ge_p3_raw *)ctx->ws[WS_BATCH_TORSION].p);
+        k_batch_torsion_test<<<cdiv(nb, 64), 64, 0, ss>>>((const ge_p3_raw *)ctx->ws[WS_BATCH_TORSION].p, nb, (uint8_t *)ctx->ws[WS_ITEM_STATUS].p);
     }
     ctx->launches += 3;
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_join, ss));
@@ -902,7 +897,7 @@ static int verify_batches_tail(dalek_b200_ctx *ctx, const VerifyCall &call, cons
     if ((rc = verify_equation(ctx, b, n, nkeys, 0, n, &all_ok))) return rc;
     CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
     std::vector<uint8_t> status(nb);                                     // (a pageable read-back blocks the host: only now)
-    CUDA_TRY(ctx, cudaMemcpyAsync(status.data(), ctx->misc6.p, nb, cudaMemcpyDeviceToHost, ss));
+    CUDA_TRY(ctx, cudaMemcpyAsync(status.data(), ctx->ws[WS_ITEM_STATUS].p, nb, cudaMemcpyDeviceToHost, ss));
     CUDA_TRY(ctx, cudaStreamSynchronize(ss));
     float first_kernel_ms = elapsed_ms(ctx->ev_a, ctx->ev_b);
     std::vector<uint8_t> eq_ok(nb, 0);
@@ -913,7 +908,7 @@ static int verify_batches_tail(dalek_b200_ctx *ctx, const VerifyCall &call, cons
     if (all_ok) {
         std::fill(eq_ok.begin(), eq_ok.end(), (uint8_t)1);
     } else {
-        k_batch_mask<<<cdiv(n, 256), 256, 0, ctx->stream>>>((const uint8_t *)ctx->misc6.p, n, batch, b.zsprod, zh, b.scalars + 8 * (1 + n));
+        k_batch_mask<<<cdiv(n, 256), 256, 0, ctx->stream>>>((const uint8_t *)ctx->ws[WS_ITEM_STATUS].p, n, batch, b.zsprod, zh, b.scalars + 8 * (1 + n));
         ctx->launches++;
         todo.push_back({0, nb, false});
     }
@@ -951,7 +946,8 @@ static int verify_batches_tail(dalek_b200_ctx *ctx, const VerifyCall &call, cons
 
 // Front end shared with the per-signature verifier (single.cu): SHA-512(R || A || M) mod l (with ph_dom: SHA-512(dom2 ||
 // R || A || PH), d_msgs then holding n 64-byte prehashes and d_offs unused) and the canonical-s marks of every signature, public keys de-duplicated (rep / dense / uniq as in verify_batch).  Synchronises to return the number
-// of distinct keys.  All arrays live in the context's workspaces until the next verify call.
+// of distinct keys.  The arrays stay in their roles (WS_VERIFY_H, WS_VERIFY_MARKS, WS_VERIFY_KEY_TABLE) until the caller's
+// public call returns: nothing the caller runs after this function reserves them.
 int verify_each_front(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const uint64_t *d_offs, const uint32_t *d_sigs, const uint32_t *d_keys,
                       size_t n, EachFront *out, const Sha512Prefix *ph_dom)
 {
@@ -959,7 +955,7 @@ int verify_each_front(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const uint64_t
     VerifyBufs b;
     if ((rc = verify_reserve(ctx, n, b))) return rc;
     cudaStream_t st = ctx->stream;
-    CUDA_TRY(ctx, cudaMemsetAsync(b.flags, 0, 64, st));
+    CUDA_TRY(ctx, cudaMemsetAsync(b.flags, 0, FLAG_WORDS * sizeof(int), st));
     if (!ctx->opt_dedupe_keys) {                       // (verify_reserve only clears the table when merging is on)
         CUDA_TRY(ctx, cudaMemsetAsync(b.table, 0xff, ((size_t)b.tmask + 1) * 4, st));
         CUDA_TRY(ctx, cudaMemsetAsync(b.counters, 0, 64, st));
@@ -1007,26 +1003,26 @@ static int verify_call(dalek_b200_ctx *ctx, int kind, const VerifyArgs &a)
     const uint32_t *d_sigs = (const uint32_t *)a.sigs;
     if (on_device) {
         if ((rc = verify_reserve(ctx, n, b))) return rc;
-        CUDA_TRY(ctx, cudaMemsetAsync(b.flags, 0, 64, ctx->stream));
+        CUDA_TRY(ctx, cudaMemsetAsync(b.flags, 0, FLAG_WORDS * sizeof(int), ctx->stream));
         CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, ctx->stream));
         if ((rc = verify_front(ctx, call, b, msgs, offs, d_sigs, (const uint32_t *)a.keys, n, 0, n, ctx->ev_fork, 0))) return rc;
     } else {
         const uint8_t *sigs = (const uint8_t *)a.sigs, *pubkeys = (const uint8_t *)a.keys;
         const uint64_t *key_points = (const uint64_t *)a.key_points;
         size_t mbytes = n ? (size_t)offs[n] : 0;
-        if ((rc = ws_reserve(ctx, ctx->misc1, mbytes + 16))) return rc;
-        if ((rc = ws_reserve(ctx, ctx->msg_offs, (n + 1) * 8))) return rc;
-        if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * 96))) return rc;   // sigs + keys
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_MSGS], mbytes + 16))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_MSG_OFFSETS], (n + 1) * 8))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_IN], std::max<size_t>(1, n) * 96))) return rc;   // sigs + keys
         if ((rc = verify_reserve(ctx, n, b))) return rc;
-        uint8_t *d_msgs = (uint8_t *)ctx->misc1.p, *d_sig8 = (uint8_t *)ctx->points_in.p, *d_keys = d_sig8 + n * 64;
+        uint8_t *d_msgs = (uint8_t *)ctx->ws[WS_STAGING_MSGS].p, *d_sig8 = (uint8_t *)ctx->ws[WS_STAGING_IN].p, *d_keys = d_sig8 + n * 64;
         if (key_points) {
-            if ((rc = ws_reserve(ctx, ctx->key_pts, std::max<size_t>(1, n) * 160))) return rc;
-            call.d_key_points = (const uint64_t *)ctx->key_pts.p;
+            if ((rc = ws_reserve(ctx, ctx->ws[WS_VERIFY_KEY_POINTS], std::max<size_t>(1, n) * 160))) return rc;
+            call.d_key_points = (const uint64_t *)ctx->ws[WS_VERIFY_KEY_POINTS].p;
         }
-        uint64_t *d_offs = (uint64_t *)ctx->msg_offs.p;
+        uint64_t *d_offs = (uint64_t *)ctx->ws[WS_MSG_OFFSETS].p;
         d_sigs = (const uint32_t *)d_sig8;
         cudaStream_t st = ctx->stream, sc = ctx->stream_copy;
-        CUDA_TRY(ctx, cudaMemsetAsync(b.flags, 0, 64, st));
+        CUDA_TRY(ctx, cudaMemsetAsync(b.flags, 0, FLAG_WORDS * sizeof(int), st));
         CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, st));
         CUDA_TRY(ctx, cudaStreamWaitEvent(sc, ctx->ev_fork, 0));
         // stream the batch in up to 8 pieces (boundaries on call.chunk multiples): the copy of piece k+1
@@ -1044,7 +1040,7 @@ static int verify_call(dalek_b200_ctx *ctx, int kind, const VerifyArgs &a)
                 CUDA_TRY(ctx, cudaMemcpyAsync(d_offs + i0, offs + i0, (cnt + 1) * 8, cudaMemcpyHostToDevice, sc));
                 CUDA_TRY(ctx, cudaMemcpyAsync(d_sig8 + i0 * 64, sigs + i0 * 64, cnt * 64, cudaMemcpyHostToDevice, sc));
                 CUDA_TRY(ctx, cudaMemcpyAsync(d_keys + i0 * 32, pubkeys + i0 * 32, cnt * 32, cudaMemcpyHostToDevice, sc));
-                if (key_points) CUDA_TRY(ctx, cudaMemcpyAsync((char *)ctx->key_pts.p + i0 * 160, key_points + 20 * i0, cnt * 160, cudaMemcpyHostToDevice, sc));
+                if (key_points) CUDA_TRY(ctx, cudaMemcpyAsync((char *)ctx->ws[WS_VERIFY_KEY_POINTS].p + i0 * 160, key_points + 20 * i0, cnt * 160, cudaMemcpyHostToDevice, sc));
             }
             CUDA_TRY(ctx, cudaEventRecord(ctx->ev_grp[k], sc));
             if ((rc = verify_front(ctx, call, b, d_msgs, d_offs, d_sigs, (const uint32_t *)d_keys, n, i0, i1, ctx->ev_grp[k], k))) return rc;
@@ -1132,7 +1128,7 @@ int ed25519_b200_last_zs(dalek_b200_ctx *ctx, uint8_t *zs_out, size_t n)
 {
     if (!ctx || !zs_out || n > ctx->last_zs_n) return DALEK_E_INVALID_ARG;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    if (n) CUDA_TRY(ctx, cudaMemcpy(zs_out, ctx->zs.p, n * 16, cudaMemcpyDeviceToHost));
+    if (n) CUDA_TRY(ctx, cudaMemcpy(zs_out, ctx->ws[WS_VERIFY_Z].p, n * 16, cudaMemcpyDeviceToHost));
     return 0;
 }
 

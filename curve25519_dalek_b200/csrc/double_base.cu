@@ -2,7 +2,7 @@
 //   EdwardsPoint::vartime_double_scalar_mul_basepoint    C/edwards.rs:1078-1087 -> vartime_double_base.rs:23-72
 //   RistrettoPoint::vartime_double_scalar_mul_basepoint  C/ristretto.rs:1051-1063
 // k_vartime_double_base: one thread per item.  It decodes A_i (point_load.cuh), runs double_base.cuh with A_i's 8-entry
-// table in local memory and B's 8 entries (row 0 of ctx->base_table) in shared memory, and encodes the result.  The
+// table in local memory and B's 8 entries (row 0 of WS_BASE_TABLE) in shared memory, and encodes the result.  The
 // scalars are used as given, not reduced: A_i may carry a torsion component, and then a A_i != (a mod l) A_i.
 // Variable time: scalars and points are public, so no staged copy is cleared.
 #include <algorithm>
@@ -81,13 +81,13 @@ static inline bool db_fmt_ok(int f)
     return f == DALEK_POINTS_COMPRESSED || f == DALEK_POINTS_EXTENDED || f == DALEK_POINTS_RISTRETTO;
 }
 
-// B's table and a cleared status word in ctx->misc0
+// B's table and a cleared status word in WS_CALL_SCRATCH
 static int db_setup(dalek_b200_ctx *ctx, int **status)
 {
     int rc;
     if ((rc = base_table_ensure(ctx))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->misc0, 64))) return rc;
-    *status = (int *)ctx->misc0.p;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_CALL_SCRATCH], 64))) return rc;
+    *status = (int *)ctx->ws[WS_CALL_SCRATCH].p;
     CUDA_TRY(ctx, cudaMemsetAsync(*status, 0, 4, ctx->stream));
     return 0;
 }
@@ -116,7 +116,7 @@ int dalek_b200_vartime_double_base_batch(dalek_b200_ctx *ctx, const uint8_t *ab,
     CallTimer timer(ctx);
     int *d_status, rc;
     if ((rc = db_setup(ctx, &d_status))) return rc;
-    const ge_niels_packed *base = (const ge_niels_packed *)ctx->base_table.p;
+    const ge_niels_packed *base = (const ge_niels_packed *)ctx->ws[WS_BASE_TABLE].p;
     rc = run_pieces(ctx, nullptr, nullptr, ab, 64, (const uint8_t *)points, msm_point_bytes(point_fmt), out, 32, ok, ok ? 1 : 0, n,
                     [&](const uint8_t *, const uint64_t *, const uint8_t *d_ab, const uint8_t *d_p, size_t m, uint8_t *d_o, uint8_t *d_ok,
                         cudaStream_t st) {
@@ -138,7 +138,7 @@ int dalek_b200_vartime_double_base_batch_dev(dalek_b200_ctx *ctx, const void *d_
     CallTimer timer(ctx);
     int *d_status, rc;
     if ((rc = db_setup(ctx, &d_status))) return rc;
-    const ge_niels_packed *base = (const ge_niels_packed *)ctx->base_table.p;
+    const ge_niels_packed *base = (const ge_niels_packed *)ctx->ws[WS_BASE_TABLE].p;
     const size_t pin = msm_point_bytes(point_fmt);
     const size_t piece = n >= (1u << 17) ? (size_t)1 << 16 : n;     // the pieces of run_pieces
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, ctx->stream));

@@ -17,6 +17,137 @@ struct DevBuf {
     size_t cap = 0;
 };
 
+// The device workspaces of a context, one per role: the array ws indexed by WsRole.  Each comment names the files that
+// may use the role, the owner first, then its lifetime in brackets: [call] the contents are valid within one public call,
+// [cross-call] they survive until the named later call, [context] built once and kept.  Roles that only hold storage for
+// one call are shared by the families listed; everything that must survive a call, is live while another role of the
+// same files is, or is read by a nested call has a role of its own.  Workspaces grow on demand (ws_reserve) and are
+// reused across calls; WS_FLAGS, WS_MSM_WINDOWS and WS_MSM_RESULT are reserved at their bounds by msm_driver_ws_reserve.
+// tests/test_workspace_roles.py checks the file lists against the sources.
+enum WsRole {
+    // ---- per-item staging of one call, shared by every family that stages items ----
+    // api.cu, base.cu, batch.cu, precomp.cu, scalars.cu, sign.cu, straus.cu [call] 32-byte scalars (MSM scalars, verify's
+    // MSM coefficients, the signer's seeds, the results of the scalar batch calls)
+    WS_SCALARS,
+    // pieces.h, api.cu, base.cu, batch.cu, lizard.cu, precomp.cu, scalars.cu, sign.cu, single.cu, straus.cu, varmul.cu
+    // [call] fixed-width inputs staged from the host: MSM input points, signatures and keys, the inputs of run_pieces
+    WS_STAGING_IN,
+    // pieces.h, api.cu, batch.cu, lizard.cu, precomp.cu, straus.cu, varmul.cu [call] outputs of run_pieces and the
+    // prepared Niels points of an MSM (verify's MSM points)
+    WS_STAGING_OUT,
+    // pieces.h, base.cu, batch.cu, scalars.cu, single.cu, straus.cu [call] flat messages (or fixed-stride prehashes) at
+    // their own offsets; calls that stage no messages keep one-call per-item scratch here: compressed outputs (base.cu),
+    // group products of the scalar inversion (scalars.cu), the decoded Niels points of the constant-time MSM (straus.cu)
+    WS_STAGING_MSGS,
+    // pieces.h, batch.cu, single.cu [call] the n + 1 message offsets of WS_STAGING_MSGS
+    WS_MSG_OFFSETS,
+    // double_base.cu, lizard.cu, montgomery.cu, straus.cu, varmul.cu [call] small per-call scratch: status words,
+    // broadcast operands and tables, the G/H tables of the Ristretto double-base batch
+    WS_CALL_SCRATCH,
+    // ---- tables built once per context ----
+    // base.cu, double_base.cu, single.cu [context] 64 x 8 affine Niels entries (j+1) 16^i B (base_table_ensure)
+    WS_BASE_TABLE,
+    // x25519.cu, sign.cu [context] comb table of B in balanced FP64 doubles (comb_base_table_ensure)
+    WS_COMB_BASE_TABLE,
+    // ---- the MSM drivers ----
+    // api.cu, batch.cu, precomp.cu, scalars.cu, straus.cu [call] status words; slots FLAG_*
+    WS_FLAGS,
+    // api.cu, batch.cu, precomp.cu [call] the window accumulators of one MSM (MSM_WINDOWS_MAX ge_p3_raw), read by
+    // msm_reduce_finish
+    WS_MSM_WINDOWS,
+    // api.cu, batch.cu, precomp.cu, straus.cu [call] MSM results: up to three MsmResult and a 32-byte Ristretto encoding
+    WS_MSM_RESULT,
+    // api.cu [cross-call] a shard's record (nwin x 160 B + status word), from ..._partial_async until ..._combine_dev
+    WS_SHARD_RECORD,
+    // api.cu [call] the host records of msm_combine_records, staged
+    WS_COMBINE_RECORDS,
+    // api.cu [call] the ranks x nwin window accumulators of msm_combine_records
+    WS_COMBINE_WINDOWS,
+    // msm_batch.cu [call] the workspace of the pieces on the main stream
+    WS_MSM_BATCH_0,
+    // msm_batch.cu [call] the workspace of the pieces on the second stream
+    WS_MSM_BATCH_1,
+    // ---- the MSM engine (msm.cu) and the Straus paths that stand in for it ----
+    // msm.cu [call] extended-point preparation: the Z product of each group of points (then its inverse), running products
+    WS_PREP_PROD,
+    // msm.cu, straus_vt.cu [call] the digit sort's records, 8 B per non-zero digit; the NAF digits of the vartime Straus MSM
+    WS_MSM_DIGITS,
+    // msm.cu [call] the sorted point indices
+    WS_MSM_SORTED,
+    // msm.cu [call] bucket counts | coarse counts | heavy list
+    WS_MSM_COUNTS,
+    // msm.cu [call] bucket offsets | scan part sums | coarse bin cursors | extra-slice prefix and counts
+    WS_MSM_OFFSETS,
+    // msm.cu [call] tasks per bucket
+    WS_MSM_NTASKS,
+    // msm.cu [call] first task of each bucket | each window's base
+    WS_MSM_TASK_OFF,
+    // msm.cu [call] the tasks (bucket, first entry)
+    WS_MSM_TASKS,
+    // msm.cu [call] one partial sum per task
+    WS_MSM_TASK_SUMS,
+    // msm.cu [call] task length histogram | cursor | start | order
+    WS_MSM_TASK_ORDER,
+    // msm.cu, straus.cu [call] bucket sums (persistent over the chunks of one call); the per-point accumulators of the
+    // constant-time Straus MSM
+    WS_MSM_BUCKETS,
+    // msm.cu, straus.cu, straus_vt.cu [call] the bucket reduction's pool of running sums; the Straus paths' tables or
+    // partial sums
+    WS_MSM_REDUCE_POOL,
+    // msm.cu, straus_vt.cu [call] per-window sums of the reduction; the vartime Straus MSM's per-warp results
+    WS_MSM_REDUCE_SUMS,
+    // msm.cu [cross-call] the reduction's sum descriptors, kept while the width they were built for (sum_desc_c) repeats
+    WS_MSM_SUM_DESC,
+    // msm.cu [call] the first stage of the reduction's plain sums
+    WS_MSM_SUM_PART,
+    // ---- verification (batch.cu) and the per-signature verifier (single.cu) ----
+    // batch.cu, sign.cu [call] SHA-512(R || A || M), 64 B per signature; in a sign call the signer's expanded keys
+    WS_VERIFY_HRAM,
+    // batch.cu, sign.cu [call] h_i (z_i h_i once merged), 32 B per signature, read by single.cu after verify_each_front;
+    // in a sign call the signer's verifying keys
+    WS_VERIFY_H,
+    // batch.cu [call] z_i s_i
+    WS_VERIFY_ZS_PROD,
+    // batch.cu [cross-call] the 128-bit z_i, until the next verify call (ed25519_b200_last_zs)
+    WS_VERIFY_Z,
+    // batch.cu [call] partial sums of the z_i s_i
+    WS_VERIFY_SUMS,
+    // batch.cu [call] key de-duplication: hash table | rep | uniq | dense | counters, read by single.cu after
+    // verify_each_front
+    WS_VERIFY_KEY_TABLE,
+    // batch.cu [call] per-key sums of z_i h_i over a range of signatures
+    WS_VERIFY_KEY_ACC,
+    // batch.cu [call] failure marks per signature (s, R) and per key, read by single.cu after verify_each_front
+    WS_VERIFY_MARKS,
+    // batch.cu [call] the callers' decompressed key points, staged
+    WS_VERIFY_KEY_POINTS,
+    // batch.cu [call] the small-order sum of each batch of a verify_batches call
+    WS_BATCH_TORSION,
+    // batch.cu, single.cu [call] one status byte per batch (verify_batches) or per signature (verify_each)
+    WS_ITEM_STATUS,
+    // single.cu [call] per-key comb tables of verify_each: the 16^i A powers of each key
+    WS_EACH_POW,
+    // single.cu [call] per-key comb tables of verify_each: the tables
+    WS_EACH_TABLES,
+    // single.cu [call] per-key comb tables of verify_each: each key's status
+    WS_EACH_KEY_STATUS,
+    WS_COUNT
+};
+
+// Slots (int words) of WS_FLAGS.  A call clears the slots it uses before its kernels write them.
+enum {
+    FLAG_STATUS = 0,    // an MSM input point did not decode; a zero scalar in a batch inversion (scalars.cu)
+    FLAG_BAD_A = 0,     // verify: a public key did not decode
+    FLAG_BAD_S = 1,     // verify: an s was not canonical
+    FLAG_BAD_R = 2,     // verify: an R did not decode
+    FLAG_COMBINE = 8,   // msm_combine_records: a record's status word; apart from FLAG_STATUS, which a partial call in
+                        // flight still reads
+    FLAG_WORDS = 16
+};
+
+// window accumulators of an MSM at the narrowest window width, c = 4 (msm_window_count_for_bits)
+#define MSM_WINDOWS_MAX (256 / 4 + 1)
+
 struct dalek_b200_ctx {
     int device = 0;
     int sm_count = 132;
@@ -55,19 +186,14 @@ struct dalek_b200_ctx {
     float last_call_ms = 0.f;
     int last_kernel_launches = 0;
     bool async_open = false;       // a ..._partial_async call is in flight: its device span ends in ..._combine_dev
-    // device workspaces (grown on demand, reused across calls)
-    DevBuf scalars, points_in, points, digits, counts, offsets, sorted, buckets, red_a, red_b, red_c,
-        red_d, key_pts, result, flags, misc0, misc1, misc2, misc3, misc4, misc5, zs, base_table, ntasks, task_off, tasks, task_sums, msg_offs, sum_desc, sum_part, key_table, key_acc, task_order, sig_status, misc6, each_pow, each_tab, each_kstat;
-    DevBuf prep_prod;   // extended-point preparation: the Z product of each group of points (then its inverse), and running products
+    DevBuf ws[WS_COUNT];            // device workspaces, one per role (WsRole)
     uint32_t hash_seed[4] = {0x243F6A88u, 0x85A308D3u, 0x13198A2Eu, 0x03707344u};   // key of the public-key de-duplication hash, redrawn per context
     int sum_desc_c = -1;
     bool base_table_ready = false;
     bool each_attr_set = false;     // the same for k_verify_each_comb
     bool comb_attr_set = false;     // cudaFuncAttributeMaxDynamicSharedMemorySize set for the comb kernel on this device
     bool sort_attr_set = false;     // the same for the two digit-sort kernels of msm.cu, at their call-independent bounds
-    DevBuf comb_base_table;         // comb table of the Ed25519 basepoint (comb.cuh) for X25519 public keys and signing, built once
     bool comb_base_table_ready = false;
-    DevBuf mb_ws[2];                // batched MSMs (msm_batch.cu): the workspace of the pieces on each of the two streams
     // pinned host staging
     void *h_pinned = nullptr;
     size_t h_pinned_cap = 0;
@@ -144,6 +270,8 @@ inline bool flat_messages_ok(const uint8_t *msgs_flat, const uint64_t *offsets, 
 }
 
 int ws_reserve(dalek_b200_ctx *ctx, DevBuf &b, size_t bytes);
+// WS_FLAGS, WS_MSM_WINDOWS and WS_MSM_RESULT at their bounds (api.cu): every call that uses them reserves them here
+int msm_driver_ws_reserve(dalek_b200_ctx *ctx);
 int pinned_reserve(dalek_b200_ctx *ctx, size_t bytes);
 
 // ---- point preparation (msm.cu) ----
@@ -157,7 +285,7 @@ inline size_t msm_point_bytes(int point_fmt) { return point_fmt == DALEK_POINTS_
 // Convert n input points (device memory, format DALEK_POINTS_*) into packed Niels form.
 // Compressed Edwards and Ristretto inputs give affine Niels (decoding yields Z = 1) and set *d_bad (device int) nonzero
 // if any fails to decode.  Extended inputs give affine Niels too, normalised to Z = 1 with one inversion per call (three
-// launches on the given stream, with the context's prep_prod workspace);
+// launches on the given stream, with the context's WS_PREP_PROD workspace);
 // with kind = PK_PNIELS they give projective Niels instead (no inversion, for the latency-bound Straus path).
 // msm_prepared_kind tells which kind a format and a requested kind give.
 int msm_prepare_points(dalek_b200_ctx *ctx, const void *d_in, int point_fmt, size_t n, void *d_out,

@@ -90,8 +90,8 @@ k_map_to_curve_inverse(const uint32_t *__restrict__ points, size_t n, uint4 *__r
 // clear the staged inputs and outputs (the payloads are plaintexts), up to what the workspaces hold, then wait
 static int lizard_wipe(dalek_b200_ctx *ctx, size_t in_bytes, size_t out_bytes)
 {
-    if (ctx->points_in.p) CUDA_TRY(ctx, cudaMemsetAsync(ctx->points_in.p, 0, std::min(in_bytes, ctx->points_in.cap), ctx->stream));
-    if (ctx->points.p) CUDA_TRY(ctx, cudaMemsetAsync(ctx->points.p, 0, std::min(out_bytes, ctx->points.cap), ctx->stream));
+    if (ctx->ws[WS_STAGING_IN].p) CUDA_TRY(ctx, cudaMemsetAsync(ctx->ws[WS_STAGING_IN].p, 0, std::min(in_bytes, ctx->ws[WS_STAGING_IN].cap), ctx->stream));
+    if (ctx->ws[WS_STAGING_OUT].p) CUDA_TRY(ctx, cudaMemsetAsync(ctx->ws[WS_STAGING_OUT].p, 0, std::min(out_bytes, ctx->ws[WS_STAGING_OUT].cap), ctx->stream));
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     return 0;
 }
@@ -173,8 +173,8 @@ int dalek_b200_ristretto_map_to_curve_inverse_batch(dalek_b200_ctx *ctx, const v
     if (!n) return DALEK_OK;
     CallTimer timer(ctx);
     int rc;
-    if ((rc = ws_reserve(ctx, ctx->misc0, 64))) return rc;
-    int *d_bad = (int *)ctx->misc0.p;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_CALL_SCRATCH], 64))) return rc;
+    int *d_bad = (int *)ctx->ws[WS_CALL_SCRATCH].p;
     CUDA_TRY(ctx, cudaMemsetAsync(d_bad, 0, 4, ctx->stream));
     const size_t pin = msm_point_bytes(point_fmt);
     rc = run_pieces(ctx, nullptr, nullptr, (const uint8_t *)points, pin, nullptr, 0, out, 512, (uint8_t *)mask, 2, n,

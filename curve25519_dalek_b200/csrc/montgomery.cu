@@ -22,7 +22,7 @@ static inline unsigned cdiv(size_t a, unsigned b) { return (unsigned)((a + b - 1
 
 #define MONT_THREADS 128
 
-// staging in ctx->misc0: status word, the broadcast integer (up to 64 bytes), the broadcast u
+// staging in WS_CALL_SCRATCH: status word, the broadcast integer (up to 64 bytes), the broadcast u
 #define MT_STATUS 0
 #define MT_INT 64
 #define MT_U 128
@@ -118,14 +118,14 @@ static int mont_read_status(dalek_b200_ctx *ctx, const int *d_status, int *statu
     return 0;
 }
 
-// the ladder over host buffers (arguments already checked, n > 0): broadcast items staged in ctx->misc0, the rest
+// the ladder over host buffers (arguments already checked, n > 0): broadcast items staged in WS_CALL_SCRATCH, the rest
 // streamed in pieces with u first (word-aligned) and the integers second (read bytewise, any int_bytes)
 static int mont_ladder_host(dalek_b200_ctx *ctx, const uint8_t *ints, size_t int_bytes, size_t n_ints, int nbits, const uint8_t *us,
                             size_t n_points, size_t n, uint8_t *out)
 {
     int rc;
-    if ((rc = ws_reserve(ctx, ctx->misc0, MT_BYTES))) return rc;
-    char *base = (char *)ctx->misc0.p;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_CALL_SCRATCH], MT_BYTES))) return rc;
+    char *base = (char *)ctx->ws[WS_CALL_SCRATCH].p;
     const bool bi = n_ints == 1, bu = n_points == 1;
     if (bi) CUDA_TRY(ctx, cudaMemcpyAsync(base + MT_INT, ints, int_bytes, cudaMemcpyHostToDevice, ctx->stream));
     if (bu) CUDA_TRY(ctx, cudaMemcpyAsync(base + MT_U, us, 32, cudaMemcpyHostToDevice, ctx->stream));
@@ -176,8 +176,8 @@ int dalek_b200_montgomery_mul_batch_dev(dalek_b200_ctx *ctx, const void *d_scala
     if (!n) return DALEK_OK;
     CallTimer timer(ctx);
     int rc;
-    if ((rc = ws_reserve(ctx, ctx->misc0, MT_BYTES))) return rc;
-    int *d_status = (int *)((char *)ctx->misc0.p + MT_STATUS);
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_CALL_SCRATCH], MT_BYTES))) return rc;
+    int *d_status = (int *)((char *)ctx->ws[WS_CALL_SCRATCH].p + MT_STATUS);
     CUDA_TRY(ctx, cudaMemsetAsync(d_status, 0, 4, ctx->stream));
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, ctx->stream));
     mont_launch(d_scalars, n_scalars == 1 ? 0 : 32, 32, 255, d_us, n_points == 1 ? 0 : 1, n, d_out, 1, d_status, ctx->stream);
@@ -216,8 +216,8 @@ int dalek_b200_montgomery_to_edwards_batch(dalek_b200_ctx *ctx, const uint8_t *u
     if (!n) return DALEK_OK;
     CallTimer timer(ctx);
     int rc;
-    if ((rc = ws_reserve(ctx, ctx->misc0, MT_BYTES))) return rc;
-    int *d_status = (int *)((char *)ctx->misc0.p + MT_STATUS);
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_CALL_SCRATCH], MT_BYTES))) return rc;
+    int *d_status = (int *)((char *)ctx->ws[WS_CALL_SCRATCH].p + MT_STATUS);
     CUDA_TRY(ctx, cudaMemsetAsync(d_status, 0, 4, ctx->stream));
     const size_t ok_sz = ok ? 1 : 0;
     rc = run_pieces(ctx, nullptr, nullptr, us, 32, signs, 1, out, 32, ok, ok_sz, n,

@@ -370,8 +370,8 @@ int msm_prepare_points_on(dalek_b200_ctx *ctx, cudaStream_t st, const void *d_in
         // other on one stream
         const unsigned G = cdiv(n, PREP_GROUP);
         int rc;
-        if ((rc = ws_reserve(ctx, ctx->prep_prod, 2 * (size_t)G * sizeof(fe64)))) return rc;
-        fe64 *prod = (fe64 *)ctx->prep_prod.p;
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_PREP_PROD], 2 * (size_t)G * sizeof(fe64)))) return rc;
+        fe64 *prod = (fe64 *)ctx->ws[WS_PREP_PROD].p;
         k_prep_zprod<<<G, PREP_THREADS, 0, st>>>((const uint64_t *)d_in, prod, n);
         k_prep_invert<<<1, PREP_THREADS, 0, st>>>(prod, prod + G, G);
         k_prep_finish<<<G, PREP_THREADS, 0, st>>>((const uint64_t *)d_in, prod, (ge_niels_packed *)d_out, n);
@@ -1240,31 +1240,31 @@ int msm_accumulate_chunk(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const g
     cudaStream_t st = ctx->stream;
     int rc;
     // counts | coarse counts | heavy list (count + entries): one memset clears the coarse counts and the heavy count
-    if ((rc = ws_reserve(ctx, ctx->counts, (total_buckets + (size_t)nwin * nc + 1 + max_heavy) * 4))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_COUNTS], (total_buckets + (size_t)nwin * nc + 1 + max_heavy) * 4))) return rc;
     // offsets | scan part sums | coarse bin cursors | extra-slice prefix of the bins | extra slices per window
-    if ((rc = ws_reserve(ctx, ctx->offsets, (total_buckets + (size_t)nwin * parts + 2 * (size_t)nwin * nc + nwin) * 4))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->ntasks, total_buckets * 4))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->task_off, total_buckets * 4 + (nwin + 1) * 4))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->tasks, max_tasks * 8))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->task_sums, max_tasks * sizeof(ge_p3_raw)))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->task_order, (3 * TASK_BINS + max_tasks) * 4))) return rc;   // hist | cursor | start | order
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_OFFSETS], (total_buckets + (size_t)nwin * parts + 2 * (size_t)nwin * nc + nwin) * 4))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_NTASKS], total_buckets * 4))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_TASK_OFF], total_buckets * 4 + (nwin + 1) * 4))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_TASKS], max_tasks * 8))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_TASK_SUMS], max_tasks * sizeof(ge_p3_raw)))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_TASK_ORDER], (3 * TASK_BINS + max_tasks) * 4))) return rc;   // hist | cursor | start | order
     // the sort's records: 8 B per non-zero digit, in (bucket window, coarse bin) order
-    if ((rc = ws_reserve(ctx, ctx->digits, std::max<size_t>(1, n) * nact * 8))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->sorted, std::max<size_t>(1, n) * nact * 4))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->buckets, total_buckets * sizeof(ge_p3_raw)))) return rc;
-    uint32_t *counts = (uint32_t *)ctx->counts.p, *offsets = (uint32_t *)ctx->offsets.p;
-    uint32_t *ntasks = (uint32_t *)ctx->ntasks.p, *task_off = (uint32_t *)ctx->task_off.p;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_DIGITS], std::max<size_t>(1, n) * nact * 8))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_SORTED], std::max<size_t>(1, n) * nact * 4))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_BUCKETS], total_buckets * sizeof(ge_p3_raw)))) return rc;
+    uint32_t *counts = (uint32_t *)ctx->ws[WS_MSM_COUNTS].p, *offsets = (uint32_t *)ctx->ws[WS_MSM_OFFSETS].p;
+    uint32_t *ntasks = (uint32_t *)ctx->ws[WS_MSM_NTASKS].p, *task_off = (uint32_t *)ctx->ws[WS_MSM_TASK_OFF].p;
     uint32_t *win_base = task_off + total_buckets;
     uint32_t *ccount = counts + total_buckets, *heavy = ccount + (size_t)nwin * nc;
     uint32_t *part_sums = offsets + total_buckets, *ccursor = part_sums + (size_t)nwin * parts;
     uint32_t *xpre = ccursor + (size_t)nwin * nc, *xtot = xpre + (size_t)nwin * nc;
-    uint2 *tasks = (uint2 *)ctx->tasks.p;
-    uint32_t *t_hist = (uint32_t *)ctx->task_order.p, *t_cursor = t_hist + TASK_BINS, *t_start = t_cursor + TASK_BINS;
+    uint2 *tasks = (uint2 *)ctx->ws[WS_MSM_TASKS].p;
+    uint32_t *t_hist = (uint32_t *)ctx->ws[WS_MSM_TASK_ORDER].p, *t_cursor = t_hist + TASK_BINS, *t_start = t_cursor + TASK_BINS;
     uint32_t *order = t_start + TASK_BINS;
-    ge_p3_raw *task_sums = (ge_p3_raw *)ctx->task_sums.p;
-    uint2 *records = (uint2 *)ctx->digits.p;
-    uint32_t *sorted = (uint32_t *)ctx->sorted.p;
-    ge_p3_raw *buckets = (ge_p3_raw *)ctx->buckets.p;
+    ge_p3_raw *task_sums = (ge_p3_raw *)ctx->ws[WS_MSM_TASK_SUMS].p;
+    uint2 *records = (uint2 *)ctx->ws[WS_MSM_DIGITS].p;
+    uint32_t *sorted = (uint32_t *)ctx->ws[WS_MSM_SORTED].p;
+    ge_p3_raw *buckets = (ge_p3_raw *)ctx->ws[WS_MSM_BUCKETS].p;
 
     const size_t part_smem = SORT_TILE * 8 + (2 * (size_t)nc + 33) * 4;
     const size_t fine_smem = SORT_FINE_CAP * 12 + ((1u << F) + 33) * 4;
@@ -1334,7 +1334,7 @@ int msm_reduce_finish(dalek_b200_ctx *ctx, int c, ge_p3_raw *d_windows, MsmResul
     const uint32_t nb = 1u << (c - 1);
     cudaStream_t st = ctx->stream;
     int rc;
-    ge_p3_raw *buckets = (ge_p3_raw *)ctx->buckets.p;
+    ge_p3_raw *buckets = (ge_p3_raw *)ctx->ws[WS_MSM_BUCKETS].p;
     LevelInfo li; li.nlevels = 0;
     std::vector<uint32_t> lvl_m, lvl_nout;
     size_t pool_pts = 0;
@@ -1350,9 +1350,9 @@ int msm_reduce_finish(dalek_b200_ctx *ctx, int c, ge_p3_raw *d_windows, MsmResul
             n_in = n_out; first = false;
         }
     }
-    if ((rc = ws_reserve(ctx, ctx->red_a, std::max<size_t>(1, pool_pts) * sizeof(ge_p3_raw)))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->red_b, (size_t)16 * nwin * sizeof(ge_p3_raw)))) return rc;
-    ge_p3_raw *pool = (ge_p3_raw *)ctx->red_a.p, *A = (ge_p3_raw *)ctx->red_b.p;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_REDUCE_POOL], std::max<size_t>(1, pool_pts) * sizeof(ge_p3_raw)))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_REDUCE_SUMS], (size_t)16 * nwin * sizeof(ge_p3_raw)))) return rc;
+    ge_p3_raw *pool = (ge_p3_raw *)ctx->ws[WS_MSM_REDUCE_POOL].p, *A = (ge_p3_raw *)ctx->ws[WS_MSM_REDUCE_SUMS].p;
     const ge_p3_raw *S_in = buckets;
     uint32_t n_in = nb;
     size_t pos = 0;
@@ -1378,16 +1378,16 @@ int msm_reduce_finish(dalek_b200_ctx *ctx, int c, ge_p3_raw *d_windows, MsmResul
                 d2.push_back(make_uint2(first_piece, (uint32_t)d1.size() - first_piece));
             }
         const size_t n1 = d1.size(), n2 = d2.size();
-        if ((rc = ws_reserve(ctx, ctx->sum_desc, (n1 + n2) * sizeof(uint2)))) return rc;
-        if ((rc = ws_reserve(ctx, ctx->sum_part, n1 * sizeof(ge_p3_raw)))) return rc;
-        uint2 *dd1 = (uint2 *)ctx->sum_desc.p, *dd2 = dd1 + n1;
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_SUM_DESC], (n1 + n2) * sizeof(uint2)))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_SUM_PART], n1 * sizeof(ge_p3_raw)))) return rc;
+        uint2 *dd1 = (uint2 *)ctx->ws[WS_MSM_SUM_DESC].p, *dd2 = dd1 + n1;
         if (ctx->sum_desc_c != desc_key) {
             CUDA_TRY(ctx, cudaMemcpyAsync(dd1, d1.data(), n1 * sizeof(uint2), cudaMemcpyHostToDevice, st));
             CUDA_TRY(ctx, cudaMemcpyAsync(dd2, d2.data(), n2 * sizeof(uint2), cudaMemcpyHostToDevice, st));
             CUDA_TRY(ctx, cudaStreamSynchronize(st));       // d1/d2 are host temporaries (rare: once per width)
             ctx->sum_desc_c = desc_key;
         }
-        ge_p3_raw *parts = (ge_p3_raw *)ctx->sum_part.p;
+        ge_p3_raw *parts = (ge_p3_raw *)ctx->ws[WS_MSM_SUM_PART].p;
         k_plain_sum<<<(unsigned)n1, 128, 0, st>>>(pool, dd1, parts);
         k_plain_sum<<<(unsigned)n2, 128, 0, st>>>(parts, dd2, A);
         ctx->launches += 2;

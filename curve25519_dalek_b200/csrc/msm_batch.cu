@@ -264,9 +264,10 @@ static int mb_run(dalek_b200_ctx *ctx, const uint8_t *scalars, const void *point
     mb_carve(slot[0], nullptr, pl.max_terms, pl.max_segs, pl.max_chunks, pin, ct, !on_device);
     const size_t ws_bytes = slot[0].bytes;
     const int nslots = pl.pieces.size() > 1 ? 2 : 1;
+    DevBuf *mb_ws[2] = {&ctx->ws[WS_MSM_BATCH_0], &ctx->ws[WS_MSM_BATCH_1]};   // the pieces on each of the two streams
     for (int k = 0; k < nslots; k++) {
-        if ((rc = ws_reserve(ctx, ctx->mb_ws[k], ws_bytes))) return rc;
-        mb_carve(slot[k], (char *)ctx->mb_ws[k].p, pl.max_terms, pl.max_segs, pl.max_chunks, pin, ct, !on_device);
+        if ((rc = ws_reserve(ctx, *mb_ws[k], ws_bytes))) return rc;
+        mb_carve(slot[k], (char *)mb_ws[k]->p, pl.max_terms, pl.max_segs, pl.max_chunks, pin, ct, !on_device);
     }
     int *status = slot[0].status;
     cudaStream_t ss[2] = {ctx->stream, ctx->stream2};
@@ -311,7 +312,7 @@ static int mb_run(dalek_b200_ctx *ctx, const uint8_t *scalars, const void *point
     CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_pinned, status, 4, cudaMemcpyDeviceToHost, ctx->stream));
     if (ct)                                // zeroize on drop
         for (int k = 0; k < nslots; k++)
-            CUDA_TRY(ctx, cudaMemsetAsync((char *)ctx->mb_ws[k].p + slot[k].secret0, 0, slot[k].bytes - slot[k].secret0, ctx->stream));
+            CUDA_TRY(ctx, cudaMemsetAsync((char *)mb_ws[k]->p + slot[k].secret0, 0, slot[k].bytes - slot[k].secret0, ctx->stream));
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     int bad = *(const int *)ctx->h_pinned;
     float ms = 0.f;

@@ -9,9 +9,9 @@
 
 // Per item: optionally a message of the flat layout (msgs + n + 1 offsets, include/dalek_b200.h; offs = NULL: none),
 // in_sz bytes of `in` (0: none), optionally in2_sz bytes of a second input `in2`, out_sz bytes of `out` and optionally
-// out2_sz bytes of a second output `out2`.  The messages are staged in ctx->misc1 at their own offsets and the offsets in
-// ctx->msg_offs, the fixed-width inputs in ctx->points_in (first all of `in`, then all of `in2`), the outputs in
-// ctx->points.  launch(d_msgs, d_offs, d_in, d_in2, m, d_out, d_out2, stream) enqueues the kernel of one piece of m items
+// out2_sz bytes of a second output `out2`.  The messages are staged in WS_STAGING_MSGS at their own offsets and the offsets in
+// WS_MSG_OFFSETS, the fixed-width inputs in WS_STAGING_IN (first all of `in`, then all of `in2`), the outputs in
+// WS_STAGING_OUT.  launch(d_msgs, d_offs, d_in, d_in2, m, d_out, d_out2, stream) enqueues the kernel of one piece of m items
 // and returns an engine code; d_offs points at the piece's m + 1 offsets, which stay absolute (d_msgs is the base of the
 // whole staged buffer).  A callback that takes one more size_t argument also receives lo, the index of the piece's first
 // item in the batch (for per-item data the kernel reads from elsewhere, such as the signer's expanded keys).  Pieces hold `piece` items (0: 2^16 from 2^17 items up, else one piece).  Sets last_kernel_ms
@@ -23,14 +23,14 @@ static int run_pieces(dalek_b200_ctx *ctx, const uint8_t *msgs, const uint64_t *
 {
     int rc;
     if (offs) {
-        if ((rc = ws_reserve(ctx, ctx->misc1, (n ? (size_t)offs[n] : 0) + 16))) return rc;
-        if ((rc = ws_reserve(ctx, ctx->msg_offs, (n + 1) * 8))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_MSGS], (n ? (size_t)offs[n] : 0) + 16))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_MSG_OFFSETS], (n + 1) * 8))) return rc;
     }
-    if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * (in_sz + in2_sz)))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points, std::max<size_t>(1, n) * (out_sz + out2_sz)))) return rc;
-    uint8_t *d_msgs = (uint8_t *)ctx->misc1.p, *d_in = (uint8_t *)ctx->points_in.p, *d_in2 = d_in + n * in_sz;
-    uint8_t *d_out = (uint8_t *)ctx->points.p, *d_out2 = d_out + n * out_sz;
-    uint64_t *d_offs = (uint64_t *)ctx->msg_offs.p;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_IN], std::max<size_t>(1, n) * (in_sz + in2_sz)))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_OUT], std::max<size_t>(1, n) * (out_sz + out2_sz)))) return rc;
+    uint8_t *d_msgs = (uint8_t *)ctx->ws[WS_STAGING_MSGS].p, *d_in = (uint8_t *)ctx->ws[WS_STAGING_IN].p, *d_in2 = d_in + n * in_sz;
+    uint8_t *d_out = (uint8_t *)ctx->ws[WS_STAGING_OUT].p, *d_out2 = d_out + n * out_sz;
+    uint64_t *d_offs = (uint64_t *)ctx->ws[WS_MSG_OFFSETS].p;
     cudaStream_t ss[2] = {ctx->stream, ctx->stream2};
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, ctx->stream));
     CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->ev_fork, 0));
@@ -68,12 +68,12 @@ static int run_pieces(dalek_b200_ctx *ctx, const uint8_t *msgs, const uint64_t *
     return 0;
 }
 
-// clear the staged inputs (ctx->points_in) and results (ctx->points) of a call that handled secrets (zeroize on drop),
+// clear the staged inputs (WS_STAGING_IN) and results (WS_STAGING_OUT) of a call that handled secrets (zeroize on drop),
 // then wait for the stream
 static inline int wipe_staging(dalek_b200_ctx *ctx, size_t in_bytes, size_t out_bytes)
 {
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->points_in.p, 0, in_bytes, ctx->stream));
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->points.p, 0, out_bytes, ctx->stream));
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->ws[WS_STAGING_IN].p, 0, in_bytes, ctx->stream));
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->ws[WS_STAGING_OUT].p, 0, out_bytes, ctx->stream));
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     return 0;
 }

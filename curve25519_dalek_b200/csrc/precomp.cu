@@ -104,16 +104,16 @@ int dalek_b200_precomp_new(dalek_b200_ctx *ctx, const void *static_points, int p
         return DALEK_E_NOMEM;
     }
     auto fail = [&](int code) { cudaFree(pre->d_points); delete pre; return code; };
-    if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * msm_point_bytes(point_fmt)))) return fail(rc);
-    if ((rc = ws_reserve(ctx, ctx->flags, 64))) return fail(rc);
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_IN], std::max<size_t>(1, n) * msm_point_bytes(point_fmt)))) return fail(rc);
+    if ((rc = msm_driver_ws_reserve(ctx))) return fail(rc);
     if ((rc = pinned_reserve(ctx, 256))) return fail(rc);
     int *h_bad = (int *)ctx->h_pinned;
     *h_bad = 0;
-    if (cudaMemsetAsync(ctx->flags.p, 0, 64, st) != cudaSuccess) return fail(DALEK_E_CUDA);
-    if (n && cudaMemcpyAsync(ctx->points_in.p, static_points, n * msm_point_bytes(point_fmt), cudaMemcpyHostToDevice, st) != cudaSuccess)
+    if (cudaMemsetAsync(ctx->ws[WS_FLAGS].p, 0, FLAG_WORDS * sizeof(int), st) != cudaSuccess) return fail(DALEK_E_CUDA);
+    if (n && cudaMemcpyAsync(ctx->ws[WS_STAGING_IN].p, static_points, n * msm_point_bytes(point_fmt), cudaMemcpyHostToDevice, st) != cudaSuccess)
         return fail(DALEK_E_CUDA);
-    if ((rc = msm_prepare_points(ctx, ctx->points_in.p, point_fmt, n, pre->d_points, (int *)ctx->flags.p))) return fail(rc);
-    if (cudaMemcpyAsync(h_bad, ctx->flags.p, 4, cudaMemcpyDeviceToHost, st) != cudaSuccess) return fail(DALEK_E_CUDA);
+    if ((rc = msm_prepare_points(ctx, ctx->ws[WS_STAGING_IN].p, point_fmt, n, pre->d_points, (int *)ctx->ws[WS_FLAGS].p + FLAG_STATUS))) return fail(rc);
+    if (cudaMemcpyAsync(h_bad, (const int *)ctx->ws[WS_FLAGS].p + FLAG_STATUS, 4, cudaMemcpyDeviceToHost, st) != cudaSuccess) return fail(DALEK_E_CUDA);
     if (cudaStreamSynchronize(st) != cudaSuccess) return fail(DALEK_E_CUDA);
     if (*h_bad) { ctx->last_error = "a static point does not decode"; return fail(DALEK_NONE); }
     pre->d_table = nullptr; pre->c = 0; pre->nwin = 0;
@@ -169,17 +169,14 @@ int dalek_b200_precomp_mixed_msm(dalek_b200_ctx *ctx, const dalek_b200_precomp *
     // window widths: the table fixes the static width; the dynamic part picks its own
     const int c = use_table ? pre->c : msm_choose_window_bits(ctx, n_static + n_dynamic);
     const int c_dyn = use_table ? msm_choose_window_bits(ctx, n_dynamic) : c;
-    const int nwin = std::max(msm_window_count_for_bits(c), msm_window_count_for_bits(c_dyn));
-    if ((rc = ws_reserve(ctx, ctx->scalars, std::max<size_t>(1, n_static + n_dynamic) * 32))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n_dynamic) * din))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points, std::max<size_t>(1, n_dynamic) * sizeof(ge_niels_packed)))) return rc;
-    ge_niels_packed *d_dpts = (ge_niels_packed *)ctx->points.p;
-    if ((rc = ws_reserve(ctx, ctx->flags, 64))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->misc0, (size_t)nwin * sizeof(ge_p3_raw)))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->result, 3 * sizeof(MsmResult) + 64))) return rc;
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->flags.p, 0, 64, st));
-    uint32_t *d_ss = (uint32_t *)ctx->scalars.p, *d_ds = d_ss + 8 * n_static;
-    MsmResult *d_res = (MsmResult *)ctx->result.p, *d_r1 = d_res + 1, *d_r2 = d_res + 2;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_SCALARS], std::max<size_t>(1, n_static + n_dynamic) * 32))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_IN], std::max<size_t>(1, n_dynamic) * din))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_OUT], std::max<size_t>(1, n_dynamic) * sizeof(ge_niels_packed)))) return rc;
+    ge_niels_packed *d_dpts = (ge_niels_packed *)ctx->ws[WS_STAGING_OUT].p;
+    if ((rc = msm_driver_ws_reserve(ctx))) return rc;
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->ws[WS_FLAGS].p, 0, FLAG_WORDS * sizeof(int), st));
+    uint32_t *d_ss = (uint32_t *)ctx->ws[WS_SCALARS].p, *d_ds = d_ss + 8 * n_static;
+    MsmResult *d_res = (MsmResult *)ctx->ws[WS_MSM_RESULT].p, *d_r1 = d_res + 1, *d_r2 = d_res + 2;
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_fork, st));
     CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream_copy, ctx->ev_fork, 0));
     // static scalars in up to 4 chunks, then the dynamic inputs, all on the copy stream
@@ -191,7 +188,7 @@ int dalek_b200_precomp_mixed_msm(dalek_b200_ctx *ctx, const dalek_b200_precomp *
     }
     if (n_dynamic) {
         CUDA_TRY(ctx, cudaMemcpyAsync(d_ds, dynamic_scalars, n_dynamic * 32, cudaMemcpyHostToDevice, ctx->stream_copy));
-        CUDA_TRY(ctx, cudaMemcpyAsync(ctx->points_in.p, dynamic_points, n_dynamic * din, cudaMemcpyHostToDevice, ctx->stream_copy));
+        CUDA_TRY(ctx, cudaMemcpyAsync(ctx->ws[WS_STAGING_IN].p, dynamic_points, n_dynamic * din, cudaMemcpyHostToDevice, ctx->stream_copy));
     }
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_grp[K], ctx->stream_copy));
     for (int k = 0; k < K; k++) {
@@ -206,25 +203,25 @@ int dalek_b200_precomp_mixed_msm(dalek_b200_ctx *ctx, const dalek_b200_precomp *
     }
     CUDA_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_grp[K], 0));
     if (use_table) {
-        if ((rc = msm_reduce_finish(ctx, c, (ge_p3_raw *)ctx->misc0.p, n_dynamic ? d_r1 : d_res, true))) return rc;
+        if ((rc = msm_reduce_finish(ctx, c, (ge_p3_raw *)ctx->ws[WS_MSM_WINDOWS].p, n_dynamic ? d_r1 : d_res, true))) return rc;
         if (n_dynamic) {
-            if ((rc = msm_prepare_points(ctx, ctx->points_in.p, dynamic_fmt, n_dynamic, d_dpts, (int *)ctx->flags.p))) return rc;
+            if ((rc = msm_prepare_points(ctx, ctx->ws[WS_STAGING_IN].p, dynamic_fmt, n_dynamic, d_dpts, (int *)ctx->ws[WS_FLAGS].p + FLAG_STATUS))) return rc;
             if ((rc = msm_accumulate_chunk(ctx, d_ds, d_dpts, n_dynamic, c_dyn, true))) return rc;
-            if ((rc = msm_reduce_finish(ctx, c_dyn, (ge_p3_raw *)ctx->misc0.p, d_r2))) return rc;
+            if ((rc = msm_reduce_finish(ctx, c_dyn, (ge_p3_raw *)ctx->ws[WS_MSM_WINDOWS].p, d_r2))) return rc;
             k_add_results<<<1, 1, 0, st>>>(d_r1, d_r2, d_res);
             ctx->launches++;
         }
     } else {
         if (n_dynamic) {
-            if ((rc = msm_prepare_points(ctx, ctx->points_in.p, dynamic_fmt, n_dynamic, d_dpts, (int *)ctx->flags.p))) return rc;
+            if ((rc = msm_prepare_points(ctx, ctx->ws[WS_STAGING_IN].p, dynamic_fmt, n_dynamic, d_dpts, (int *)ctx->ws[WS_FLAGS].p + FLAG_STATUS))) return rc;
             if ((rc = msm_accumulate_chunk(ctx, d_ds, d_dpts, n_dynamic, c, false))) return rc;
         }
-        if ((rc = msm_reduce_finish(ctx, c, (ge_p3_raw *)ctx->misc0.p, d_res))) return rc;
+        if ((rc = msm_reduce_finish(ctx, c, (ge_p3_raw *)ctx->ws[WS_MSM_WINDOWS].p, d_res))) return rc;
     }
     uint32_t *d_enc = pre->ristretto ? (uint32_t *)(d_res + 3) : nullptr;
     if (d_enc && (rc = ristretto_encode_result(ctx, d_res, d_enc))) return rc;
     // DALEK_NONE: a dynamic point was None (optional_mixed_multiscalar_mul)
-    return msm_read_result(ctx, d_res, (const int *)ctx->flags.p, d_enc, out_compressed, out_limbs);
+    return msm_read_result(ctx, d_res, (const int *)ctx->ws[WS_FLAGS].p + FLAG_STATUS, d_enc, out_compressed, out_limbs);
 }
 
 }  // extern "C"

@@ -126,14 +126,14 @@ int dalek_b200_scalar_from_wide_batch(dalek_b200_ctx *ctx, const uint8_t *in, si
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     int rc;
     cudaStream_t st = ctx->stream;
-    if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * 64))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->scalars, std::max<size_t>(1, n) * 32))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_IN], std::max<size_t>(1, n) * 64))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_SCALARS], std::max<size_t>(1, n) * 32))) return rc;
     if (n) {
-        CUDA_TRY(ctx, cudaMemcpyAsync(ctx->points_in.p, in, n * 64, cudaMemcpyHostToDevice, st));
-        k_scalar_from_wide<<<cdiv(n, 256), 256, 0, st>>>((const uint32_t *)ctx->points_in.p, n, (uint32_t *)ctx->scalars.p);
+        CUDA_TRY(ctx, cudaMemcpyAsync(ctx->ws[WS_STAGING_IN].p, in, n * 64, cudaMemcpyHostToDevice, st));
+        k_scalar_from_wide<<<cdiv(n, 256), 256, 0, st>>>((const uint32_t *)ctx->ws[WS_STAGING_IN].p, n, (uint32_t *)ctx->ws[WS_SCALARS].p);
         ctx->launches++;
         CUDA_TRY(ctx, cudaGetLastError());
-        CUDA_TRY(ctx, cudaMemcpyAsync(out, ctx->scalars.p, n * 32, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(ctx, cudaMemcpyAsync(out, ctx->ws[WS_SCALARS].p, n * 32, cudaMemcpyDeviceToHost, st));
     }
     CUDA_TRY(ctx, cudaStreamSynchronize(st));
     return DALEK_OK;
@@ -146,26 +146,26 @@ int dalek_b200_scalar_invert_batch(dalek_b200_ctx *ctx, const uint8_t *in, size_
     int rc;
     cudaStream_t st = ctx->stream;
     const size_t groups = (n + SC_K - 1) / SC_K;
-    if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * 32))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->scalars, std::max<size_t>(1, n) * 32))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->misc1, std::max<size_t>(1, groups) * 32 + 64))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->flags, 64))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_IN], std::max<size_t>(1, n) * 32))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_SCALARS], std::max<size_t>(1, n) * 32))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_MSGS], std::max<size_t>(1, groups) * 32 + 64))) return rc;
+    if ((rc = msm_driver_ws_reserve(ctx))) return rc;
     if ((rc = pinned_reserve(ctx, 256))) return rc;
-    uint32_t *d_groups = (uint32_t *)ctx->misc1.p, *d_prod = d_groups + 8 * std::max<size_t>(1, groups);
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->flags.p, 0, 64, st));
+    uint32_t *d_groups = (uint32_t *)ctx->ws[WS_STAGING_MSGS].p, *d_prod = d_groups + 8 * std::max<size_t>(1, groups);
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->ws[WS_FLAGS].p, 0, FLAG_WORDS * sizeof(int), st));
     if (n) {
-        CUDA_TRY(ctx, cudaMemcpyAsync(ctx->points_in.p, in, n * 32, cudaMemcpyHostToDevice, st));
-        k_scalar_invert_groups<<<cdiv(groups, 128), 128, 0, st>>>((const uint32_t *)ctx->points_in.p, n, (uint32_t *)ctx->scalars.p, d_groups,
-                                                                  (int *)ctx->flags.p);
+        CUDA_TRY(ctx, cudaMemcpyAsync(ctx->ws[WS_STAGING_IN].p, in, n * 32, cudaMemcpyHostToDevice, st));
+        k_scalar_invert_groups<<<cdiv(groups, 128), 128, 0, st>>>((const uint32_t *)ctx->ws[WS_STAGING_IN].p, n, (uint32_t *)ctx->ws[WS_SCALARS].p, d_groups,
+                                                                  (int *)ctx->ws[WS_FLAGS].p + FLAG_STATUS);
         ctx->launches++;
     }
     k_scalar_product<<<1, 256, 0, st>>>(d_groups, groups, d_prod);      // empty input: the empty product, 1
     ctx->launches++;
     CUDA_TRY(ctx, cudaGetLastError());
     int *h_zero = (int *)((char *)ctx->h_pinned + 64);
-    if (n) CUDA_TRY(ctx, cudaMemcpyAsync(out, ctx->scalars.p, n * 32, cudaMemcpyDeviceToHost, st));
+    if (n) CUDA_TRY(ctx, cudaMemcpyAsync(out, ctx->ws[WS_SCALARS].p, n * 32, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_pinned, d_prod, 32, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(ctx, cudaMemcpyAsync(h_zero, ctx->flags.p, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(h_zero, (const int *)ctx->ws[WS_FLAGS].p + FLAG_STATUS, 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(ctx, cudaStreamSynchronize(st));
     if (*h_zero) { ctx->last_error = "invert_batch: a scalar is zero (scalar.rs:796-799: inputs MUST be nonzero)"; return DALEK_E_INVALID_ARG; }
     memcpy(out_product, ctx->h_pinned, 32);

@@ -141,18 +141,18 @@ static int sign_attrs(dalek_b200_ctx *ctx)
     return 0;
 }
 
-// Expand n_seeds seeds into ctx->misc2 (n_seeds x 64 B, secret) and their verifying keys into ctx->misc3 (n_seeds x 32 B),
-// on the main stream; the seeds are staged in ctx->scalars.
+// Expand n_seeds seeds into WS_VERIFY_HRAM (n_seeds x 64 B, secret) and their verifying keys into WS_VERIFY_H (n_seeds x 32 B),
+// on the main stream; the seeds are staged in WS_SCALARS.
 static int expand_keys(dalek_b200_ctx *ctx, const uint8_t *seeds, size_t n_seeds)
 {
     int rc;
-    if ((rc = ws_reserve(ctx, ctx->scalars, n_seeds * 32))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->misc2, n_seeds * 64))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->misc3, n_seeds * 32))) return rc;
-    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->scalars.p, seeds, n_seeds * 32, cudaMemcpyHostToDevice, ctx->stream));
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_SCALARS], n_seeds * 32))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_VERIFY_HRAM], n_seeds * 64))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_VERIFY_H], n_seeds * 32))) return rc;
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->ws[WS_SCALARS].p, seeds, n_seeds * 32, cudaMemcpyHostToDevice, ctx->stream));
     k_sign_keys<<<cdiv(n_seeds, SIGN_THREADS), SIGN_THREADS, SIGN_SMEM, ctx->stream>>>(
-        (const uint32_t *)ctx->scalars.p, (const double *)ctx->comb_base_table.p, n_seeds, (uint32_t *)ctx->misc2.p,
-        (uint32_t *)ctx->misc3.p);
+        (const uint32_t *)ctx->ws[WS_SCALARS].p, (const double *)ctx->ws[WS_COMB_BASE_TABLE].p, n_seeds, (uint32_t *)ctx->ws[WS_VERIFY_HRAM].p,
+        (uint32_t *)ctx->ws[WS_VERIFY_H].p);
     ctx->launches++;
     CUDA_TRY(ctx, cudaGetLastError());
     return 0;
@@ -176,10 +176,10 @@ static int wipe_secrets(dalek_b200_ctx *ctx, DevBuf *a, size_t a_bytes, DevBuf *
     return rc;
 }
 
-// the staged seeds (ctx->scalars) and the expanded keys (ctx->misc2) of expand_keys
+// the staged seeds (WS_SCALARS) and the expanded keys (WS_VERIFY_HRAM) of expand_keys
 static int wipe_keys(dalek_b200_ctx *ctx, size_t n_seeds, int rc)
 {
-    return wipe_secrets(ctx, &ctx->scalars, n_seeds * 32, &ctx->misc2, n_seeds * 64, rc);
+    return wipe_secrets(ctx, &ctx->ws[WS_SCALARS], n_seeds * 32, &ctx->ws[WS_VERIFY_HRAM], n_seeds * 64, rc);
 }
 
 // Sign n messages (flat layout, or prehashes when ph_dom is set) with n_seeds = n or 1 keys; sigs_out: n x 64 B.
@@ -191,8 +191,8 @@ static int sign_common(dalek_b200_ctx *ctx, const uint8_t *seeds, size_t n_seeds
     if ((rc = comb_base_table_ensure(ctx))) return rc;
     if ((rc = sign_attrs(ctx))) return rc;
     if ((rc = expand_keys(ctx, seeds, n_seeds))) return wipe_keys(ctx, n_seeds, rc);
-    const double *table = (const double *)ctx->comb_base_table.p;
-    const uint32_t *expanded = (const uint32_t *)ctx->misc2.p, *pks = (const uint32_t *)ctx->misc3.p;
+    const double *table = (const double *)ctx->ws[WS_COMB_BASE_TABLE].p;
+    const uint32_t *expanded = (const uint32_t *)ctx->ws[WS_VERIFY_HRAM].p, *pks = (const uint32_t *)ctx->ws[WS_VERIFY_H].p;
     const int one_key = n_seeds == 1;
     Sha512Prefix dom = ph_dom ? *ph_dom : Sha512Prefix{};
     rc = run_pieces(ctx, ph_dom ? nullptr : msgs_flat, ph_dom ? nullptr : msg_offsets, prehashes, ph_dom ? 64 : 0, nullptr, 0,
@@ -221,7 +221,7 @@ int ed25519_b200_verifying_keys(dalek_b200_ctx *ctx, const uint8_t *seeds, size_
     int rc;
     if ((rc = comb_base_table_ensure(ctx))) return rc;
     if ((rc = sign_attrs(ctx))) return rc;
-    const double *table = (const double *)ctx->comb_base_table.p;
+    const double *table = (const double *)ctx->ws[WS_COMB_BASE_TABLE].p;
     rc = run_pieces(ctx, nullptr, nullptr, seeds, 32, nullptr, 0, pubkeys_out, 32, nullptr, 0, n,
                     [&](const uint8_t *, const uint64_t *, const uint8_t *d_s, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *,
                         cudaStream_t st) {
@@ -229,7 +229,7 @@ int ed25519_b200_verifying_keys(dalek_b200_ctx *ctx, const uint8_t *seeds, size_
                                                                                           (uint32_t *)d_o);
                         return 0;
                     });
-    return wipe_secrets(ctx, &ctx->points_in, n * 32, nullptr, 0, rc);                  // the staged seeds
+    return wipe_secrets(ctx, &ctx->ws[WS_STAGING_IN], n * 32, nullptr, 0, rc);                  // the staged seeds
 }
 
 int ed25519_b200_sign_flat(dalek_b200_ctx *ctx, const uint8_t *seeds, size_t n_seeds, const uint8_t *msgs_flat,

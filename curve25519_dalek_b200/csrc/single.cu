@@ -131,7 +131,7 @@ static int verify_each_dev(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const uin
 {
     if (!n) return 0;
     cudaStream_t st = ctx->stream;
-    const ge_niels_packed *base = (const ge_niels_packed *)ctx->base_table.p;
+    const ge_niels_packed *base = (const ge_niels_packed *)ctx->ws[WS_BASE_TABLE].p;
     if (ph_dom) k_verify_each_ph<<<cdiv(n, 128), 128, 0, st>>>(d_msgs, *ph_dom, d_sigs, d_keys, n, strict, base, d_out);
     else k_verify_each<<<cdiv(n, 128), 128, 0, st>>>(d_msgs, d_offs, d_sigs, d_keys, n, strict, base, d_out);
     ctx->launches++;
@@ -348,17 +348,17 @@ static int verify_each_comb(dalek_b200_ctx *ctx, const uint8_t *d_msgs, const ui
     if (tab_bytes > ((size_t)8 << 30)) return 0;
     if (ctx->opt_each_comb == 1 && f.nkeys * 8 > n) return 0;             // a table costs about what eight plain verifications cost
     cudaStream_t st = ctx->stream;
-    if ((rc = ws_reserve(ctx, ctx->each_pow, f.nkeys * 64 * sizeof(ge_p3_raw)))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->each_tab, tab_bytes))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->each_kstat, f.nkeys))) return rc;
-    k_each_key_pow16<<<cdiv(f.nkeys, 64), 64, 0, st>>>(d_keys, f.uniq, f.nkeys, (ge_p3_raw *)ctx->each_pow.p, (uint8_t *)ctx->each_kstat.p);
-    k_each_key_rows<<<cdiv(f.nkeys * 512, 128), 128, 0, st>>>((const ge_p3_raw *)ctx->each_pow.p, f.nkeys, (double *)ctx->each_tab.p);
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_EACH_POW], f.nkeys * 64 * sizeof(ge_p3_raw)))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_EACH_TABLES], tab_bytes))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_EACH_KEY_STATUS], f.nkeys))) return rc;
+    k_each_key_pow16<<<cdiv(f.nkeys, 64), 64, 0, st>>>(d_keys, f.uniq, f.nkeys, (ge_p3_raw *)ctx->ws[WS_EACH_POW].p, (uint8_t *)ctx->ws[WS_EACH_KEY_STATUS].p);
+    k_each_key_rows<<<cdiv(f.nkeys * 512, 128), 128, 0, st>>>((const ge_p3_raw *)ctx->ws[WS_EACH_POW].p, f.nkeys, (double *)ctx->ws[WS_EACH_TABLES].p);
     if (!ctx->each_attr_set) {
         CUDA_TRY(ctx, cudaFuncSetAttribute(k_verify_each_comb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EACH_COMB_SMEM));
         ctx->each_attr_set = true;
     }
-    k_verify_each_comb<<<cdiv((n + EACH_K - 1) / EACH_K, 128), 128, EACH_COMB_SMEM, st>>>(d_sigs, f.hs, f.bad_s, f.rep, f.dense, (const uint8_t *)ctx->each_kstat.p,
-                                                       (const double *)ctx->each_tab.p, (const ge_niels_packed *)ctx->base_table.p, 0, n, strict, d_out);
+    k_verify_each_comb<<<cdiv((n + EACH_K - 1) / EACH_K, 128), 128, EACH_COMB_SMEM, st>>>(d_sigs, f.hs, f.bad_s, f.rep, f.dense, (const uint8_t *)ctx->ws[WS_EACH_KEY_STATUS].p,
+                                                       (const double *)ctx->ws[WS_EACH_TABLES].p, (const ge_niels_packed *)ctx->ws[WS_BASE_TABLE].p, 0, n, strict, d_out);
     ctx->launches += 3;
     CUDA_TRY(ctx, cudaGetLastError());
     *used = true;
@@ -379,8 +379,8 @@ static int verify_each_resident(dalek_b200_ctx *ctx, const uint8_t *d_msgs, cons
                                 const uint32_t *d_keys, size_t n, int strict, const Sha512Prefix *ph_dom, uint8_t *results)
 {
     int rc;
-    if ((rc = ws_reserve(ctx, ctx->misc6, std::max<size_t>(1, n)))) return rc;
-    uint8_t *d_out = (uint8_t *)ctx->misc6.p;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_ITEM_STATUS], std::max<size_t>(1, n)))) return rc;
+    uint8_t *d_out = (uint8_t *)ctx->ws[WS_ITEM_STATUS].p;
     bool comb = false;
     if ((rc = verify_each_comb(ctx, d_msgs, d_offs, d_sigs, d_keys, n, strict, d_out, &comb, ph_dom))) return rc;
     if (!comb && (rc = verify_each_dev(ctx, d_msgs, d_offs, d_sigs, d_keys, n, strict, d_out, ph_dom))) return rc;
@@ -415,11 +415,11 @@ int ed25519_b200_verify_each_flat(dalek_b200_ctx *ctx, const uint8_t *msgs_flat,
         // keys may repeat: everything crosses PCIe first (the key tables need every key), then either the comb path or,
         // when the keys turn out not to repeat, the plain kernel on the resident copies
         const size_t mbytes = (size_t)msg_offsets[n];
-        if ((rc = ws_reserve(ctx, ctx->misc1, mbytes + 16))) return rc;
-        if ((rc = ws_reserve(ctx, ctx->msg_offs, (n + 1) * 8))) return rc;
-        if ((rc = ws_reserve(ctx, ctx->points_in, n * 96))) return rc;
-        uint8_t *d_msgs = (uint8_t *)ctx->misc1.p, *d_sigs = (uint8_t *)ctx->points_in.p, *d_keys = d_sigs + n * 64;
-        uint64_t *d_offs = (uint64_t *)ctx->msg_offs.p;
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_MSGS], mbytes + 16))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_MSG_OFFSETS], (n + 1) * 8))) return rc;
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_IN], n * 96))) return rc;
+        uint8_t *d_msgs = (uint8_t *)ctx->ws[WS_STAGING_MSGS].p, *d_sigs = (uint8_t *)ctx->ws[WS_STAGING_IN].p, *d_keys = d_sigs + n * 64;
+        uint64_t *d_offs = (uint64_t *)ctx->ws[WS_MSG_OFFSETS].p;
         cudaStream_t st = ctx->stream;
         if (mbytes) CUDA_TRY(ctx, cudaMemcpyAsync(d_msgs, msgs_flat, mbytes, cudaMemcpyHostToDevice, st));
         CUDA_TRY(ctx, cudaMemcpyAsync(d_offs, msg_offsets, (n + 1) * 8, cudaMemcpyHostToDevice, st));
@@ -428,7 +428,7 @@ int ed25519_b200_verify_each_flat(dalek_b200_ctx *ctx, const uint8_t *msgs_flat,
         return verify_each_resident(ctx, d_msgs, d_offs, (const uint32_t *)d_sigs, (const uint32_t *)d_keys, n, strict, nullptr, results);
     }
     // independent per signature: pieces alternate between two streams (copy-in -> kernel -> copy-out)
-    const ge_niels_packed *base = (const ge_niels_packed *)ctx->base_table.p;
+    const ge_niels_packed *base = (const ge_niels_packed *)ctx->ws[WS_BASE_TABLE].p;
     rc = run_pieces(ctx, msgs_flat, msg_offsets, sigs, 64, pubkeys, 32, results, 1, nullptr, 0, n,
                     [&](const uint8_t *d_msgs, const uint64_t *d_offs, const uint8_t *d_sigs, const uint8_t *d_keys, size_t m,
                         uint8_t *d_out, uint8_t *, cudaStream_t st) {
@@ -453,9 +453,9 @@ int ed25519_b200_verify_prehashed_each(dalek_b200_ctx *ctx, const uint8_t *preha
     if ((rc = base_table_ensure(ctx))) return rc;
     Sha512Prefix dom;
     ed25519ph_dom2(dom, context, context_len);
-    if ((rc = ws_reserve(ctx, ctx->misc1, n * 64))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points_in, n * 96))) return rc;
-    uint8_t *d_ph = (uint8_t *)ctx->misc1.p, *d_sigs = (uint8_t *)ctx->points_in.p, *d_keys = d_sigs + n * 64;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_MSGS], n * 64))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_IN], n * 96))) return rc;
+    uint8_t *d_ph = (uint8_t *)ctx->ws[WS_STAGING_MSGS].p, *d_sigs = (uint8_t *)ctx->ws[WS_STAGING_IN].p, *d_keys = d_sigs + n * 64;
     cudaStream_t st = ctx->stream;
     CUDA_TRY(ctx, cudaMemcpyAsync(d_ph, prehashes, n * 64, cudaMemcpyHostToDevice, st));
     CUDA_TRY(ctx, cudaMemcpyAsync(d_sigs, sigs, n * 64, cudaMemcpyHostToDevice, st));

@@ -146,9 +146,9 @@ int straus_ct_msm(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const void *d_
 {
     int rc;
     cudaStream_t st = ctx->stream;
-    if ((rc = ws_reserve(ctx, ctx->buckets, std::max<size_t>(1, n) * sizeof(ge_p3_raw)))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->red_a, std::max<size_t>(1, (n + 7) / 8) * sizeof(ge_p3_raw)))) return rc;
-    ge_p3_raw *a = (ge_p3_raw *)ctx->buckets.p, *b = (ge_p3_raw *)ctx->red_a.p;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_BUCKETS], std::max<size_t>(1, n) * sizeof(ge_p3_raw)))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_REDUCE_POOL], std::max<size_t>(1, (n + 7) / 8) * sizeof(ge_p3_raw)))) return rc;
+    ge_p3_raw *a = (ge_p3_raw *)ctx->ws[WS_MSM_BUCKETS].p, *b = (ge_p3_raw *)ctx->ws[WS_MSM_REDUCE_POOL].p;
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, st));                // ev_a .. ev_b: the products (also recorded for n = 0)
     if (n == 0) k_store_identity<<<1, 1, 0, st>>>(a);
     else k_ct_scalar_mul<<<cdiv(n, 64), 64, 0, st>>>(d_scalars, (const ge_pniels_packed *)d_points_pniels, n, a);
@@ -279,11 +279,11 @@ static int double_base_setup(dalek_b200_ctx *ctx, const uint8_t G[32], const uin
     int rc;
     cudaStream_t st = ctx->stream;
     const size_t head = 64 + 2 * 8 * 40 * 4 + 64;
-    if ((rc = ws_reserve(ctx, ctx->misc0, head + COMB_GH_BYTES))) return rc;
-    uint32_t *d_gh = (uint32_t *)ctx->misc0.p;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_CALL_SCRATCH], head + COMB_GH_BYTES))) return rc;
+    uint32_t *d_gh = (uint32_t *)ctx->ws[WS_CALL_SCRATCH].p;
     uint32_t *d_tables = d_gh + 16;
     plan.d_status = (int *)(d_tables + 640);
-    double *d_comb = (double *)((char *)ctx->misc0.p + head);
+    double *d_comb = (double *)((char *)ctx->ws[WS_CALL_SCRATCH].p + head);
     if ((rc = pinned_reserve(ctx, 256))) return rc;
     memcpy(ctx->h_pinned, G, 32); memcpy((char *)ctx->h_pinned + 32, H, 32);
     CUDA_TRY(ctx, cudaMemcpyAsync(d_gh, ctx->h_pinned, 64, cudaMemcpyHostToDevice, st));
@@ -358,27 +358,26 @@ int dalek_b200_edwards_ct_msm(dalek_b200_ctx *ctx, const uint8_t *scalars, const
     for (size_t i = 0; i < n; i++)
         if (scalars[32 * i + 31] & 0x80) { ctx->last_error = "scalar with bit 255 set (Scalar invariant #1)"; return DALEK_E_INVALID_ARG; }
     const size_t pin = msm_point_bytes(point_fmt);
-    if ((rc = ws_reserve(ctx, ctx->scalars, std::max<size_t>(1, n) * 32))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points_in, std::max<size_t>(1, n) * pin))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->points, std::max<size_t>(1, n) * sizeof(ge_pniels_packed)))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->flags, 64))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->result, sizeof(MsmResult)))) return rc;
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->flags.p, 0, 64, st));
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_SCALARS], std::max<size_t>(1, n) * 32))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_IN], std::max<size_t>(1, n) * pin))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_OUT], std::max<size_t>(1, n) * sizeof(ge_pniels_packed)))) return rc;
+    if ((rc = msm_driver_ws_reserve(ctx))) return rc;
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->ws[WS_FLAGS].p, 0, FLAG_WORDS * sizeof(int), st));
     if (n) {
-        CUDA_TRY(ctx, cudaMemcpyAsync(ctx->scalars.p, scalars, n * 32, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(ctx, cudaMemcpyAsync(ctx->points_in.p, points, n * pin, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(ctx, cudaMemcpyAsync(ctx->ws[WS_SCALARS].p, scalars, n * 32, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(ctx, cudaMemcpyAsync(ctx->ws[WS_STAGING_IN].p, points, n * pin, cudaMemcpyHostToDevice, st));
     }
-    const void *d_pn = ctx->points.p;
+    const void *d_pn = ctx->ws[WS_STAGING_OUT].p;
     if (point_fmt == DALEK_POINTS_COMPRESSED) {
         // decompress to Niels (Z = 1), then widen to the projective-Niels layout the kernel reads
-        if ((rc = ws_reserve(ctx, ctx->misc1, std::max<size_t>(1, n) * sizeof(ge_niels_packed)))) return rc;
-        if ((rc = msm_prepare_points(ctx, ctx->points_in.p, point_fmt, n, ctx->misc1.p, (int *)ctx->flags.p))) return rc;
-        launch_niels_to_pniels(ctx, ctx->misc1.p, ctx->points.p, n);
+        if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_MSGS], std::max<size_t>(1, n) * sizeof(ge_niels_packed)))) return rc;
+        if ((rc = msm_prepare_points(ctx, ctx->ws[WS_STAGING_IN].p, point_fmt, n, ctx->ws[WS_STAGING_MSGS].p, (int *)ctx->ws[WS_FLAGS].p + FLAG_STATUS))) return rc;
+        launch_niels_to_pniels(ctx, ctx->ws[WS_STAGING_MSGS].p, ctx->ws[WS_STAGING_OUT].p, n);
     } else {
-        if ((rc = msm_prepare_points(ctx, ctx->points_in.p, point_fmt, n, ctx->points.p, (int *)ctx->flags.p, PK_PNIELS))) return rc;
+        if ((rc = msm_prepare_points(ctx, ctx->ws[WS_STAGING_IN].p, point_fmt, n, ctx->ws[WS_STAGING_OUT].p, (int *)ctx->ws[WS_FLAGS].p + FLAG_STATUS, PK_PNIELS))) return rc;
     }
-    if ((rc = straus_ct_msm(ctx, (const uint32_t *)ctx->scalars.p, d_pn, n, (MsmResult *)ctx->result.p))) return rc;
-    rc = msm_read_result(ctx, (const MsmResult *)ctx->result.p, (const int *)ctx->flags.p, nullptr, out_compressed, out_limbs);
+    if ((rc = straus_ct_msm(ctx, (const uint32_t *)ctx->ws[WS_SCALARS].p, d_pn, n, (MsmResult *)ctx->ws[WS_MSM_RESULT].p))) return rc;
+    rc = msm_read_result(ctx, (const MsmResult *)ctx->ws[WS_MSM_RESULT].p, (const int *)ctx->ws[WS_FLAGS].p + FLAG_STATUS, nullptr, out_compressed, out_limbs);
     if (rc == DALEK_NONE) { ctx->last_error = "a compressed point does not decode (multiscalar_mul takes points, not Options)"; return DALEK_E_INVALID_ARG; }
     return rc;
 }

@@ -75,21 +75,21 @@ int straus_vartime_msm(dalek_b200_ctx *ctx, const uint32_t *d_scalars, const voi
     int rc;
     cudaStream_t st = ctx->stream;
     const size_t n1 = n ? n : 1, nwarps = (n + 7) / 8;
-    if ((rc = ws_reserve(ctx, ctx->digits, n1 * NAF_LEN))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->red_a, n1 * 8 * sizeof(ge_pniels_packed)))) return rc;
-    if ((rc = ws_reserve(ctx, ctx->red_b, (nwarps ? nwarps : 1) * sizeof(ge_p3_raw)))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_DIGITS], n1 * NAF_LEN))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_REDUCE_POOL], n1 * 8 * sizeof(ge_pniels_packed)))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_MSM_REDUCE_SUMS], (nwarps ? nwarps : 1) * sizeof(ge_p3_raw)))) return rc;
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, st));             // ev_a .. ev_b: the Straus kernels (also recorded for n = 0)
     if (n) {
         const unsigned grid = (unsigned)((n + 63) / 64);
         if (point_kind == PK_NIELS)
-            k_straus_prepare<PK_NIELS><<<grid, 64, 0, st>>>(d_scalars, d_points, n, (int8_t *)ctx->digits.p, (ge_pniels_packed *)ctx->red_a.p);
+            k_straus_prepare<PK_NIELS><<<grid, 64, 0, st>>>(d_scalars, d_points, n, (int8_t *)ctx->ws[WS_MSM_DIGITS].p, (ge_pniels_packed *)ctx->ws[WS_MSM_REDUCE_POOL].p);
         else
-            k_straus_prepare<PK_PNIELS><<<grid, 64, 0, st>>>(d_scalars, d_points, n, (int8_t *)ctx->digits.p, (ge_pniels_packed *)ctx->red_a.p);
-        k_straus_vartime<<<(unsigned)nwarps, 32, 0, st>>>((const int8_t *)ctx->digits.p, (const ge_pniels_packed *)ctx->red_a.p, n, (ge_p3_raw *)ctx->red_b.p);
+            k_straus_prepare<PK_PNIELS><<<grid, 64, 0, st>>>(d_scalars, d_points, n, (int8_t *)ctx->ws[WS_MSM_DIGITS].p, (ge_pniels_packed *)ctx->ws[WS_MSM_REDUCE_POOL].p);
+        k_straus_vartime<<<(unsigned)nwarps, 32, 0, st>>>((const int8_t *)ctx->ws[WS_MSM_DIGITS].p, (const ge_pniels_packed *)ctx->ws[WS_MSM_REDUCE_POOL].p, n, (ge_p3_raw *)ctx->ws[WS_MSM_REDUCE_SUMS].p);
         ctx->launches += 2;
     }
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, st));
     ctx->last_kernel_launches = 1;
     CUDA_TRY(ctx, cudaGetLastError());
-    return msm_combine_windows(ctx, (const ge_p3_raw *)ctx->red_b.p, (int)nwarps, 1, 1, d_result);   // nwin = 1: plain sum of the warps' results
+    return msm_combine_windows(ctx, (const ge_p3_raw *)ctx->ws[WS_MSM_REDUCE_SUMS].p, (int)nwarps, 1, 1, d_result);   // nwin = 1: plain sum of the warps' results
 }

@@ -26,7 +26,7 @@ static inline unsigned cdiv(size_t a, unsigned b) { return (unsigned)((a + b - 1
 #define VARMUL_COMB_THREADS 384
 #define VARMUL_COMB_MIN 16384         // shared-point batches from this size use the comb (measured, DESIGN.md §6)
 
-// staging in ctx->misc0: status word, the broadcast scalar, the broadcast point, the comb table
+// staging in WS_CALL_SCRATCH: status word, the broadcast scalar, the broadcast point, the comb table
 #define VM_STATUS 0
 #define VM_SCALAR 64
 #define VM_POINT 128
@@ -183,8 +183,8 @@ static int varmul_setup(dalek_b200_ctx *ctx, size_t n_scalars, int point_fmt, si
 static int varmul_prepare(dalek_b200_ctx *ctx, VarmulPlan &pl, const void *d_point)
 {
     int rc;
-    if ((rc = ws_reserve(ctx, ctx->misc0, VM_TABLE + COMB_BASE_DOUBLES * sizeof(double)))) return rc;
-    char *base = (char *)ctx->misc0.p;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_CALL_SCRATCH], VM_TABLE + COMB_BASE_DOUBLES * sizeof(double)))) return rc;
+    char *base = (char *)ctx->ws[WS_CALL_SCRATCH].p;
     pl.status = (int *)(base + VM_STATUS);
     pl.table = (const double *)(base + VM_TABLE);
     CUDA_TRY(ctx, cudaMemsetAsync(pl.status, 0, 4, ctx->stream));
@@ -234,8 +234,8 @@ int dalek_b200_mul_batch(dalek_b200_ctx *ctx, const uint8_t *scalars, size_t n_s
     CallTimer timer(ctx);
     const size_t pin = msm_point_bytes(point_fmt);
     const bool bs = n_scalars == 1, bp = n_points == 1;
-    if ((rc = ws_reserve(ctx, ctx->misc0, VM_TABLE + COMB_BASE_DOUBLES * sizeof(double)))) return rc;
-    char *base = (char *)ctx->misc0.p;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_CALL_SCRATCH], VM_TABLE + COMB_BASE_DOUBLES * sizeof(double)))) return rc;
+    char *base = (char *)ctx->ws[WS_CALL_SCRATCH].p;
     if (bs) CUDA_TRY(ctx, cudaMemcpyAsync(base + VM_SCALAR, scalars, 32, cudaMemcpyHostToDevice, ctx->stream));
     if (bp) CUDA_TRY(ctx, cudaMemcpyAsync(base + VM_POINT, points, pin, cudaMemcpyHostToDevice, ctx->stream));
     if ((rc = varmul_prepare(ctx, pl, base + VM_POINT))) return rc;
@@ -250,8 +250,8 @@ int dalek_b200_mul_batch(dalek_b200_ctx *ctx, const uint8_t *scalars, size_t n_s
     if (rc) return rc;
     int status = 0;
     if ((rc = varmul_read_status(ctx, pl.status, &status))) return rc;
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->points_in.p, 0, std::max<size_t>(1, n) * (s_sz + p_sz), ctx->stream));   // zeroize on drop
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->points.p, 0, std::max<size_t>(1, n) * (32 + ok_sz), ctx->stream));
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->ws[WS_STAGING_IN].p, 0, std::max<size_t>(1, n) * (s_sz + p_sz), ctx->stream));   // zeroize on drop
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->ws[WS_STAGING_OUT].p, 0, std::max<size_t>(1, n) * (32 + ok_sz), ctx->stream));
     CUDA_TRY(ctx, cudaMemsetAsync(base + VM_SCALAR, 0, 32, ctx->stream));
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     return (status & VM_BAD_POINT) ? DALEK_NONE : DALEK_OK;

@@ -110,12 +110,12 @@ int comb_base_table_ensure(dalek_b200_ctx *ctx)
 {
     if (ctx->comb_base_table_ready) return 0;
     int rc;
-    if ((rc = ws_reserve(ctx, ctx->comb_base_table, X25519_COMB_DOUBLES * sizeof(double)))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_COMB_BASE_TABLE], X25519_COMB_DOUBLES * sizeof(double)))) return rc;
     if ((rc = x25519_base_smem_attr<DALEK_POINTS_MONTGOMERY, 1>(ctx)) || (rc = x25519_base_smem_attr<DALEK_POINTS_MONTGOMERY, 0>(ctx)) ||
         (rc = x25519_base_smem_attr<DALEK_POINTS_COMPRESSED, 1>(ctx)) || (rc = x25519_base_smem_attr<DALEK_POINTS_COMPRESSED, 0>(ctx)) ||
         (rc = x25519_base_smem_attr<DALEK_POINTS_RISTRETTO, 0>(ctx)))
         return rc;
-    k_x25519_base_table<<<4, 128, 0, ctx->stream>>>((double *)ctx->comb_base_table.p);
+    k_x25519_base_table<<<4, 128, 0, ctx->stream>>>((double *)ctx->ws[WS_COMB_BASE_TABLE].p);
     ctx->launches++;
     CUDA_TRY(ctx, cudaGetLastError());
     ctx->comb_base_table_ready = true;
@@ -147,7 +147,7 @@ static int x25519_base_batch(dalek_b200_ctx *ctx, const uint8_t *scalars, size_t
 {
     int rc;
     if ((rc = comb_base_table_ensure(ctx))) return rc;
-    const double *table = (const double *)ctx->comb_base_table.p;
+    const double *table = (const double *)ctx->ws[WS_COMB_BASE_TABLE].p;
     rc = run_pieces(ctx, nullptr, nullptr, scalars, 32, nullptr, 0, out, 32, nullptr, 0, n,
                     [&](const uint8_t *, const uint64_t *, const uint8_t *dk, const uint8_t *, size_t m, uint8_t *d_o, uint8_t *,
                         cudaStream_t st) {
