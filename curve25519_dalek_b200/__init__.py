@@ -29,6 +29,9 @@ touches the CPU checker used by the tests.  Names follow the reference:
   EdwardsPoint.mul_base_batch / mul_base_clamped_batch and RistrettoPoint.mul_base_batch (src/edwards.rs:918-957,
       src/ristretto.rs:939): constant-time s B at every batch size
   ed25519_to_montgomery (ed25519-dalek/src/verifying.rs:476): VerifyingKey::to_montgomery
+  EdwardsPoint / RistrettoPoint .add_batch / sub_batch / neg_batch / double_batch / eq_batch / is_identity_batch / sum /
+      sum_batch and EdwardsPoint.mul_by_cofactor_batch (src/edwards.rs:501-520, :786-876, :1365-1367; src/ristretto.rs:
+      809-908): the group operators, one thread per item, and many segmented sums in one call
 """
 from .engine import (Engine, MultiEngine, EngineError, EdwardsPoint, RistrettoPoint, MontgomeryPoint, SignatureError, verify_batch, default_engine,
                      library_path, load_library, POINTS_COMPRESSED, POINTS_EXTENDED, POINTS_RISTRETTO, POINTS_MONTGOMERY,

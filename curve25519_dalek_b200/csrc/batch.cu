@@ -511,15 +511,6 @@ __global__ void k_batch_status(const uint8_t *__restrict__ bad_s, const uint8_t 
 // sums B_1, B_3 (each scalar residue mod 8 written as a + 3 b, a, b in {-1, 0, 1}), S = B_1 + 3 B_3, a shuffle tree over
 // the group (k_batch_torsion); then the 252 doublings of [l] on one thread per batch (k_batch_torsion_test).  Four mixed
 // additions per signature and one scalar multiplication per BATCH.
-__device__ __forceinline__ void ge64_shfl_down(ge64_p3 &o, const ge64_p3 &p, int d)
-{
-#pragma unroll
-    for (int k = 0; k < 5; k++) {
-        o.X.v[k] = __shfl_down_sync(0xffffffffu, p.X.v[k], d); o.Y.v[k] = __shfl_down_sync(0xffffffffu, p.Y.v[k], d);
-        o.Z.v[k] = __shfl_down_sync(0xffffffffu, p.Z.v[k], d); o.T.v[k] = __shfl_down_sync(0xffffffffu, p.T.v[k], d);
-    }
-}
-
 // the group order l = 2^252 + 27742317777372353535851937790883648493 (scalar.rs constants::BASEPOINT_ORDER), low 128 bits
 __constant__ uint32_t c_l_low[4] = {0x5cf5d3edu, 0x5812631au, 0xa2f79cd6u, 0x14def9deu};
 

@@ -207,6 +207,11 @@ k_ristretto_double_and_compress_batch(const uint64_t *__restrict__ in, size_t n,
     }
 }
 
+void edwards_compress_enqueue(const uint64_t *d_limbs, size_t n, uint32_t *d_out, cudaStream_t st)
+{
+    k_compress_batch<<<cdiv(cdiv(n, CODEC_K), 128), 128, 0, st>>>(d_limbs, n, d_out);
+}
+
 extern "C" {
 
 int dalek_b200_edwards_decompress_batch(dalek_b200_ctx *ctx, const uint8_t *in, size_t n, uint64_t *out_limbs, uint8_t *ok)

@@ -29,11 +29,12 @@ enum WsRole {
     // api.cu, base.cu, batch.cu, precomp.cu, scalars.cu, sign.cu, straus.cu [call] 32-byte scalars (MSM scalars, verify's
     // MSM coefficients, the signer's seeds, the results of the scalar batch calls)
     WS_SCALARS,
-    // pieces.h, api.cu, base.cu, batch.cu, lizard.cu, precomp.cu, scalars.cu, sign.cu, single.cu, straus.cu, varmul.cu
-    // [call] fixed-width inputs staged from the host: MSM input points, signatures and keys, the inputs of run_pieces
+    // pieces.h, api.cu, base.cu, batch.cu, lizard.cu, point_ops.cu, precomp.cu, scalars.cu, sign.cu, single.cu, straus.cu,
+    // varmul.cu [call] fixed-width inputs staged from the host: MSM input points, signatures and keys, the inputs of
+    // run_pieces, the points of a segmented sum
     WS_STAGING_IN,
-    // pieces.h, api.cu, batch.cu, lizard.cu, precomp.cu, straus.cu, varmul.cu [call] outputs of run_pieces and the
-    // prepared Niels points of an MSM (verify's MSM points)
+    // pieces.h, api.cu, batch.cu, lizard.cu, point_ops.cu, precomp.cu, straus.cu, varmul.cu [call] outputs of run_pieces
+    // and the prepared Niels points of an MSM (verify's MSM points)
     WS_STAGING_OUT,
     // pieces.h, base.cu, batch.cu, scalars.cu, single.cu, straus.cu [call] flat messages (or fixed-stride prehashes) at
     // their own offsets; calls that stage no messages keep one-call per-item scratch here: compressed outputs (base.cu),
@@ -41,8 +42,8 @@ enum WsRole {
     WS_STAGING_MSGS,
     // pieces.h, batch.cu, single.cu [call] the n + 1 message offsets of WS_STAGING_MSGS
     WS_MSG_OFFSETS,
-    // double_base.cu, lizard.cu, montgomery.cu, straus.cu, varmul.cu [call] small per-call scratch: status words,
-    // broadcast operands and tables, the G/H tables of the Ristretto double-base batch
+    // double_base.cu, lizard.cu, montgomery.cu, point_ops.cu, straus.cu, varmul.cu [call] small per-call scratch: status
+    // words, broadcast operands and tables, the G/H tables of the Ristretto double-base batch
     WS_CALL_SCRATCH,
     // ---- tables built once per context ----
     // base.cu, double_base.cu, single.cu [context] 64 x 8 affine Niels entries (j+1) 16^i B (base_table_ensure)
@@ -67,6 +68,10 @@ enum WsRole {
     WS_MSM_BATCH_0,
     // msm_batch.cu [call] the workspace of the pieces on the second stream
     WS_MSM_BATCH_1,
+    // ---- group operations (point_ops.cu) ----
+    // point_ops.cu [call] extended results before their shared-inversion encoding; the segmented sum's decoded points,
+    // chunk plans, partial sums and results
+    WS_POINT_OPS,
     // ---- the MSM engine (msm.cu) and the Straus paths that stand in for it ----
     // msm.cu [call] extended-point preparation: the Z product of each group of points (then its inverse), running products
     WS_PREP_PROD,
@@ -351,6 +356,10 @@ int base_table_ensure(dalek_b200_ctx *ctx);
 // context and shared by the X25519 public keys and the Ed25519 signer (sign.cu) ----
 #define COMB_BASE_DOUBLES (64 * 8 * 15)
 int comb_base_table_ensure(dalek_b200_ctx *ctx);
+
+// EdwardsPoint::compress_batch (codecs.cu): n extended points as canonical radix-2^51 limbs (device) -> n x 32 B at d_out,
+// one shared inversion per CODEC_K points, enqueued on st
+void edwards_compress_enqueue(const uint64_t *d_limbs, size_t n, uint32_t *d_out, cudaStream_t st);
 
 // RistrettoPoint::compress of an MSM result (straus.cu): 8 words at d_enc
 int ristretto_encode_result(dalek_b200_ctx *ctx, const MsmResult *d_res, uint32_t *d_enc);

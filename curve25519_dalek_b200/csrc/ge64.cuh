@@ -116,3 +116,15 @@ FE_HD void ge64_to_p3(ge_p3 &o, const ge64_p3 &p)
 {
     fe64_to_fe(o.X, p.X); fe64_to_fe(o.Y, p.Y); fe64_to_fe(o.Z, p.Z); fe64_to_fe(o.T, p.T);
 }
+
+#if defined(__CUDACC__)
+// o = p of the lane d above (every lane of the warp takes part): one step of a warp's shuffle tree
+__device__ __forceinline__ void ge64_shfl_down(ge64_p3 &o, const ge64_p3 &p, int d)
+{
+#pragma unroll
+    for (int k = 0; k < 5; k++) {
+        o.X.v[k] = __shfl_down_sync(0xffffffffu, p.X.v[k], d); o.Y.v[k] = __shfl_down_sync(0xffffffffu, p.Y.v[k], d);
+        o.Z.v[k] = __shfl_down_sync(0xffffffffu, p.Z.v[k], d); o.T.v[k] = __shfl_down_sync(0xffffffffu, p.T.v[k], d);
+    }
+}
+#endif

@@ -117,6 +117,13 @@ def load_library():
     lib.dalek_b200_ristretto_lizard_encode_batch.argtypes = [vp, vp, sz, vp]
     lib.dalek_b200_ristretto_lizard_decode_batch.argtypes = [vp, vp, C.c_int, sz, vp, vp]
     lib.dalek_b200_ristretto_map_to_curve_inverse_batch.argtypes = [vp, vp, C.c_int, sz, vp, vp]
+    for name in ("dalek_b200_point_add_batch", "dalek_b200_point_add_batch_dev"):
+        getattr(lib, name).argtypes = [vp, vp, sz, vp, sz, C.c_int, sz, C.c_int, C.c_int, vp, vp]
+    for name in ("dalek_b200_point_unary_batch", "dalek_b200_point_unary_batch_dev"):
+        getattr(lib, name).argtypes = [vp, C.c_int, vp, C.c_int, sz, C.c_int, C.c_int, vp, vp]
+    lib.dalek_b200_point_eq_batch.argtypes = [vp, vp, sz, vp, sz, C.c_int, sz, C.c_int, vp]
+    for name in ("dalek_b200_point_sum_batch", "dalek_b200_point_sum_batch_dev"):
+        getattr(lib, name).argtypes = [vp, vp, C.c_int, C.c_int, vp, sz, C.c_int, vp, vp]
     _lib = lib
     return lib
 
@@ -473,6 +480,80 @@ class Engine:
         del keep
         return rc, bytes(out)[:32 * m], bytes(ok)[:m], (list(limbs)[:20 * m] if want_limbs else None)
 
+    # ---- group operations ----
+    def _point_results(self, fn, args, n, out_fmt, device_ptrs, out, want_ok):
+        """Run a point call that writes n results in out_fmt (32 B, or 20 u64 for EXTENDED) and n ok bytes."""
+        size = 160 if out_fmt == POINTS_EXTENDED else 32
+        if device_ptrs:
+            ok = None
+            if out is None or want_ok:
+                import torch
+                dev = torch.device("cuda", self.device)
+                if out is None:
+                    out = torch.empty(size * max(n, 1), dtype=torch.uint8, device=dev)
+                if want_ok:
+                    ok = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+            rc = self._check(fn(self.h, *args, _ptr(out), _ptr(ok)))
+            return rc, out, ok
+        res = (C.c_uint8 * (size * max(n, 1)))() if out is None else out
+        ok = (C.c_uint8 * max(n, 1))() if want_ok else None
+        rc = self._check(fn(self.h, *args, _ptr(res), C.addressof(ok) if want_ok else None))
+        return rc, (bytes(res)[:size * n] if out is None else out), (bytes(ok)[:n] if want_ok else None)
+
+    @staticmethod
+    def _point_flags(point_fmt, ristretto, sub=False):
+        return (1 if sub else 0) | (2 if ristretto and point_fmt == POINTS_EXTENDED else 0)
+
+    @staticmethod
+    def _own_encoding(point_fmt, ristretto):
+        return POINTS_RISTRETTO if point_fmt == POINTS_RISTRETTO or ristretto else POINTS_COMPRESSED
+
+    def point_add_batch(self, a, n_a, b, n_b, n, point_fmt=POINTS_COMPRESSED, sub=False, ristretto=False, out_fmt=None,
+                        device_ptrs=False, out=None, want_ok=False):
+        """out[i] = A_i + B_i, or A_i - B_i with sub (dalek_b200_point_add_batch): n_a and n_b are each 1 (broadcast) or n.
+        point_fmt COMPRESSED is Edwards, RISTRETTO Ristretto, EXTENDED Edwards unless `ristretto`.  out_fmt: the group's
+        own encoding (the default) or POINTS_EXTENDED (n x 160 B of canonical limbs).  Returns (rc, out, ok or None) as
+        mul_batch does; rc 1 (DALEK_NONE) when an input does not decode (its ok byte is 0 and its slot the identity)."""
+        of = self._own_encoding(point_fmt, ristretto) if out_fmt is None else out_fmt
+        fn = self.lib.dalek_b200_point_add_batch_dev if device_ptrs else self.lib.dalek_b200_point_add_batch
+        keep = (a, b)
+        r = self._point_results(fn, (_ptr(a), n_a, _ptr(b), n_b, point_fmt, n, self._point_flags(point_fmt, ristretto, sub), of),
+                                n, of, device_ptrs, out, want_ok)
+        del keep
+        return r
+
+    def point_unary_batch(self, op, points, n, point_fmt=POINTS_COMPRESSED, ristretto=False, out_fmt=None, device_ptrs=False,
+                          out=None, want_ok=False):
+        """out[i] = -P_i, 2 P_i or 8 P_i for op "neg", "double" or "mul_by_cofactor" (Edwards only)
+        (dalek_b200_point_unary_batch); formats and results as point_add_batch."""
+        ops = {"neg": 0, "double": 1, "mul_by_cofactor": 2}
+        of = self._own_encoding(point_fmt, ristretto) if out_fmt is None else out_fmt
+        fn = self.lib.dalek_b200_point_unary_batch_dev if device_ptrs else self.lib.dalek_b200_point_unary_batch
+        return self._point_results(fn, (ops[op] if isinstance(op, str) else op, _ptr(points), point_fmt, n,
+                                        self._point_flags(point_fmt, ristretto), of), n, of, device_ptrs, out, want_ok)
+
+    def point_eq_batch(self, a, n_a, b, n_b, n, point_fmt=POINTS_COMPRESSED, ristretto=False):
+        """eq | both_decoded << 1 per item (dalek_b200_point_eq_batch), the group's ct_eq; b = None compares with the identity.
+        Returns (rc, n bytes); rc 1 when an input does not decode."""
+        out = (C.c_uint8 * max(n, 1))()
+        rc = self._check(self.lib.dalek_b200_point_eq_batch(self.h, _ptr(a), n_a, _ptr(b), n_b, point_fmt, n,
+                                                            self._point_flags(point_fmt, ristretto), C.addressof(out)))
+        return rc, bytes(out)[:n]
+
+    def point_sum_batch(self, points, offsets, m, point_fmt=POINTS_COMPRESSED, ristretto=False, out_fmt=None, device_ptrs=False,
+                        out=None, want_ok=False):
+        """Sum of each segment offsets[j] .. offsets[j+1] of the flat points (dalek_b200_point_sum_batch): offsets are m + 1
+        uint64 starting at 0.  Formats and results as point_add_batch (m results); an empty segment gives the identity, one
+        with an undecodable point ok 0 and the identity.  With device_ptrs points, offsets and the results are device
+        buffers."""
+        of = self._own_encoding(point_fmt, ristretto) if out_fmt is None else out_fmt
+        fn = self.lib.dalek_b200_point_sum_batch_dev if device_ptrs else self.lib.dalek_b200_point_sum_batch
+        keep = (points, offsets)
+        r = self._point_results(fn, (_ptr(points), point_fmt, self._point_flags(point_fmt, ristretto), _ptr(offsets), m, of), m, of,
+                                device_ptrs, out, want_ok)
+        del keep
+        return r
+
     def torsion_batch(self, points, n, point_fmt=POINTS_COMPRESSED):
         """is_small_order | is_torsion_free << 1 | decoded << 2 per Edwards point (0 for an undecodable one), as bytes."""
         out = (C.c_uint8 * max(n, 1))()
@@ -728,9 +809,122 @@ def _expect_all(results):
     return results
 
 
-class EdwardsPoint:
+def _point_binary(a, b, fmt, sub, engine):
+    single_a, as_ = _items(a, 32, "points")
+    single_b, bs = _items(b, 32, "points")
+    n = _broadcast_len(single_a, as_, single_b, bs)
+    if n == 0:
+        return []
+    eng = engine or default_engine()
+    rc, raw, _ = eng.point_add_batch(b"".join(as_), len(as_), b"".join(bs), len(bs), n, fmt, sub=sub)
+    if rc == 1:
+        raise ValueError("a point does not decode")
+    outs = [raw[32 * i:32 * i + 32] for i in range(n)]
+    return outs[0] if single_a and single_b else outs
+
+
+def _point_unary(points, op, fmt, engine):
+    single, ps = _items(points, 32, "points")
+    if not ps:
+        return []
+    eng = engine or default_engine()
+    rc, raw, _ = eng.point_unary_batch(op, b"".join(ps), len(ps), fmt)
+    if rc == 1:
+        raise ValueError("a point does not decode")
+    outs = [raw[32 * i:32 * i + 32] for i in range(len(ps))]
+    return outs[0] if single else outs
+
+
+def _point_eq(a, b, fmt, engine):
+    single_a, as_ = _items(a, 32, "points")
+    if b is None:
+        single_b, bs = True, []
+        n = len(as_)
+    else:
+        single_b, bs = _items(b, 32, "points")
+        n = _broadcast_len(single_a, as_, single_b, bs)
+    if n == 0:
+        return []
+    eng = engine or default_engine()
+    rc, flags = eng.point_eq_batch(b"".join(as_), len(as_), b"".join(bs) if b is not None else None, len(bs), n, fmt)
+    if rc == 1:
+        raise ValueError("a point does not decode")
+    outs = [bool(f & 1) for f in flags]
+    return outs[0] if single_a and single_b else outs
+
+
+def _point_sum_batch(point_lists, fmt, engine):
+    import array
+    lists = [_items(list(p), 32, "points")[1] for p in point_lists]
+    m = len(lists)
+    if m == 0:
+        return []
+    offs = array.array("Q", [0])
+    for p in lists:
+        offs.append(offs[-1] + len(p))
+    eng = engine or default_engine()
+    rc, raw, _ = eng.point_sum_batch(b"".join(b"".join(p) for p in lists), offs.tobytes(), m, fmt)
+    if rc == 1:
+        raise ValueError("a point does not decode")
+    return [raw[32 * j:32 * j + 32] for j in range(m)]
+
+
+class _GroupOps:
+    """The group operators (edwards.rs:786-876, ristretto.rs:809-908) on 32-byte encodings of the class's group, one thread
+    per item on the GPU.  One item (bytes) gives one result, a list gives the list; in the binary forms a single item is
+    used for every item of the other operand.  An undecodable encoding raises ValueError."""
+    _FMT = None
+
+    @classmethod
+    def add_batch(cls, a, b, engine=None):
+        """Add: A + B."""
+        return _point_binary(a, b, cls._FMT, False, engine)
+
+    @classmethod
+    def sub_batch(cls, a, b, engine=None):
+        """Sub: A - B."""
+        return _point_binary(a, b, cls._FMT, True, engine)
+
+    @classmethod
+    def neg_batch(cls, points, engine=None):
+        """Neg: -P."""
+        return _point_unary(points, "neg", cls._FMT, engine)
+
+    @classmethod
+    def double_batch(cls, points, engine=None):
+        """Group::double: 2P."""
+        return _point_unary(points, "double", cls._FMT, engine)
+
+    @classmethod
+    def eq_batch(cls, a, b, engine=None):
+        """ConstantTimeEq / PartialEq of the group (not of the bytes): a bool per item."""
+        return _point_eq(a, b, cls._FMT, engine)
+
+    @classmethod
+    def is_identity_batch(cls, points, engine=None):
+        """IsIdentity (traits.rs:33-48): a bool per item."""
+        return _point_eq(points, None, cls._FMT, engine)
+
+    @classmethod
+    def sum(cls, points, engine=None):
+        """Sum<T> (edwards.rs:837-851, ristretto.rs:882-892): the fold of the points from the identity."""
+        return _point_sum_batch([list(points)], cls._FMT, engine)[0]
+
+    @classmethod
+    def sum_batch(cls, point_lists, engine=None):
+        """Sum of each list of points, one call for all lists: the list of results (the identity for an empty list)."""
+        return _point_sum_batch(point_lists, cls._FMT, engine)
+
+
+class EdwardsPoint(_GroupOps):
     """Mirror of the trait impls on curve25519_dalek::edwards::EdwardsPoint.  Points are handled in
     their 32-byte CompressedEdwardsY encoding; results are returned compressed."""
+    _FMT = POINTS_COMPRESSED
+
+    @staticmethod
+    def mul_by_cofactor_batch(points, engine=None):
+        """EdwardsPoint::mul_by_cofactor (edwards.rs:1365-1367): 8P."""
+        return _point_unary(points, "mul_by_cofactor", POINTS_COMPRESSED, engine)
 
     @staticmethod
     def optional_multiscalar_mul(scalars, points, engine=None):
@@ -1209,8 +1403,9 @@ class VartimeRistrettoPrecomputation(_Precomputation):
     _FMT = POINTS_RISTRETTO
 
 
-class RistrettoPoint:
+class RistrettoPoint(_GroupOps):
     """Mirror of the forwarding impls in curve25519-dalek/src/ristretto.rs:964-994 (CompressedRistretto I/O)."""
+    _FMT = POINTS_RISTRETTO
 
     @staticmethod
     def vartime_multiscalar_mul(scalars, points, engine=None):

@@ -379,6 +379,56 @@ int dalek_b200_msm_batch(dalek_b200_ctx *ctx, const uint8_t *scalars /* total x 
 int dalek_b200_msm_batch_dev(dalek_b200_ctx *ctx, const void *d_scalars, const void *d_points, int point_fmt, const void *d_offsets,
                              size_t m, int constant_time, uint8_t *out, uint64_t *out_limbs, uint8_t *ok);
 
+/* -------- group operations on Edwards and Ristretto points --------------------------------------
+ * Add, Sub, Neg, Group::double, mul_by_cofactor, ct_eq / is_identity and Sum (C/edwards.rs:501-520, :786-876, :1365-1367;
+ * C/ristretto.rs:809-908; C/traits.rs:33-48) over batches.
+ *   The input format fixes the group: COMPRESSED is Edwards, RISTRETTO is Ristretto, EXTENDED (20 radix-2^51 limbs, any Z)
+ *     is Edwards unless flags carry DALEK_POINT_RISTRETTO, which makes the limbs a Ristretto representative.  The flag
+ *     with COMPRESSED is DALEK_E_INVALID_ARG.
+ *   out_fmt is the group's own encoding (COMPRESSED for Edwards, RISTRETTO for Ristretto) or EXTENDED: canonical limbs of
+ *     an equal point (a representative of the coset for Ristretto), so that chains stay on the device without decoding
+ *     again.  Any other combination is DALEK_E_INVALID_ARG.
+ *   Broadcast: n_a and n_b are each 1 or n.  n = 0 (m = 0) is a successful no-op.  A NULL buffer with items to process is
+ *     DALEK_E_INVALID_ARG, except ok.  Bad formats, flags, ops and offsets are found before any device work.
+ *   An undecodable input gives ok[i] = 0 and the identity's encoding (or limbs) in its slot, and the call returns
+ *     DALEK_NONE; every other ok[i] is 1.
+ *   Constant time in the points: no branch, loop bound or address depends on a coordinate, a decode outcome or an
+ *     equality; counts, offsets, formats, ops and flags are public.  Host-buffer calls stream the batch in pieces and
+ *     clear the device copies of their inputs, intermediates and results before they return, also after a failed
+ *     launch; the _dev calls clear the engine's intermediates.  No option affects these calls. */
+#define DALEK_POINT_SUB 1                 /* point_add_batch: out = A - B */
+#define DALEK_POINT_RISTRETTO 2           /* EXTENDED points are Ristretto representatives */
+#define DALEK_POINT_NEG 0                 /* point_unary_batch ops */
+#define DALEK_POINT_DOUBLE 1
+#define DALEK_POINT_MUL_BY_COFACTOR 2     /* Edwards only: a Ristretto input is DALEK_E_INVALID_ARG */
+/* out[i] = A_i + B_i, or A_i - B_i with DALEK_POINT_SUB.  out: n x 32 B, or n x 160 B for EXTENDED. */
+int dalek_b200_point_add_batch(dalek_b200_ctx *ctx, const void *a, size_t n_a, const void *b, size_t n_b, int in_fmt, size_t n,
+                               int flags, int out_fmt, void *out, uint8_t *ok /* n bytes, nullable */);
+/* same, every buffer a device pointer; blocks until done */
+int dalek_b200_point_add_batch_dev(dalek_b200_ctx *ctx, const void *d_a, size_t n_a, const void *d_b, size_t n_b, int in_fmt,
+                                   size_t n, int flags, int out_fmt, void *d_out, void *d_ok);
+/* out[i] = -P_i, 2 P_i or 8 P_i (op DALEK_POINT_NEG, _DOUBLE, _MUL_BY_COFACTOR); any other op is DALEK_E_INVALID_ARG */
+int dalek_b200_point_unary_batch(dalek_b200_ctx *ctx, int op, const void *points, int in_fmt, size_t n, int flags, int out_fmt,
+                                 void *out, uint8_t *ok);
+int dalek_b200_point_unary_batch_dev(dalek_b200_ctx *ctx, int op, const void *d_points, int in_fmt, size_t n, int flags,
+                                     int out_fmt, void *d_out, void *d_ok);
+/* out[i] = eq | both_decoded << 1, eq the group's ct_eq (Edwards: X1 Z2 = X2 Z1 and Y1 Z2 = Y2 Z1; Ristretto:
+ * X1 Y2 = Y1 X2 or X1 X2 = Y1 Y2), 0 when an input does not decode (the call then returns DALEK_NONE).  b = NULL compares
+ * with the identity (is_identity; n_b is ignored).  Points are compared as group elements, not as bytes: a non-canonical
+ * CompressedEdwardsY equals its canonical form, and two representatives of one Ristretto coset are equal as Ristretto
+ * points and unequal as Edwards points.  Host buffers. */
+int dalek_b200_point_eq_batch(dalek_b200_ctx *ctx, const void *a, size_t n_a, const void *b, size_t n_b, int in_fmt, size_t n,
+                              int flags, uint8_t *out /* n bytes */);
+/* Sum (fold from the identity) of each segment: result j is the sum of the points offsets[j] .. offsets[j+1] (m + 1 u64
+ * offsets, offsets[0] = 0, non-decreasing, offsets[m] < 2^31, else DALEK_E_INVALID_ARG before any device work).  An empty
+ * segment gives the identity; a segment with an undecodable point gives ok[j] = 0 and the identity.  out: m x 32 B, or
+ * m x 160 B for EXTENDED. */
+int dalek_b200_point_sum_batch(dalek_b200_ctx *ctx, const void *points, int in_fmt, int flags, const uint64_t *offsets, size_t m,
+                               int out_fmt, void *out, uint8_t *ok /* m bytes, nullable */);
+/* same, every buffer a device pointer; the offsets are read back once (8 bytes per segment) to plan the chunks */
+int dalek_b200_point_sum_batch_dev(dalek_b200_ctx *ctx, const void *d_points, int in_fmt, int flags, const void *d_offsets, size_t m,
+                                   int out_fmt, void *d_out, void *d_ok);
+
 /* -------- hash to group ------------------------------------------------------------------------
  * Host buffers; each call blocks and streams the batch in pieces like the codecs.  The maps are total: these calls never
  * return DALEK_NONE.  n = 0 is a successful no-op; with n > 0 a NULL buffer other than msgs_flat is DALEK_E_INVALID_ARG.
