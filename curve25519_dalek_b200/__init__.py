@@ -32,14 +32,18 @@ touches the CPU checker used by the tests.  Names follow the reference:
   EdwardsPoint / RistrettoPoint .add_batch / sub_batch / neg_batch / double_batch / eq_batch / is_identity_batch / sum /
       sum_batch and EdwardsPoint.mul_by_cofactor_batch (src/edwards.rs:501-520, :786-876, :1365-1367; src/ristretto.rs:
       809-908): the group operators, one thread per item, and many segmented sums in one call
+  Scalar.from_bytes_mod_order_batch / from_bytes_mod_order_wide_batch / from_canonical_bytes_batch / hash_from_bytes_batch
+      / add_batch / sub_batch / mul_batch / neg_batch / div_by_2_batch / invert_each / invert_batch_alloc / sum / sum_batch
+      / product / product_batch (src/scalar.rs:235-263, :317-374, :454-476, :617-670, :739-870): arithmetic mod l on
+      canonical scalars, one thread per item, and many segmented sums and products in one call
 """
-from .engine import (Engine, MultiEngine, EngineError, EdwardsPoint, RistrettoPoint, MontgomeryPoint, SignatureError, verify_batch, default_engine,
+from .engine import (Engine, MultiEngine, EngineError, EdwardsPoint, RistrettoPoint, MontgomeryPoint, Scalar, SignatureError, verify_batch, default_engine,
                      library_path, load_library, POINTS_COMPRESSED, POINTS_EXTENDED, POINTS_RISTRETTO, POINTS_MONTGOMERY,
                      VartimeEdwardsPrecomputation, VartimeRistrettoPrecomputation, x25519, x25519_public_keys,
                      X25519_BASEPOINT_BYTES, ed25519_verifying_keys, ed25519_sign, ed25519_sign_prehashed,
                      ed25519_verify_prehashed, ed25519_to_montgomery)
 
-__all__ = ["Engine", "MultiEngine", "EngineError", "EdwardsPoint", "RistrettoPoint", "MontgomeryPoint", "SignatureError", "verify_batch", "default_engine",
+__all__ = ["Engine", "MultiEngine", "EngineError", "EdwardsPoint", "RistrettoPoint", "MontgomeryPoint", "Scalar", "SignatureError", "verify_batch", "default_engine",
            "library_path", "load_library", "POINTS_COMPRESSED", "POINTS_EXTENDED", "POINTS_RISTRETTO", "POINTS_MONTGOMERY",
            "VartimeEdwardsPrecomputation", "VartimeRistrettoPrecomputation", "x25519", "x25519_public_keys",
            "X25519_BASEPOINT_BYTES", "ed25519_verifying_keys", "ed25519_sign", "ed25519_sign_prehashed",

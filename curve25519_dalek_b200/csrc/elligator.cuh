@@ -4,6 +4,7 @@
 //   ristretto_elligator       RistrettoPoint::elligator_ristretto_flavor      C/ristretto/elligator.rs:15-51
 //   ristretto_from_uniform    RistrettoPoint::from_uniform_bytes              C/ristretto.rs:774-790
 //   ristretto_hash_from_bytes RistrettoPoint::hash_from_bytes::<Sha512>       C/ristretto.rs:736-761
+//   h2c_sha512_digest         its SHA-512 step, shared with Scalar::hash_from_bytes (scalars.cu)
 //   ell2_encode               montgomery::elligator_encode (RFC 9380 G.2.1)   C/montgomery.rs:276-363
 //   ell2_map_to_curve         EdwardsPoint::map_to_curve (rational map)       C/edwards.rs:651-686
 //   h2c_from_bytes_wide       FieldElement::from_bytes_wide                   C/field.rs:110-147
@@ -200,14 +201,21 @@ H2C_FN void ristretto_from_uniform(ge_p3 &P, const uint32_t w[16])
     ge_add(P, R1, R2);
 }
 
-// RistrettoPoint::hash_from_bytes::<Sha512> (C/ristretto.rs:736-761) -> CompressedRistretto as eight words
-H2C_FN void ristretto_hash_from_bytes(uint32_t out[8], const uint8_t *msg, size_t mlen)
+// SHA-512 of a message as 16 little-endian words: the 64 bytes that RistrettoPoint::hash_from_bytes (C/ristretto.rs:
+// 736-761) and Scalar::hash_from_bytes (C/scalar.rs:617-624) feed to from_uniform_bytes and from_bytes_mod_order_wide
+H2C_FN void h2c_sha512_digest(uint32_t w[16], const uint8_t *msg, size_t mlen)
 {
     uint64_t h[8];
     h2c_sha512_iv(h);
     h2c_sha512<false>(h, 0, mlen, nullptr, [&](size_t q) -> uint32_t { return msg[q]; });
-    uint32_t w[16];
     h2c_digest_words(w, h);
+}
+
+// RistrettoPoint::hash_from_bytes::<Sha512> (C/ristretto.rs:736-761) -> CompressedRistretto as eight words
+H2C_FN void ristretto_hash_from_bytes(uint32_t out[8], const uint8_t *msg, size_t mlen)
+{
+    uint32_t w[16];
+    h2c_sha512_digest(w, msg, mlen);
     ge_p3 P;
     ristretto_from_uniform(P, w);
     ristretto_compress<1>(out, P);

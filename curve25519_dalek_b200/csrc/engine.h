@@ -33,8 +33,8 @@ enum WsRole {
     // varmul.cu [call] fixed-width inputs staged from the host: MSM input points, signatures and keys, the inputs of
     // run_pieces, the points of a segmented sum
     WS_STAGING_IN,
-    // pieces.h, api.cu, batch.cu, lizard.cu, point_ops.cu, precomp.cu, straus.cu, varmul.cu [call] outputs of run_pieces
-    // and the prepared Niels points of an MSM (verify's MSM points)
+    // pieces.h, api.cu, batch.cu, lizard.cu, point_ops.cu, precomp.cu, scalars.cu, straus.cu, varmul.cu [call] outputs of
+    // run_pieces and the prepared Niels points of an MSM (verify's MSM points)
     WS_STAGING_OUT,
     // pieces.h, base.cu, batch.cu, scalars.cu, single.cu, straus.cu [call] flat messages (or fixed-stride prehashes) at
     // their own offsets; calls that stage no messages keep one-call per-item scratch here: compressed outputs (base.cu),
@@ -42,8 +42,8 @@ enum WsRole {
     WS_STAGING_MSGS,
     // pieces.h, batch.cu, single.cu [call] the n + 1 message offsets of WS_STAGING_MSGS
     WS_MSG_OFFSETS,
-    // double_base.cu, lizard.cu, montgomery.cu, point_ops.cu, straus.cu, varmul.cu [call] small per-call scratch: status
-    // words, broadcast operands and tables, the G/H tables of the Ristretto double-base batch
+    // double_base.cu, lizard.cu, montgomery.cu, point_ops.cu, scalars.cu, straus.cu, varmul.cu [call] small per-call
+    // scratch: status words, broadcast operands and tables, the G/H tables of the Ristretto double-base batch
     WS_CALL_SCRATCH,
     // ---- tables built once per context ----
     // base.cu, double_base.cu, single.cu [context] 64 x 8 affine Niels entries (j+1) 16^i B (base_table_ensure)
@@ -72,6 +72,9 @@ enum WsRole {
     // point_ops.cu [call] extended results before their shared-inversion encoding; the segmented sum's decoded points,
     // chunk plans, partial sums and results
     WS_POINT_OPS,
+    // ---- scalar arithmetic (scalars.cu) ----
+    // scalars.cu [call] the scalar Sum / Product: chunk plans, partial sums or products, results
+    WS_SCALAR_FOLD,
     // ---- the MSM engine (msm.cu) and the Straus paths that stand in for it ----
     // msm.cu [call] extended-point preparation: the Z product of each group of points (then its inverse), running products
     WS_PREP_PROD,
@@ -275,6 +278,17 @@ inline bool flat_messages_ok(const uint8_t *msgs_flat, const uint64_t *offsets, 
 }
 
 int ws_reserve(dalek_b200_ctx *ctx, DevBuf &b, size_t bytes);
+
+#if defined(__CUDACC__)
+// *bad |= some thread of the warp had a bad input (good = 0): one warp-wide OR and one atomic per warp, whatever the
+// inputs (point_ops.cu, scalars.cu)
+__device__ __forceinline__ void warp_report_bad(uint32_t good, int *bad)
+{
+    const unsigned act = __activemask();
+    const uint32_t any_bad = __reduce_or_sync(act, 1u - good);
+    if ((threadIdx.x & 31) == (unsigned)(__ffs(act) - 1)) atomicOr(bad, (int)any_bad);
+}
+#endif
 // WS_FLAGS, WS_MSM_WINDOWS and WS_MSM_RESULT at their bounds (api.cu): every call that uses them reserves them here
 int msm_driver_ws_reserve(dalek_b200_ctx *ctx);
 int pinned_reserve(dalek_b200_ctx *ctx, size_t bytes);

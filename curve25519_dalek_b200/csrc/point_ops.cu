@@ -40,14 +40,6 @@ static inline unsigned cdiv(size_t a, unsigned b) { return (unsigned)((a + b - 1
 #define PO_BCAST_B 512
 #define PO_SCRATCH 1024
 
-// *bad |= some thread of the warp did not decode its input: one atomic per warp, whatever the points
-__device__ __forceinline__ void po_report(uint32_t good, int *bad)
-{
-    const unsigned act = __activemask();
-    const uint32_t any_bad = __reduce_or_sync(act, 1u - good);
-    if ((threadIdx.x & 31) == (unsigned)(__ffs(act) - 1)) atomicOr(bad, (int)any_bad);
-}
-
 __device__ __forceinline__ void ps_store(double *__restrict__ o, const ge64_p3 &P)
 {
 #pragma unroll
@@ -87,7 +79,7 @@ k_point_op(const uint32_t *__restrict__ a, size_t a_step, const uint32_t *__rest
         for (int k = 0; k < 20; k++) limbs[20 * i + k] = l[k];
     }
     if (ok) ok[i] = (uint8_t)good;
-    po_report(good, bad);
+    warp_report_bad(good, bad);
 }
 
 // out[i] = eq | both_decoded << 1; b = NULL compares with the identity
@@ -104,7 +96,7 @@ k_point_eq(const uint32_t *__restrict__ a, size_t a_step, const uint32_t *__rest
     if (b) good &= varmul_load_point<FMT>(B, b, b_step * i);          // public: the call compares with the identity
     const uint32_t e = rist ? ristretto_eq(A, B) : edwards_eq(A, B);   // the group is public
     out[i] = (uint8_t)((e & good) | (good << 1));
-    po_report(good, bad);
+    warp_report_bad(good, bad);
 }
 
 // point i of the piece -> 20 doubles (FP64 limbs at scale 1) and its decode flag; an undecodable point is the identity
@@ -202,7 +194,7 @@ k_sum_finish(const double *__restrict__ partial, const uint8_t *__restrict__ par
         for (int k = 0; k < 20; k++) limbs[20 * j + k] = l[k];
     }
     ok[j] = (uint8_t)good;
-    po_report(good, bad);
+    warp_report_bad(good, bad);
 }
 
 // ---- argument rules ----
@@ -416,14 +408,6 @@ static void ps_carve(PsSlot &s, char *p, const std::vector<PsLevel> &lv, size_t 
     s.enc = (uint32_t *)take(m * 32);
     s.ok = (uint8_t *)take(m);
     s.bytes = at;
-}
-
-static bool ps_offsets_ok(const uint64_t *offsets, size_t m)
-{
-    if (offsets[0] != 0) return false;
-    for (size_t j = 0; j < m; j++)
-        if (offsets[j] > offsets[j + 1]) return false;
-    return offsets[m] < (1ull << 31);
 }
 
 // threads of a chunk's CTA: enough warps for the longest chunk, at most PS_THREADS

@@ -1,5 +1,5 @@
-// point_ops.cuh -- per-item group arithmetic of the batched point operations (point_ops.cu), host-compilable, and the
-// host plan of the segmented sum.
+// point_ops.cuh -- per-item group arithmetic of the batched point operations (point_ops.cu), host-compilable; the host
+// plan of the segmented sum is in ps_plan.h.
 //   Add / Sub          C/edwards.rs:795-835, C/ristretto.rs:838-880        point_apply (PO_ADD, PO_SUB)
 //   Neg                C/edwards.rs:853-876, C/ristretto.rs:894-908        point_apply (PO_NEG)
 //   Group::double      C/edwards.rs:786-788 (and the Ristretto impl)       point_apply (PO_DOUBLE)
@@ -13,10 +13,8 @@
 #pragma once
 #include <stdint.h>
 
-#include <algorithm>
-#include <vector>
-
 #include "ge64.cuh"
+#include "ps_plan.h"
 
 enum { PO_ADD = 0, PO_SUB = 1, PO_NEG = 2, PO_DOUBLE = 3, PO_COFACTOR = 4 };
 
@@ -84,46 +82,4 @@ FE_HD void ge64_cmov_identity(ge64_p3 &p, uint32_t c)
 FE_HD void point_to_limbs(uint64_t l[20], const ge_p3 &p)
 {
     fe_to_limbs51(l, p.X); fe_to_limbs51(l + 5, p.Y); fe_to_limbs51(l + 10, p.Z); fe_to_limbs51(l + 15, p.T);
-}
-
-// ---- the plan of the segmented sum (host) ----
-// A level cuts segments (m + 1 offsets) into chunks of at most `chunk` consecutive items that never cross a segment
-// boundary.  The chunks tile the items in order, so chunk c covers items [start[c], start[c+1]); segment j owns
-// chunks [base[j], base[j+1]) (none when it is empty).  The next level's segments are the chunks' partial sums:
-// its offsets are this level's base.
-struct PsLevel {
-    std::vector<uint32_t> start;    // nchunks + 1
-    std::vector<uint32_t> base;     // m + 1
-    uint32_t max_len = 0;           // the longest chunk
-    uint32_t max_per_seg = 0;       // the most chunks of one segment
-};
-
-template <typename Off>
-static inline void ps_plan_level(PsLevel &L, const Off *offsets, size_t m, uint32_t chunk)
-{
-    L.start.clear(); L.base.clear(); L.max_len = 0; L.max_per_seg = 0;
-    L.base.reserve(m + 1);
-    for (size_t j = 0; j < m; j++) {
-        L.base.push_back((uint32_t)L.start.size());
-        const uint64_t lo = (uint64_t)offsets[j], hi = (uint64_t)offsets[j + 1];
-        uint32_t k = 0;
-        for (uint64_t c = lo; c < hi; c += chunk, k++) {
-            L.start.push_back((uint32_t)c);
-            L.max_len = std::max(L.max_len, (uint32_t)std::min<uint64_t>(chunk, hi - c));
-        }
-        L.max_per_seg = std::max(L.max_per_seg, k);
-    }
-    L.base.push_back((uint32_t)L.start.size());
-    L.start.push_back(m ? (uint32_t)offsets[m] : 0u);
-}
-
-// Pieces of whole chunks of a level with at most `piece` items each (piece >= chunk): cuts[k] .. cuts[k+1] are the
-// chunks of piece k.
-static inline void ps_pieces(std::vector<uint32_t> &cuts, const std::vector<uint32_t> &start, uint32_t piece)
-{
-    cuts.assign(1, 0);
-    const uint32_t nchunks = (uint32_t)start.size() - 1;
-    for (uint32_t c = 0; c < nchunks; c++)
-        if (start[c + 1] - start[cuts.back()] > piece) cuts.push_back(c);
-    if (cuts.back() != nchunks) cuts.push_back(nchunks);
 }

@@ -1,9 +1,11 @@
 // sc.cuh -- arithmetic modulo the group order l = 2^252 + 27742317777372353535851937790883648493
 // on 32-bit words.  Values cross this header as 8 little-endian 32-bit words.  Device code under nvcc; a plain C++
-// compiler builds it for the host (tests/host/sc_host_check.cpp), with SC_L / SC_MU as host constants.
+// compiler builds it for the host (tests/host/sc_host_check.cpp, tests/host/scalar_ops_host_check.cpp), with SC_L /
+// SC_MU as host constants.
 //
-// Branch-free in the values: every conditional subtraction of l is a masked select, so that the signer (sign.cu) can
-// reduce secrets (r, k a + r) here.  Loop counts are fixed.
+// Branch-free in the values: every conditional subtraction or addition of l is a masked select, so that the signer
+// (sign.cu) can reduce secrets (r, k a + r) here and the scalar batch calls (scalars.cu) can compute on them.  Loop counts
+// and the inversion's exponent are fixed.
 //
 // The reference uses five 52-bit limbs with Montgomery reduction, R = 2^260
 // (curve25519-dalek/src/backend/serial/u64/scalar.rs:60-343).  Only canonical values are
@@ -132,4 +134,45 @@ SC_HD void sc_neg(uint32_t *r, const uint32_t *a)
     const uint32_t m = 0u - ((nz | (0u - nz)) >> 31);   // all ones iff a != 0
 #pragma unroll
     for (int i = 0; i < 8; i++) r[i] = u[i] & m;
+}
+
+// r = a - b mod l, inputs < l (C/scalar.rs:353-362): l is added back under a mask when the difference borrows
+SC_HD void sc_sub(uint32_t *r, const uint32_t *a, const uint32_t *b)
+{
+    uint32_t d[8];
+    const uint32_t m = 0u - mp_sub<8>(d, a, b);      // all ones: a < b
+    uint64_t carry = 0;
+#pragma unroll
+    for (int i = 0; i < 8; i++) { uint64_t t = (uint64_t)d[i] + (SC_L[i] & m) + carry; r[i] = (uint32_t)t; carry = t >> 32; }
+}
+
+// r = a / 2 mod l for a < l (Scalar::div_by_2, C/scalar.rs:858-870): l is added under a mask when a is odd, then the
+// even sum (< 2^254, no carry out of 256 bits) is shifted right by one bit across the words
+SC_HD void sc_div_by_2(uint32_t *r, const uint32_t *a)
+{
+    const uint32_t m = 0u - (a[0] & 1u);
+    uint32_t t[8];
+    uint64_t carry = 0;
+#pragma unroll
+    for (int i = 0; i < 8; i++) { uint64_t s = (uint64_t)a[i] + (SC_L[i] & m) + carry; t[i] = (uint32_t)s; carry = s >> 32; }
+#pragma unroll
+    for (int i = 0; i < 7; i++) r[i] = (t[i] >> 1) | (t[i + 1] << 31);
+    r[7] = t[7] >> 1;
+}
+
+// a^(l-2) mod l by left-to-right square-and-multiply over the bits of l - 2 (uniform control flow: the exponent is public);
+// Scalar::invert's value (C/scalar.rs:739-741), 0 for a = 0
+SC_HD void sc_invert(uint32_t r[8], const uint32_t a[8])
+{
+    uint32_t e[8], acc[8];
+#pragma unroll
+    for (int i = 0; i < 8; i++) { e[i] = SC_L[i]; acc[i] = i == 0 ? 1u : 0u; }
+    e[0] -= 2;                                            // l is odd and l[0] >= 2: no borrow
+#pragma unroll 1
+    for (int bit = 252; bit >= 0; bit--) {
+        sc_mul(acc, acc, acc);
+        if ((e[bit >> 5] >> (bit & 31)) & 1) sc_mul(acc, acc, a);
+    }
+#pragma unroll
+    for (int i = 0; i < 8; i++) r[i] = acc[i];
 }

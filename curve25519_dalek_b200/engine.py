@@ -86,6 +86,14 @@ def load_library():
     lib.ed25519_b200_verify_each_flat_dev.argtypes = [vp, vp, vp, vp, vp, sz, C.c_int, vp]
     lib.dalek_b200_scalar_from_wide_batch.argtypes = [vp, vp, sz, vp]
     lib.dalek_b200_scalar_invert_batch.argtypes = [vp, vp, sz, vp, vp]
+    for name in ("dalek_b200_scalar_binary_batch", "dalek_b200_scalar_binary_batch_dev"):
+        getattr(lib, name).argtypes = [vp, C.c_int, vp, sz, vp, sz, sz, vp]
+    for name in ("dalek_b200_scalar_unary_batch", "dalek_b200_scalar_unary_batch_dev"):
+        getattr(lib, name).argtypes = [vp, C.c_int, vp, sz, vp]
+    lib.dalek_b200_scalar_from_bytes_batch.argtypes = [vp, vp, sz, C.c_int, vp, vp]
+    lib.dalek_b200_scalar_hash_from_bytes_batch.argtypes = [vp, vp, vp, sz, vp]
+    for name in ("dalek_b200_scalar_fold_batch", "dalek_b200_scalar_fold_batch_dev"):
+        getattr(lib, name).argtypes = [vp, C.c_int, vp, vp, sz, vp]
     lib.ed25519_b200_last_zs.argtypes = [vp, vp, sz]
     lib.dalek_b200_edwards_mul_base_batch.argtypes = [vp, vp, sz, vp, vp]
     lib.ed25519_b200_sign_batch_flat.argtypes = [vp, vp, vp, vp, sz, vp, vp]
@@ -309,6 +317,65 @@ class Engine:
         prod = (C.c_uint8 * 32)()
         self._check(self.lib.dalek_b200_scalar_invert_batch(self.h, _ptr(scalars), n, C.addressof(out), C.addressof(prod)))
         return bytes(out)[:32 * n], bytes(prod)
+
+    # ---- scalar arithmetic: canonical 32-byte scalars in and out; a non-canonical input raises EngineError ----
+    SCALAR_BINARY_OPS = {"add": 0, "sub": 1, "mul": 2}
+    SCALAR_UNARY_OPS = {"neg": 0, "invert": 1, "div_by_2": 2}
+    SCALAR_FOLD_OPS = {"sum": 0, "product": 1}
+
+    def _scalar_results(self, fn, args, n, device_ptrs, out):
+        """Run a scalar call that writes n x 32 B: into `out` if given, else a new buffer (a CUDA tensor with device_ptrs,
+        bytes otherwise)."""
+        if device_ptrs:
+            if out is None:
+                import torch
+                out = torch.empty(32 * max(n, 1), dtype=torch.uint8, device=torch.device("cuda", self.device))
+            self._check(fn(self.h, *args, _ptr(out)))
+            return out
+        res = (C.c_uint8 * (32 * max(n, 1)))() if out is None else out
+        self._check(fn(self.h, *args, _ptr(res)))
+        return bytes(res)[:32 * n] if out is None else out
+
+    def scalar_binary_batch(self, op, a, n_a, b, n_b, n, device_ptrs=False, out=None):
+        """out[i] = A_i + B_i, A_i - B_i or A_i * B_i for op "add", "sub" or "mul" (dalek_b200_scalar_binary_batch): n_a and
+        n_b are each 1 (broadcast) or n.  With device_ptrs every buffer is a device pointer or CUDA tensor, and `out` may be
+        a non-broadcast input (in place)."""
+        fn = self.lib.dalek_b200_scalar_binary_batch_dev if device_ptrs else self.lib.dalek_b200_scalar_binary_batch
+        keep = (a, b)
+        r = self._scalar_results(fn, (self.SCALAR_BINARY_OPS.get(op, op), _ptr(a), n_a, _ptr(b), n_b, n), n, device_ptrs, out)
+        del keep
+        return r
+
+    def scalar_unary_batch(self, op, scalars, n, device_ptrs=False, out=None):
+        """out[i] = -S_i, S_i^-1 (0 for 0) or S_i / 2 for op "neg", "invert" or "div_by_2" (dalek_b200_scalar_unary_batch);
+        buffers as scalar_binary_batch."""
+        fn = self.lib.dalek_b200_scalar_unary_batch_dev if device_ptrs else self.lib.dalek_b200_scalar_unary_batch
+        return self._scalar_results(fn, (self.SCALAR_UNARY_OPS.get(op, op), _ptr(scalars), n), n, device_ptrs, out)
+
+    def scalar_from_bytes_batch(self, data, n, canonical=False):
+        """Scalar::from_bytes_mod_order, or from_canonical_bytes with `canonical`, for n x 32 B: (rc, n x 32 B, n ok bytes);
+        rc 1 (DALEK_NONE) when a canonical decoding fails (its ok byte is 0 and its slot zero)."""
+        out = (C.c_uint8 * (32 * max(n, 1)))()
+        ok = (C.c_uint8 * max(n, 1))()
+        rc = self._check(self.lib.dalek_b200_scalar_from_bytes_batch(self.h, _ptr(data), n, 1 if canonical else 0, C.addressof(out),
+                                                                     C.addressof(ok)))
+        return rc, bytes(out)[:32 * n], bytes(ok)[:n]
+
+    def scalar_hash_from_bytes_batch(self, msgs_flat, offsets, n):
+        """Scalar::hash_from_bytes::<Sha512> for n flat messages (layout of ristretto_hash_from_bytes_batch) -> n x 32 B."""
+        out = (C.c_uint8 * (32 * max(n, 1)))()
+        self._check(self.lib.dalek_b200_scalar_hash_from_bytes_batch(self.h, _ptr(msgs_flat), _ptr(offsets), n, C.addressof(out)))
+        return bytes(out)[:32 * n]
+
+    def scalar_fold_batch(self, op, scalars, offsets, m, device_ptrs=False, out=None):
+        """Sum or Product (op "sum" or "product") of each segment offsets[j] .. offsets[j+1] of the flat scalars
+        (dalek_b200_scalar_fold_batch): offsets are m + 1 uint64 starting at 0; an empty segment gives 0 or 1.  With
+        device_ptrs scalars, offsets and the results are device buffers.  -> m x 32 B."""
+        fn = self.lib.dalek_b200_scalar_fold_batch_dev if device_ptrs else self.lib.dalek_b200_scalar_fold_batch
+        keep = (scalars, offsets)
+        r = self._scalar_results(fn, (self.SCALAR_FOLD_OPS.get(op, op), _ptr(scalars), _ptr(offsets), m), m, device_ptrs, out)
+        del keep
+        return r
 
     # ---- batch codecs ----
     def decompress_batch(self, encodings, n, ristretto=False):
@@ -1069,6 +1136,151 @@ def _mul_base_batch(scalars, fmt, clamped, engine):
     raw = eng.mul_base_ct_batch(b"".join(ss), len(ss), fmt, clamped=clamped)
     outs = [raw[32 * i:32 * i + 32] for i in range(len(ss))]
     return outs[0] if single else outs
+
+
+def _scalar_binary(a, b, op, engine):
+    single_a, as_ = _items(a, 32, "scalars")
+    single_b, bs = _items(b, 32, "scalars")
+    n = _broadcast_len(single_a, as_, single_b, bs)
+    if n == 0:
+        return []
+    eng = engine or default_engine()
+    raw = eng.scalar_binary_batch(op, b"".join(as_), len(as_), b"".join(bs), len(bs), n)
+    outs = [raw[32 * i:32 * i + 32] for i in range(n)]
+    return outs[0] if single_a and single_b else outs
+
+
+def _scalar_unary(scalars, op, engine):
+    single, ss = _items(scalars, 32, "scalars")
+    if not ss:
+        return []
+    eng = engine or default_engine()
+    raw = eng.scalar_unary_batch(op, b"".join(ss), len(ss))
+    outs = [raw[32 * i:32 * i + 32] for i in range(len(ss))]
+    return outs[0] if single else outs
+
+
+def _scalar_fold_batch(scalar_lists, op, engine):
+    import array
+    lists = [_items(list(s), 32, "scalars")[1] for s in scalar_lists]
+    m = len(lists)
+    if m == 0:
+        return []
+    offs = array.array("Q", [0])
+    for s in lists:
+        offs.append(offs[-1] + len(s))
+    eng = engine or default_engine()
+    raw = eng.scalar_fold_batch(op, b"".join(b"".join(s) for s in lists) or b"\0", offs.tobytes(), m)
+    return [raw[32 * j:32 * j + 32] for j in range(m)]
+
+
+class Scalar:
+    """Mirror of curve25519_dalek::scalar::Scalar (scalar.rs) on 32-byte little-endian encodings, batched on the GPU.  One
+    item (bytes) gives one result, a list gives the list; in the binary forms a single item is used for every item of the
+    other operand.  The arithmetic takes canonical scalars (< l, invariant #2) and returns canonical ones; a
+    non-canonical input raises EngineError (the reference's Add and Sub are wrong for unreduced scalars, so nothing is
+    reduced silently).  Constant time in the scalar values."""
+
+    @staticmethod
+    def from_bytes_mod_order_batch(data, engine=None):
+        """Scalar::from_bytes_mod_order (scalar.rs:235-244): any 32 bytes, reduced mod l."""
+        single, items = _items(data, 32, "scalar encodings")
+        if not items:
+            return []
+        eng = engine or default_engine()
+        _, raw, _ = eng.scalar_from_bytes_batch(b"".join(items), len(items))
+        outs = [raw[32 * i:32 * i + 32] for i in range(len(items))]
+        return outs[0] if single else outs
+
+    @staticmethod
+    def from_bytes_mod_order_wide_batch(data, engine=None):
+        """Scalar::from_bytes_mod_order_wide (scalar.rs:248-250): any 64 bytes, reduced mod l."""
+        single, items = _items(data, 64, "wide scalar encodings")
+        if not items:
+            return []
+        eng = engine or default_engine()
+        raw = eng.scalar_from_wide_batch(b"".join(items), len(items))
+        outs = [raw[32 * i:32 * i + 32] for i in range(len(items))]
+        return outs[0] if single else outs
+
+    @staticmethod
+    def from_canonical_bytes_batch(data, engine=None):
+        """Scalar::from_canonical_bytes (scalar.rs:259-263): the 32 bytes when canonical, else None."""
+        single, items = _items(data, 32, "scalar encodings")
+        if not items:
+            return []
+        eng = engine or default_engine()
+        _, raw, ok = eng.scalar_from_bytes_batch(b"".join(items), len(items), canonical=True)
+        outs = [raw[32 * i:32 * i + 32] if ok[i] else None for i in range(len(items))]
+        return outs[0] if single else outs
+
+    @staticmethod
+    def hash_from_bytes_batch(messages, engine=None):
+        """Scalar::hash_from_bytes::<Sha512> (scalar.rs:617-624): SHA-512 of each message mod l, the list of scalars."""
+        eng = engine or default_engine()
+        flat, offs, n = _flat_messages(messages)
+        raw = eng.scalar_hash_from_bytes_batch(flat, offs, n)
+        return [raw[32 * i:32 * i + 32] for i in range(n)]
+
+    @staticmethod
+    def add_batch(a, b, engine=None):
+        """Add (scalar.rs:334-349): a + b mod l."""
+        return _scalar_binary(a, b, "add", engine)
+
+    @staticmethod
+    def sub_batch(a, b, engine=None):
+        """Sub (scalar.rs:354-362): a - b mod l."""
+        return _scalar_binary(a, b, "sub", engine)
+
+    @staticmethod
+    def mul_batch(a, b, engine=None):
+        """Mul (scalar.rs:317-322): a b mod l."""
+        return _scalar_binary(a, b, "mul", engine)
+
+    @staticmethod
+    def neg_batch(scalars, engine=None):
+        """Neg (scalar.rs:366-374): -s mod l (0 for 0)."""
+        return _scalar_unary(scalars, "neg", engine)
+
+    @staticmethod
+    def div_by_2_batch(scalars, engine=None):
+        """Scalar::div_by_2 (scalar.rs:858-870): s / 2 mod l."""
+        return _scalar_unary(scalars, "div_by_2", engine)
+
+    @staticmethod
+    def invert_each(scalars, engine=None):
+        """Scalar::invert (scalar.rs:739-741) of each scalar on its own: s^(l-2), so 0 gives 0.  Not the reference's
+        invert_batch, which requires nonzero inputs and returns the product of the inverses."""
+        return _scalar_unary(scalars, "invert", engine)
+
+    @staticmethod
+    def invert_batch_alloc(scalars, engine=None):
+        """Scalar::invert_batch_alloc (scalar.rs:802-853): (the list of inverses, the product of all inverses).  Inputs are
+        taken mod l; a zero input raises EngineError, as the reference requires nonzero inputs."""
+        _, ss = _items(list(scalars), 32, "scalars")
+        eng = engine or default_engine()
+        raw, prod = eng.scalar_invert_batch(b"".join(ss) or b"\0", len(ss))
+        return [raw[32 * i:32 * i + 32] for i in range(len(ss))], prod
+
+    @staticmethod
+    def sum(scalars, engine=None):
+        """Sum<T> (scalar.rs:466-476): the sum of the scalars, 0 when there are none."""
+        return _scalar_fold_batch([list(scalars)], "sum", engine)[0]
+
+    @staticmethod
+    def sum_batch(scalar_lists, engine=None):
+        """The Sum of each list of scalars, one call for all lists."""
+        return _scalar_fold_batch(scalar_lists, "sum", engine)
+
+    @staticmethod
+    def product(scalars, engine=None):
+        """Product<T> (scalar.rs:454-464): the product of the scalars, 1 when there are none."""
+        return _scalar_fold_batch([list(scalars)], "product", engine)[0]
+
+    @staticmethod
+    def product_batch(scalar_lists, engine=None):
+        """The Product of each list of scalars, one call for all lists."""
+        return _scalar_fold_batch(scalar_lists, "product", engine)
 
 
 class MontgomeryPoint:

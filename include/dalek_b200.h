@@ -89,7 +89,8 @@ int dalek_b200_last_kernel_ms(const dalek_b200_ctx *ctx, float *ms, int *launche
 int dalek_b200_last_stage_ms(const dalek_b200_ctx *ctx, const char *stage, float *ms);
 /* Milliseconds between CUDA events recorded on the context's stream at entry of the last MSM / verify_batch /
  * precomputed-MSM / X25519 / to_montgomery_batch / hash-to-group / Lizard / map_to_curve / map_to_curve_inverse / mul_batch
- * / vartime_double_base_batch / MontgomeryPoint / mul_base_ct_batch call, or of the last ed25519_b200_verifying_keys /
+ * / vartime_double_base_batch / MontgomeryPoint / mul_base_ct_batch / scalar_binary_batch / scalar_unary_batch /
+ * scalar_from_bytes_batch / scalar_hash_from_bytes_batch / scalar_fold_batch call, or of the last ed25519_b200_verifying_keys /
  * sign_flat / sign_prehashed / verify_prehashed_each call, and after the last work it enqueued (all of the call's streams
  * joined): the device time of that call, copies of host-buffer calls included. */
 int dalek_b200_last_call_ms(const dalek_b200_ctx *ctx, float *ms);
@@ -486,6 +487,59 @@ int dalek_b200_scalar_from_wide_batch(dalek_b200_ctx *ctx, const uint8_t *in, si
  * nonzero inputs (scalar.rs:796-799): a zero input is DALEK_E_INVALID_ARG here. */
 int dalek_b200_scalar_invert_batch(dalek_b200_ctx *ctx, const uint8_t *in, size_t n, uint8_t *out,
                                    uint8_t out_product[32]);
+
+/* -------- scalar arithmetic ------------------------------------------------------------------------
+ * Add, Sub, Mul, Neg, invert, div_by_2, from_bytes_mod_order, from_canonical_bytes, hash_from_bytes, Sum and Product of
+ * Scalar (C/scalar.rs:235-263, :317-374, :454-476, :617-670, :739-741, :858-870) over batches of 32-byte little-endian
+ * scalars.
+ *   Inputs of the arithmetic (binary, unary and fold calls) must be canonical, < l (Scalar invariant #2,
+ *     C/scalar.rs:207-228).  Bit 255 set or a value in [l, 2^255) makes the call return DALEK_E_INVALID_ARG after the
+ *     batch has run, host and _dev calls alike; the outputs are then unspecified.  Inputs are never reduced silently:
+ *     the reference's own Add and Sub are wrong for unreduced scalars (clamped secrets, for example).
+ *   Results are canonical.  invert(0) = 0 (the reference's exponentiation gives 0^(l-2) = 0), Neg(0) = 0, the empty Sum
+ *     is 0 and the empty Product is 1.
+ *   Broadcast: n_a and n_b are each 1 or n.  out may equal a non-broadcast input exactly (in place); any other overlap is
+ *     the caller's error.  n = 0 (m = 0) is a successful no-op.  A NULL buffer with items to process is
+ *     DALEK_E_INVALID_ARG, except ok.  Bad ops, modes and offsets, and item counts of 2^56 or more, are found before any device
+ *     work.
+ *   Constant time in the scalar values at every batch size: no branch, loop bound or address depends on a value; the op,
+ *     mode, counts, broadcast and segment offsets are public, and so is the inversion's exponent l - 2.
+ *   Host-buffer calls stream the batch in pieces and clear the device copies of their inputs, intermediates and results
+ *     before they return, also after a failed launch; the _dev calls clear the engine's intermediates.  No option affects
+ *     these calls. */
+#define DALEK_SCALAR_ADD 0                /* scalar_binary_batch ops */
+#define DALEK_SCALAR_SUB 1
+#define DALEK_SCALAR_MUL 2
+#define DALEK_SCALAR_NEG 0                /* scalar_unary_batch ops */
+#define DALEK_SCALAR_INVERT 1             /* Scalar::invert per item; 0 -> 0 */
+#define DALEK_SCALAR_DIV_BY_2 2
+#define DALEK_SCALAR_SUM 0                /* scalar_fold_batch ops */
+#define DALEK_SCALAR_PRODUCT 1
+#define DALEK_SCALAR_MOD_ORDER 0          /* scalar_from_bytes_batch modes */
+#define DALEK_SCALAR_CANONICAL 1
+/* out[i] = A_i + B_i, A_i - B_i or A_i * B_i (op DALEK_SCALAR_ADD, _SUB, _MUL).  out: n x 32 B. */
+int dalek_b200_scalar_binary_batch(dalek_b200_ctx *ctx, int op, const uint8_t *a, size_t n_a, const uint8_t *b, size_t n_b, size_t n,
+                                   uint8_t *out);
+/* same, every buffer a device pointer; blocks until done */
+int dalek_b200_scalar_binary_batch_dev(dalek_b200_ctx *ctx, int op, const void *d_a, size_t n_a, const void *d_b, size_t n_b, size_t n,
+                                       void *d_out);
+/* out[i] = -S_i, S_i^-1 (0 for 0) or S_i / 2 (op DALEK_SCALAR_NEG, _INVERT, _DIV_BY_2) */
+int dalek_b200_scalar_unary_batch(dalek_b200_ctx *ctx, int op, const uint8_t *in, size_t n, uint8_t *out);
+int dalek_b200_scalar_unary_batch_dev(dalek_b200_ctx *ctx, int op, const void *d_in, size_t n, void *d_out);
+/* MOD_ORDER: Scalar::from_bytes_mod_order, any 32 bytes reduced mod l (ok all 1).  CANONICAL:
+ * Scalar::from_canonical_bytes, ok[i] = 0 and zero bytes for bit 255 set or value >= l (None); the call then returns
+ * DALEK_NONE.  Host buffers; ok n bytes, nullable. */
+int dalek_b200_scalar_from_bytes_batch(dalek_b200_ctx *ctx, const uint8_t *in, size_t n, int mode, uint8_t *out, uint8_t *ok);
+/* Scalar::hash_from_bytes::<Sha512>: SHA-512 of each message, reduced mod l as from_bytes_mod_order_wide.  Flat messages
+ * as in the hash-to-group block; constant time in the message bytes.  out: n x 32 B. */
+int dalek_b200_scalar_hash_from_bytes_batch(dalek_b200_ctx *ctx, const uint8_t *msgs_flat, const uint64_t *msg_offsets, size_t n,
+                                            uint8_t *out);
+/* Sum / Product (op DALEK_SCALAR_SUM, _PRODUCT) of each segment: result j folds the scalars offsets[j] .. offsets[j+1]
+ * (m + 1 u64 offsets, offsets[0] = 0, non-decreasing, offsets[m] < 2^31, else DALEK_E_INVALID_ARG before any device
+ * work).  out: m x 32 B.  The ring is commutative, so the result is exact whatever order the fold takes. */
+int dalek_b200_scalar_fold_batch(dalek_b200_ctx *ctx, int op, const uint8_t *scalars, const uint64_t *offsets, size_t m, uint8_t *out);
+/* same, every buffer a device pointer; the offsets are read back once (8 bytes per segment) to plan the chunks */
+int dalek_b200_scalar_fold_batch_dev(dalek_b200_ctx *ctx, int op, const void *d_scalars, const void *d_offsets, size_t m, void *d_out);
 
 /* -------- RistrettoPoint ----------------------------------------------------------------- */
 /* n independent RistrettoPoint::multiscalar_mul([a_i, b_i], [G, H]) (constant-time Straus,
