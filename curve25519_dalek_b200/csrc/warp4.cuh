@@ -52,25 +52,6 @@ __device__ __forceinline__ void w4_store(ge_p3_raw *dst, const w4_point &p, uint
     for (int i = 0; i < 10; i += 2) *reinterpret_cast<uint2 *>(o + i) = make_uint2(mine.v[i], mine.v[i + 1]);
 }
 
-// p <- 2p.  T is refreshed only when want_t (the doubling that precedes an addition).
-__device__ __forceinline__ void w4_dbl(w4_point &p, uint32_t role, bool want_t)
-{
-    fe S, in, r, XX, YY, ZZ, S2, t, Xc, Yc, Zc, Tc, f, g;
-    fe_add(S, p.X, p.Y);
-    fe_sel4(in, p.X, p.Y, p.Z, S, role);
-    fe_sq(r, in);
-    fe_gbcast(XX, r, 0); fe_gbcast(YY, r, 1); fe_gbcast(ZZ, r, 2); fe_gbcast(S2, r, 3);
-    fe_sub(t, S2, YY); fe_sub(t, t, XX); fe_carry(Xc, t);      // X' = (X+Y)^2 - YY - XX   (1)
-    fe_add(Yc, YY, XX);                                       // Y' = YY + XX              (2)
-    fe_sub(Zc, YY, XX);                                       // Z' = YY - XX              (3)
-    fe_add(t, ZZ, ZZ); fe_add(t, t, XX); fe_sub(Tc, t, YY);   // T' = 2ZZ - (YY - XX)      (5)
-    fe_sel4(f, Tc, Zc, Tc, Yc, role);                         // X3 = T'X', Y3 = Z'Y', Z3 = T'Z', T3 = Y'X'
-    fe_sel4(g, Xc, Yc, Zc, Xc, role);
-    fe_mul(r, f, g);
-    fe_gbcast(p.X, r, 0); fe_gbcast(p.Y, r, 1); fe_gbcast(p.Z, r, 2);
-    if (want_t) fe_gbcast(p.T, r, 3);
-}
-
 // p <- p + q (both extended, curve25519-dalek/src/edwards.rs:795-800 = :528-535 + curve_models.rs:411-430, :365-372)
 __device__ __forceinline__ void w4_add(w4_point &p, const w4_point &q, uint32_t role)
 {

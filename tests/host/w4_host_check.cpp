@@ -179,6 +179,21 @@ int h_w20_carry(const double *a)
     return 1;
 }
 
+// The raw output limbs of all 32 lanes of w20_mul (op 0), w20_carry (op 1) or w20_invert (op 2) for nw warps of four
+// elements each (a, b: nw x 20 limbs as integers; out: nw x 32 limbs), so that the device build of the same code can be
+// compared with this emulation limb for limb: the floored split, the carry rounded to nearest even, the carry schedule.
+void h_w20_raw(int op, int nw, const long long *a, const long long *b, long long *out)
+{
+    run_warp([&](uint32_t lane) {
+        const w20_role r = w20_roles();
+        for (int w = 0; w < nw; w++) {
+            const double x = (double)a[20 * w + r.base + r.i], y = (double)b[20 * w + r.base + r.i];
+            const double o = op == 0 ? w20_mul(x, y, r) : op == 1 ? w20_carry(x, r) : w20_invert(x, r);
+            out[32 * w + lane] = (long long)o;
+        }
+    });
+}
+
 // k doublings of one point on 20 lanes (w20_dbl_n) -> compressed
 int h_w20_dbl_n(uint8_t *out, const uint8_t *point, int k)
 {
