@@ -36,15 +36,18 @@ touches the CPU checker used by the tests.  Names follow the reference:
       / add_batch / sub_batch / mul_batch / neg_batch / div_by_2_batch / invert_each / invert_batch_alloc / sum / sum_batch
       / product / product_batch (src/scalar.rs:235-263, :317-374, :454-476, :617-670, :739-870): arithmetic mod l on
       canonical scalars, one thread per item, and many segmented sums and products in one call
+  EdwardsBasepointTable / RistrettoBasepointTable .create / basepoint / mul_base_batch / mul_base_clamped_batch
+      (traits.rs:50-74, src/edwards.rs:1127-1243, src/ristretto.rs:1080-1115): resident tables of k points, constant-time
+      s * P_{t_i} per item
 """
 from .engine import (Engine, MultiEngine, EngineError, EdwardsPoint, RistrettoPoint, MontgomeryPoint, Scalar, SignatureError, verify_batch, default_engine,
                      library_path, load_library, POINTS_COMPRESSED, POINTS_EXTENDED, POINTS_RISTRETTO, POINTS_MONTGOMERY,
                      VartimeEdwardsPrecomputation, VartimeRistrettoPrecomputation, x25519, x25519_public_keys,
                      X25519_BASEPOINT_BYTES, ed25519_verifying_keys, ed25519_sign, ed25519_sign_prehashed,
-                     ed25519_verify_prehashed, ed25519_to_montgomery)
+                     ed25519_verify_prehashed, ed25519_to_montgomery, EdwardsBasepointTable, RistrettoBasepointTable)
 
 __all__ = ["Engine", "MultiEngine", "EngineError", "EdwardsPoint", "RistrettoPoint", "MontgomeryPoint", "Scalar", "SignatureError", "verify_batch", "default_engine",
            "library_path", "load_library", "POINTS_COMPRESSED", "POINTS_EXTENDED", "POINTS_RISTRETTO", "POINTS_MONTGOMERY",
            "VartimeEdwardsPrecomputation", "VartimeRistrettoPrecomputation", "x25519", "x25519_public_keys",
            "X25519_BASEPOINT_BYTES", "ed25519_verifying_keys", "ed25519_sign", "ed25519_sign_prehashed",
-           "ed25519_verify_prehashed", "ed25519_to_montgomery"]
+           "ed25519_verify_prehashed", "ed25519_to_montgomery", "EdwardsBasepointTable", "RistrettoBasepointTable"]

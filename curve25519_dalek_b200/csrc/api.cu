@@ -81,6 +81,7 @@ int dalek_b200_set_option(dalek_b200_ctx *ctx, const char *name, long value)
     if (!strcmp(name, "verify_pieces")) { if (value < 1 || value > 8) return DALEK_E_INVALID_ARG; ctx->opt_verify_pieces = value; return 0; }
     if (!strcmp(name, "transcript_warp")) { ctx->opt_transcript_warp = value ? 1 : 0; return 0; }
     if (!strcmp(name, "transcript_blocks")) { ctx->opt_transcript_blocks = value ? 1 : 0; return 0; }
+    if (!strcmp(name, "bpt_group")) { ctx->opt_bpt_group = value ? 1 : 0; return 0; }
     if (!strcmp(name, "each_comb")) { if (value < 0 || value > 2) return DALEK_E_INVALID_ARG; ctx->opt_each_comb = value; return 0; }
     if (!strcmp(name, "small_straus")) { ctx->opt_small_straus = value ? 1 : 0; return 0; }
     if (!strcmp(name, "acc_tma")) { ctx->opt_acc_tma = value ? 1 : 0; return 0; }
@@ -96,7 +97,7 @@ int dalek_b200_get_option(const dalek_b200_ctx *ctx, const char *name, long *val
         {"window_bits", ctx->opt_window_bits}, {"host_chunks", ctx->opt_host_chunks}, {"decompress_f64", ctx->opt_decompress_f64},
         {"trace", ctx->opt_trace}, {"precomp_tables", ctx->opt_precomp_tables}, {"double_base_comb", ctx->opt_double_base_comb},
         {"dedupe_keys", ctx->opt_dedupe_keys}, {"verify_pieces", ctx->opt_verify_pieces}, {"transcript_warp", ctx->opt_transcript_warp},
-        {"transcript_blocks", ctx->opt_transcript_blocks}, {"each_comb", ctx->opt_each_comb}, {"small_straus", ctx->opt_small_straus},
+        {"transcript_blocks", ctx->opt_transcript_blocks}, {"each_comb", ctx->opt_each_comb}, {"bpt_group", ctx->opt_bpt_group}, {"small_straus", ctx->opt_small_straus},
         {"acc_tma", ctx->opt_acc_tma}, {"field_f64", ctx->opt_field_f64}, {"verify_chunk", ctx->opt_verify_chunk}};
     for (const auto &o : opts)
         if (!strcmp(name, o.name)) { *value = o.v; return 0; }

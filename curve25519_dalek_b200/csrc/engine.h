@@ -75,6 +75,10 @@ enum WsRole {
     // ---- scalar arithmetic (scalars.cu) ----
     // scalars.cu [call] the scalar Sum / Product: chunk plans, partial sums or products, results
     WS_SCALAR_FOLD,
+    // ---- resident basepoint tables (varmul.cu) ----
+    // varmul.cu [call] the items of a many-table multiplication grouped by table: a count per table for each of the two
+    // streams, then the order of the items
+    WS_BPT_ORDER,
     // ---- the MSM engine (msm.cu) and the Straus paths that stand in for it ----
     // msm.cu [call] extended-point preparation: the Z product of each group of points (then its inverse), running products
     WS_PREP_PROD,
@@ -186,6 +190,7 @@ struct dalek_b200_ctx {
     long opt_acc_tma = 0;       // bucket kernel gathers points with TMA bulk copies + mbarriers instead of cp.async (A/B option)
     long opt_transcript_warp = 1; // up to 2048 Merlin transcripts per launch run one WARP each (25-lane Keccak); 0 = one thread each
     long opt_transcript_blocks = 1; // more transcripts than that: one THREAD each with the rate block staged in shared memory (0 = byte-wise sponge)
+    long opt_bpt_group = 1;     // basepoint tables: 1 = group a many-table call's items by table before multiplying, 0 = per-lane gathers
     long opt_each_comb = 1;     // verify_each: 1 = per-key comb tables when every key signs >= 8 signatures on average, 2 = always, 0 = never
     long opt_small_straus = 1;  // fewer than 190 pairs: vartime Straus (3 launches) instead of the bucket pipeline
     long opt_field_f64 = 1;     // bucket kernel on the FP64 pipe (fe64.cuh) instead of IMAD.WIDE (fe.cuh)

@@ -78,6 +78,14 @@ def load_library():
     lib.dalek_b200_precomp_destroy.argtypes = [vp]
     lib.dalek_b200_precomp_destroy.restype = None
     lib.dalek_b200_precomp_mixed_msm.argtypes = [vp, vp, vp, sz, vp, vp, C.c_int, sz, vp, vp]
+    lib.dalek_b200_basepoint_tables_new.argtypes = [vp, vp, C.c_int, sz, vp, C.POINTER(vp)]
+    lib.dalek_b200_basepoint_tables_len.argtypes = [vp]
+    lib.dalek_b200_basepoint_tables_len.restype = sz
+    lib.dalek_b200_basepoint_tables_destroy.argtypes = [vp]
+    lib.dalek_b200_basepoint_tables_destroy.restype = None
+    lib.dalek_b200_basepoint_tables_basepoints.argtypes = [vp, vp, vp]
+    lib.dalek_b200_basepoint_tables_mul.argtypes = [vp, vp, vp, vp, sz, C.c_int, vp]
+    lib.dalek_b200_basepoint_tables_mul_dev.argtypes = [vp, vp, vp, vp, sz, C.c_int, vp]
     lib.dalek_b200_edwards_decompress_batch.argtypes = [vp, vp, sz, vp, vp]
     lib.dalek_b200_ristretto_decompress_batch.argtypes = [vp, vp, sz, vp, vp]
     lib.dalek_b200_edwards_compress_batch.argtypes = [vp, vp, sz, vp]
@@ -502,6 +510,45 @@ class Engine:
         rc = self._check(self.lib.dalek_b200_mul_batch(self.h, _ptr(scalars), n_scalars, _ptr(points), point_fmt, n_points, n, flags,
                                                        _ptr(res), C.addressof(ok) if want_ok else None))
         return rc, (bytes(res)[:32 * n] if out is None else out), (bytes(ok)[:n] if want_ok else None)
+
+    # ---- resident basepoint tables ----
+    def basepoint_tables_new(self, points, k, point_fmt=POINTS_COMPRESSED):
+        """dalek_b200_basepoint_tables_new: the comb tables of k points (k x 32-byte encodings, or k x 20 u64 limbs with
+        POINTS_EXTENDED).  Returns (rc, handle or None, ok); rc 1 (DALEK_NONE) when a point does not decode (its ok byte
+        is 0, and no handle is made)."""
+        h = C.c_void_p()
+        ok = (C.c_uint8 * max(k, 1))()
+        rc = self._check(self.lib.dalek_b200_basepoint_tables_new(self.h, _ptr(points), point_fmt, k, C.addressof(ok), C.byref(h)))
+        return rc, (h if h.value else None), bytes(ok)[:k]
+
+    def basepoint_tables_len(self, handle):
+        return int(self.lib.dalek_b200_basepoint_tables_len(handle))
+
+    def basepoint_tables_destroy(self, handle):
+        self.lib.dalek_b200_basepoint_tables_destroy(handle)
+
+    def basepoint_tables_basepoints(self, handle):
+        """The encodings of the k points of the handle, read back from their tables: k x 32 bytes."""
+        k = self.basepoint_tables_len(handle)
+        res = (C.c_uint8 * (32 * max(k, 1)))()
+        self._check(self.lib.dalek_b200_basepoint_tables_basepoints(self.h, handle, C.addressof(res)))
+        return bytes(res)[:32 * k]
+
+    def basepoint_tables_mul(self, handle, scalars, indices, n, clamped=False, device_ptrs=False, out=None):
+        """out[i] = s_i * P_{t_i} (dalek_b200_basepoint_tables_mul): indices holds n uint32 table indices, or None for
+        table 0.  Host buffers give bytes.  With device_ptrs the inputs are device buffers and the results go to `out`
+        (32 n bytes on the engine's device, a new uint8 tensor if not given)."""
+        flags = 1 if clamped else 0
+        if device_ptrs:
+            if out is None:
+                import torch
+                out = torch.empty(32 * max(n, 1), dtype=torch.uint8, device=torch.device("cuda", self.device))
+            self._check(self.lib.dalek_b200_basepoint_tables_mul_dev(self.h, handle, _ptr(scalars), _ptr(indices), n, flags,
+                                                                     _ptr(out)))
+            return out
+        res = (C.c_uint8 * (32 * max(n, 1)))() if out is None else out
+        self._check(self.lib.dalek_b200_basepoint_tables_mul(self.h, handle, _ptr(scalars), _ptr(indices), n, flags, _ptr(res)))
+        return bytes(res)[:32 * n] if out is None else out
 
     # ---- variable-time double-base scalar multiplication ----
     def vartime_double_base_batch(self, ab, points, n, point_fmt=POINTS_COMPRESSED, device_ptrs=False, out=None, want_ok=False):
@@ -1612,6 +1659,101 @@ class VartimeEdwardsPrecomputation(_Precomputation):
 
 class VartimeRistrettoPrecomputation(_Precomputation):
     """curve25519-dalek/src/ristretto.rs:1004-1049 (CompressedRistretto encodings in and out)."""
+    _FMT = POINTS_RISTRETTO
+
+
+class _BasepointTable:
+    """BasepointTable (traits.rs:50-74) for k >= 1 points at once, resident on the GPU: the comb tables of every point
+    stay in device memory until close(), and each multiplication sends scalars (and table indices) only."""
+    _FMT = POINTS_COMPRESSED
+
+    def __init__(self, points, engine=None, fmt=None):
+        """points = iterable of 32-byte encodings (or, with fmt=POINTS_EXTENDED, a buffer of k x 20 u64 limbs passed as
+        (buffer, k)).  A point that does not decode raises ValueError naming the first one."""
+        self.h = None
+        self.eng = engine or default_engine()
+        fmt = self._FMT if fmt is None else fmt
+        if fmt == POINTS_EXTENDED:
+            if self._FMT == POINTS_RISTRETTO:
+                raise ValueError("Ristretto tables are made from CompressedRistretto encodings")
+            buf, k = points
+            nbytes = buf.nbytes if hasattr(buf, "nbytes") else (buf.numel() * buf.element_size() if hasattr(buf, "numel")
+                                                                else len(buf))
+            if nbytes < 160 * k:
+                raise ValueError("%d extended points take %d bytes, the buffer holds %d" % (k, 160 * k, nbytes))
+        else:
+            _, pts = _items(list(points), 32, "points")
+            buf, k = b"".join(pts), len(pts)
+        if k == 0:
+            raise ValueError("a basepoint table needs at least one point")
+        rc, h, ok = self.eng.basepoint_tables_new(buf, k, fmt)
+        if rc == 1:
+            raise ValueError("point %d does not decode" % ok.index(0))
+        self.h, self.k, self._bases = h, k, None
+
+    @classmethod
+    def create(cls, point, engine=None):
+        """create (traits.rs:56): the table of one point."""
+        return cls([point], engine=engine)
+
+    def __len__(self):
+        return self.k
+
+    def basepoint(self, i=0):
+        """basepoint (traits.rs:59): the canonical encoding of point i, read back from its table (all k once, then kept)."""
+        if not 0 <= i < self.k:
+            raise IndexError("table index out of range")
+        if self._bases is None:
+            self._bases = self.eng.basepoint_tables_basepoints(self.h)
+        return self._bases[32 * i:32 * i + 32]
+
+    def _mul(self, scalars, indices, clamped):
+        single, ss = _items(scalars, 32, "scalars")
+        if not ss:
+            return []
+        if not clamped and any(s[31] & 0x80 for s in ss):
+            raise ValueError("a scalar has bit 255 set")
+        idx = None
+        if indices is not None:
+            import array
+            idx = array.array("I", indices)
+            if len(idx) != len(ss):
+                raise ValueError("one table index per scalar")
+            if max(idx) >= self.k:
+                raise ValueError("a table index is not below len()")
+            idx = idx.tobytes()
+        raw = self.eng.basepoint_tables_mul(self.h, b"".join(ss), idx, len(ss), clamped=clamped)
+        outs = [raw[32 * i:32 * i + 32] for i in range(len(ss))]
+        return outs[0] if single else outs
+
+    def mul_base_batch(self, scalars, indices=None):
+        """mul_base (traits.rs:62) for each 32-byte scalar (bit 255 clear, not reduced), through table indices[i] (None:
+        table 0).  Constant time in the scalars.  Returns the encoding, or the list."""
+        return self._mul(scalars, indices, False)
+
+    def mul_base_clamped_batch(self, bytes_list, indices=None):
+        """mul_base_clamped (traits.rs:66-74): any 32 bytes, clamped and not reduced; like mul_base_batch."""
+        return self._mul(bytes_list, indices, True)
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.eng.basepoint_tables_destroy(self.h)          # does not use the engine's context: safe after its close()
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class EdwardsBasepointTable(_BasepointTable):
+    """EdwardsBasepointTable (edwards.rs:1127-1243): CompressedEdwardsY (or extended limbs) in, CompressedEdwardsY out."""
+    _FMT = POINTS_COMPRESSED
+
+
+class RistrettoBasepointTable(_BasepointTable):
+    """RistrettoBasepointTable (ristretto.rs:1080-1115): CompressedRistretto in and out."""
     _FMT = POINTS_RISTRETTO
 
 

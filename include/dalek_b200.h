@@ -73,7 +73,9 @@ const char *dalek_b200_last_error(const dalek_b200_ctx *ctx);
  * kernel what the shorter tail saves), "transcript_warp" (1 = launches of up to 2048 Merlin transcripts run one warp each,
  * default), "transcript_blocks" (1 = larger launches run one thread per transcript with the rate block staged in shared
  * memory, default; 0 = byte-wise sponge), "each_comb" (per-signature verification: 1 = per-key comb tables when
- * every distinct key signs at least eight signatures on average, default; 2 = always; 0 = never), "trace" (1 = per-stage
+ * every distinct key signs at least eight signatures on average, default; 2 = always; 0 = never), "bpt_group" (basepoint
+ * tables: 1 = a many-table multiplication first groups its items by table on the device, default; 0 = every lane reads its
+ * own table), "trace" (1 = per-stage
  * device timeline of verify_batch on stderr).
  * Returns 0 or DALEK_E_INVALID_ARG. */
 int dalek_b200_set_option(dalek_b200_ctx *ctx, const char *name, long value);
@@ -211,6 +213,51 @@ int dalek_b200_precomp_mixed_msm(dalek_b200_ctx *ctx, const dalek_b200_precomp *
                                  int dynamic_fmt, size_t n_dynamic, uint8_t out_compressed[32],
                                  uint64_t out_limbs[20]);
 
+/* -------- BasepointTable: resident fixed-base tables of any points ------------------------------------------------------
+ * C/traits.rs:50-74; EdwardsBasepointTable C/edwards.rs:1127-1243, RistrettoBasepointTable C/ristretto.rs:1080-1115.
+ * A handle holds the comb tables of k points P_0..P_{k-1} in device memory: 64 rows of 8 entries (j+1) 16^i P as FP64
+ * affine Niels, 61,440 bytes per point, allocated by new and freed by destroy.  The tables are not a context workspace;
+ * a handle serves only the context that made it (another context is DALEK_E_INVALID_ARG).
+ *   Formats: COMPRESSED and EXTENDED make Edwards tables (CompressedEdwardsY out), RISTRETTO makes Ristretto tables
+ *     (CompressedRistretto out); anything else is DALEK_E_INVALID_ARG.
+ *   Constant time in the scalars at every batch size: every table row is scanned in full and the sign is applied
+ *     inside the addition.  The points, the indices, k and n are public: a table address depends on an index, never on
+ *     a scalar.  Every use of a basepoint table (a generator, a recipient's key, a commitment base) has public bases.
+ *
+ * create (traits.rs:56) for k >= 1 points (k = 0 is DALEK_E_INVALID_ARG): *out = the handle.  If a point does not
+ * decode, ok[i] = 0 for it (ok: k bytes, nullable; 1 for every other point), *out stays NULL, nothing stays allocated
+ * and the call returns DALEK_NONE.  A failed allocation returns DALEK_E_NOMEM with last_error set and no handle. */
+typedef struct dalek_b200_basepoint_tables dalek_b200_basepoint_tables;
+int dalek_b200_basepoint_tables_new(dalek_b200_ctx *ctx, const void *points, int point_fmt, size_t k,
+                                    uint8_t *ok /* k bytes, nullable */, dalek_b200_basepoint_tables **out);
+size_t dalek_b200_basepoint_tables_len(const dalek_b200_basepoint_tables *t);
+/* destroy waits for the device and frees the tables; it does not use the context, so a handle may be destroyed before
+ * or after its context.  NULL is a no-op. */
+void dalek_b200_basepoint_tables_destroy(dalek_b200_basepoint_tables *t);
+/* basepoint (traits.rs:59, C/edwards.rs:1144-1148, C/ristretto.rs:1108-1110): the k encodings of P_i read back from
+ * entry (0, 0) of each table: the canonical encoding of the decoded point (a non-canonical CompressedEdwardsY comes
+ * back canonical, a Ristretto point as the canonical encoding of its coset). */
+int dalek_b200_basepoint_tables_basepoints(dalek_b200_ctx *ctx, const dalek_b200_basepoint_tables *t,
+                                           uint8_t *out /* k x 32 B */);
+/* mul_base / mul_base_clamped (traits.rs:62-74, C/edwards.rs:1192-1243): out[i] = s_i P_{t_i}, t_i = indices[i]
+ * (indices NULL: table 0 serves every item).  The scalar is used as the integer it is, not reduced mod l, so out[i]
+ * equals dalek_b200_mul_batch(s_i, P_{t_i}) for every input, points with a torsion component included.  flags = 0:
+ * bit 255 set is DALEK_E_INVALID_ARG; flags = DALEK_MUL_CLAMPED: any 32 bytes, clamped (clamp_integer,
+ * C/scalar.rs:1407-1412) and not reduced, for Edwards and Ristretto tables alike (the trait's default method).  Other
+ * flag bits are DALEK_E_INVALID_ARG.  An index >= k is DALEK_E_INVALID_ARG.  Host buffers: the scalar and index checks
+ * run before any device work; the batch is streamed in pieces and the device copies of the scalars and results are
+ * cleared before the call returns, failed calls included.  n = 0 is a successful no-op; a NULL scalars or out with
+ * n > 0 is DALEK_E_INVALID_ARG.  With indices, the items are first grouped by table on the device (a counting sort of
+ * the public indices; option "bpt_group"), so that the threads of a warp read the same table rows. */
+int dalek_b200_basepoint_tables_mul(dalek_b200_ctx *ctx, const dalek_b200_basepoint_tables *t,
+                                    const uint8_t *scalars, const uint32_t *indices /* n, or NULL */, size_t n,
+                                    int flags, uint8_t *out /* n x 32 B */);
+/* same, every buffer a device pointer; blocks until done.  A scalar with bit 255 set (without the clamp flag) or an
+ * index >= k is reported after the batch ran: the call returns DALEK_E_INVALID_ARG and the outputs are unspecified.
+ * An index >= k is never used as an address: the kernel reads table 0 in its place. */
+int dalek_b200_basepoint_tables_mul_dev(dalek_b200_ctx *ctx, const dalek_b200_basepoint_tables *t,
+                                        const void *d_scalars, const void *d_indices, size_t n, int flags, void *d_out);
+
 /* -------- batch wire-format codecs (SURVEY 8f rank 2) -----------------------------------------
  * Points are the reference's in-memory EdwardsPoint / RistrettoPoint: 20 u64 limbs X | Y | Z | T, radix 2^51.
  * Host buffers; the batch is streamed in pieces so that the copies overlap the arithmetic.
@@ -297,9 +344,9 @@ int dalek_b200_mul_base_ct_batch(dalek_b200_ctx *ctx, const uint8_t *scalars, si
 
 /* -------- variable-base scalar multiplication -------------------------------------------------
  * out[i] = s_i * P_i: EdwardsPoint * Scalar (C/edwards.rs:890-899 -> C/backend/serial/scalar_mul/variable_base.rs:11-48),
- * EdwardsPoint::mul_clamped (C/edwards.rs:932-941) and RistrettoPoint * Scalar (C/ristretto.rs:917-926); with one point
- * for the whole batch also BasepointTable::create(P) * s and mul_base_clamped (C/edwards.rs:1140-1230,
- * C/ristretto.rs:1086-1103), which give the same points.
+ * EdwardsPoint::mul_clamped (C/edwards.rs:932-941) and RistrettoPoint * Scalar (C/ristretto.rs:917-926).
+ * BasepointTable::create(P) * s, with the table kept between calls, is dalek_b200_basepoint_tables_mul; it gives the
+ * same points.
  *   Broadcast: n_scalars and n_points are each 1 or n; 1 uses that input for every item, any other value is
  *     DALEK_E_INVALID_ARG.  n = 0 is a successful no-op.  A NULL buffer with n > 0 is DALEK_E_INVALID_ARG, except ok.
  *   Point formats: COMPRESSED (CompressedEdwardsY in and out), EXTENDED (20 radix-2^51 limbs in, any Z;
