@@ -39,15 +39,19 @@ touches the CPU checker used by the tests.  Names follow the reference:
   EdwardsBasepointTable / RistrettoBasepointTable .create / basepoint / mul_base_batch / mul_base_clamped_batch
       (traits.rs:50-74, src/edwards.rs:1127-1243, src/ristretto.rs:1080-1115): resident tables of k points, constant-time
       s * P_{t_i} per item
+  VerifyingKeySet .verify_each / verify_prehashed_each / is_weak (ed25519-dalek/src/verifying.rs:167-257, :359-459): k
+      VerifyingKeys decompressed and tabulated once on the GPU, each signature verified under its key index
 """
 from .engine import (Engine, MultiEngine, EngineError, EdwardsPoint, RistrettoPoint, MontgomeryPoint, Scalar, SignatureError, verify_batch, default_engine,
                      library_path, load_library, POINTS_COMPRESSED, POINTS_EXTENDED, POINTS_RISTRETTO, POINTS_MONTGOMERY,
                      VartimeEdwardsPrecomputation, VartimeRistrettoPrecomputation, x25519, x25519_public_keys,
                      X25519_BASEPOINT_BYTES, ed25519_verifying_keys, ed25519_sign, ed25519_sign_prehashed,
-                     ed25519_verify_prehashed, ed25519_to_montgomery, EdwardsBasepointTable, RistrettoBasepointTable)
+                     ed25519_verify_prehashed, ed25519_to_montgomery, EdwardsBasepointTable, RistrettoBasepointTable,
+                     VerifyingKeySet)
 
 __all__ = ["Engine", "MultiEngine", "EngineError", "EdwardsPoint", "RistrettoPoint", "MontgomeryPoint", "Scalar", "SignatureError", "verify_batch", "default_engine",
            "library_path", "load_library", "POINTS_COMPRESSED", "POINTS_EXTENDED", "POINTS_RISTRETTO", "POINTS_MONTGOMERY",
            "VartimeEdwardsPrecomputation", "VartimeRistrettoPrecomputation", "x25519", "x25519_public_keys",
            "X25519_BASEPOINT_BYTES", "ed25519_verifying_keys", "ed25519_sign", "ed25519_sign_prehashed",
-           "ed25519_verify_prehashed", "ed25519_to_montgomery", "EdwardsBasepointTable", "RistrettoBasepointTable"]
+           "ed25519_verify_prehashed", "ed25519_to_montgomery", "EdwardsBasepointTable", "RistrettoBasepointTable",
+           "VerifyingKeySet"]

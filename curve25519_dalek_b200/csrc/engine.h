@@ -137,12 +137,15 @@ enum WsRole {
     WS_BATCH_TORSION,
     // batch.cu, single.cu [call] one status byte per batch (verify_batches) or per signature (verify_each)
     WS_ITEM_STATUS,
-    // single.cu [call] per-key comb tables of verify_each: the 16^i A powers of each key
+    // single.cu [call] per-key comb tables of verify_each and of a verifying-key set's build: the 16^i A powers of each key
     WS_EACH_POW,
     // single.cu [call] per-key comb tables of verify_each: the tables
     WS_EACH_TABLES,
     // single.cu [call] per-key comb tables of verify_each: each key's status
     WS_EACH_KEY_STATUS,
+    // single.cu [call] a verifying-key set call: the bad-index status word, then per signature h_i, the checked key index
+    // and the non-canonical-s mark
+    WS_KEY_SET_FRONT,
     WS_COUNT
 };
 

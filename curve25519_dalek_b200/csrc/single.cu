@@ -19,6 +19,7 @@
 // warp on the same schedule.  Same group element, hence the same encoding.
 #include <algorithm>
 #include <cstring>
+#include <new>
 
 #include "../../include/dalek_b200.h"
 #include "double_base.cuh"
@@ -461,6 +462,288 @@ int ed25519_b200_verify_prehashed_each(dalek_b200_ctx *ctx, const uint8_t *preha
     CUDA_TRY(ctx, cudaMemcpyAsync(d_sigs, sigs, n * 64, cudaMemcpyHostToDevice, st));
     CUDA_TRY(ctx, cudaMemcpyAsync(d_keys, pubkeys, n * 32, cudaMemcpyHostToDevice, st));
     return verify_each_resident(ctx, d_ph, nullptr, (const uint32_t *)d_sigs, (const uint32_t *)d_keys, n, strict, &dom, results);
+}
+
+}  // extern "C"
+
+// ---- resident verifying-key sets ----------------------------------------------------------------------------------------
+// A validator set, a service's known signers or a log's issuers are known before their signatures arrive.  A set
+// decompresses and tabulates its k keys once (the per-key comb tables above, built by the same two kernels), keeps the 32
+// bytes of each key as given (the challenge hashes VerifyingKey.compressed, the caller's encoding) and then verifies any
+// number of calls through k_verify_each_comb, unchanged: a call hashes each signature under its key (k_key_set_front)
+// and needs no key de-duplication, no table build and no host synchronisation before the comb kernel.
+#define KEY_SET_BUILD_GROUP 4096        // keys per build pass: their 16^i A powers (WS_EACH_POW) stay at 40 MiB
+
+struct ed25519_b200_key_set {
+    dalek_b200_ctx *ctx;   // the context it serves; destroy does not touch it
+    int device;
+    size_t k;
+    double *d_tab;         // k x EACH_KEY_DOUBLES: the comb tables k_verify_each_comb reads
+    uint32_t *d_keys;      // k x 32 B as given, then k slot indices 0..k-1 (the `dense` map), then k status bytes
+    uint32_t *d_slots;
+    uint8_t *d_kstat;      // bit 0: the key did not decode, bit 1: small order (k_each_key_pow16)
+};
+
+// The workspace of a set call (WS_KEY_SET_FRONT): a status word (an index >= k was seen), then per signature h_i
+// (32 B), the checked key index and the non-canonical-s mark.
+struct KeySetFront { int *bad_idx; uint32_t *hs, *idx; uint8_t *bad_s; };
+
+static int key_set_front_reserve(dalek_b200_ctx *ctx, size_t n, KeySetFront &f)
+{
+    int rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_KEY_SET_FRONT], 16 + n * 37))) return rc;
+    char *p = (char *)ctx->ws[WS_KEY_SET_FRONT].p;
+    f.bad_idx = (int *)p; f.hs = (uint32_t *)(p + 16); f.idx = f.hs + 8 * n; f.bad_s = (uint8_t *)(f.idx + n);
+    CUDA_TRY(ctx, cudaMemsetAsync(f.bad_idx, 0, 4, ctx->stream));
+    return 0;
+}
+
+// one thread per signature: the key index checked (an index >= k reads key 0 and sets *bad_idx), k = SHA-512(R || A ||
+// M) mod l with A the set's stored bytes (PH = 1: SHA-512(dom2 || R || A || PH), prehash i at msgs + 64 i, offs unused;
+// verifying.rs:515-535), and the canonical-s mark (signature.rs:89-94) -- what k_verify_each_comb reads
+template <int PH>
+__global__ void __launch_bounds__(128)
+k_key_set_front(const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ offs, const __grid_constant__ Sha512Prefix dom,
+                const uint32_t *__restrict__ sigs, const uint32_t *__restrict__ key_idx, size_t n, const uint32_t *__restrict__ keys,
+                uint32_t k, uint32_t *__restrict__ hs, uint32_t *__restrict__ idx, uint8_t *__restrict__ bad_s, int *__restrict__ bad_idx)
+{
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t t = key_idx ? key_idx[i] : 0;
+    if (t >= k) { t = 0; atomicOr(bad_idx, 1); }
+    uint32_t R[8], s[8], A[8];
+#pragma unroll
+    for (int w = 0; w < 8; w++) { R[w] = sigs[16 * i + w]; s[w] = sigs[16 * i + 8 + w]; A[w] = keys[8 * (size_t)t + w]; }
+    uint32_t dig[16], h[8];
+    if (PH) sha512_pxm<2, 1>(dig, dom.b, dom.len, R, A, msgs + 64 * i, 64);
+    else sha512_ram(dig, R, A, msgs + offs[i], (size_t)(offs[i + 1] - offs[i]));
+    sc_reduce512(h, dig);
+#pragma unroll
+    for (int w = 0; w < 8; w++) hs[8 * i + w] = h[w];
+    idx[i] = t;
+    bad_s[i] = (uint8_t)!sc_is_canonical(s);
+}
+
+static int key_set_check(dalek_b200_ctx *ctx, const ed25519_b200_key_set *s)
+{
+    if (!ctx || !s) return DALEK_E_INVALID_ARG;
+    if (s->ctx != ctx) { ctx->last_error = "verifying-key set used with a context other than its own"; return DALEK_E_INVALID_ARG; }
+    return 0;
+}
+
+// the comb kernel's shared-memory limit (once per context) and the table of B
+static int key_set_prepare(dalek_b200_ctx *ctx)
+{
+    int rc;
+    if ((rc = base_table_ensure(ctx))) return rc;
+    if (!ctx->each_attr_set) {
+        CUDA_TRY(ctx, cudaFuncSetAttribute(k_verify_each_comb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EACH_COMB_SMEM));
+        ctx->each_attr_set = true;
+    }
+    return 0;
+}
+
+// front + comb over m signatures (device inputs of this piece; the front arrays at f, item lo of the batch)
+static void key_set_launch(const ed25519_b200_key_set *s, const uint8_t *d_msgs, const uint64_t *d_offs, const Sha512Prefix *ph_dom,
+                           const uint32_t *d_sigs, const uint32_t *d_idx, size_t m, int strict, const KeySetFront &f, size_t lo,
+                           const ge_niels_packed *base, uint8_t *d_out, cudaStream_t st)
+{
+    uint32_t *hs = f.hs + 8 * lo, *idx = f.idx + lo;
+    uint8_t *bad_s = f.bad_s + lo;
+    if (ph_dom)
+        k_key_set_front<1><<<cdiv(m, 128), 128, 0, st>>>(d_msgs, nullptr, *ph_dom, d_sigs, d_idx, m, s->d_keys, (uint32_t)s->k, hs, idx,
+                                                          bad_s, f.bad_idx);
+    else
+        k_key_set_front<0><<<cdiv(m, 128), 128, 0, st>>>(d_msgs, d_offs, Sha512Prefix{}, d_sigs, d_idx, m, s->d_keys, (uint32_t)s->k, hs,
+                                                          idx, bad_s, f.bad_idx);
+    k_verify_each_comb<<<cdiv((m + EACH_K - 1) / EACH_K, 128), 128, EACH_COMB_SMEM, st>>>(d_sigs, hs, bad_s, idx, s->d_slots, s->d_kstat,
+                                                                                         s->d_tab, base, 0, m, strict, d_out);
+}
+
+// a whole batch whose inputs are in device memory (the _dev call, and the staged Ed25519ph call): both kernels, then
+// the results and the index status read back
+static int key_set_resident(dalek_b200_ctx *ctx, const ed25519_b200_key_set *s, const uint8_t *d_msgs, const uint64_t *d_offs,
+                            const Sha512Prefix *ph_dom, const uint32_t *d_sigs, const uint32_t *d_idx, size_t n, int strict,
+                            uint8_t *results)
+{
+    int rc;
+    KeySetFront f;
+    if ((rc = key_set_prepare(ctx))) return rc;
+    if ((rc = key_set_front_reserve(ctx, n, f))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_ITEM_STATUS], n))) return rc;
+    if ((rc = pinned_reserve(ctx, 64))) return rc;
+    uint8_t *d_out = (uint8_t *)ctx->ws[WS_ITEM_STATUS].p;
+    cudaStream_t st = ctx->stream;
+    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, st));
+    key_set_launch(s, d_msgs, d_offs, ph_dom, d_sigs, d_idx, n, strict, f, 0, (const ge_niels_packed *)ctx->ws[WS_BASE_TABLE].p, d_out, st);
+    ctx->launches += 2;
+    CUDA_TRY(ctx, cudaGetLastError());
+    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(results, d_out, n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_pinned, f.bad_idx, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaStreamSynchronize(st));
+    float ms = 0.f;
+    if ((ms = elapsed_ms(ctx->ev_a, ctx->ev_b)) >= 0.f) ctx->last_kernel_ms = ms;
+    ctx->last_kernel_launches = 2;
+    if (*(const int *)ctx->h_pinned) { ctx->last_error = "key index >= len()"; return DALEK_E_INVALID_ARG; }
+    return verify_each_summary(results, n);
+}
+
+static bool key_indices_ok(dalek_b200_ctx *ctx, const ed25519_b200_key_set *s, const uint32_t *key_idx, size_t n)
+{
+    if (key_idx)                                                   // public: checked before any device work
+        for (size_t i = 0; i < n; i++)
+            if (key_idx[i] >= s->k) { ctx->last_error = "key index >= len()"; return false; }
+    return true;
+}
+
+static void key_set_free(ed25519_b200_key_set *s)
+{
+    cudaFree(s->d_tab);                                            // waits for the device: no call still reads the set
+    cudaFree(s->d_keys);
+    delete s;
+}
+
+extern "C" {
+
+int ed25519_b200_key_set_new(dalek_b200_ctx *ctx, const uint8_t *pubkeys, size_t k, uint8_t *ok, uint8_t *weak,
+                             ed25519_b200_key_set **out)
+{
+    if (!ctx || !out) return DALEK_E_INVALID_ARG;
+    *out = nullptr;
+    if (!pubkeys || !k || k > 0xffffffffull) return DALEK_E_INVALID_ARG;
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    CallTimer timer(ctx);
+    int rc;
+    const size_t group = std::min<size_t>(k, KEY_SET_BUILD_GROUP);
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_EACH_POW], group * 64 * sizeof(ge_p3_raw)))) return rc;
+    ed25519_b200_key_set *s = new (std::nothrow) ed25519_b200_key_set();
+    uint32_t *slots = new (std::nothrow) uint32_t[k];
+    uint8_t *kstat = new (std::nothrow) uint8_t[k];
+    auto fail = [&](int code) {
+        if (s) key_set_free(s);
+        delete[] slots; delete[] kstat;
+        return code;
+    };
+    if (!s || !slots || !kstat) { ctx->last_error = "out of host memory for the verifying-key set"; return fail(DALEK_E_NOMEM); }
+    s->ctx = ctx; s->device = ctx->device; s->k = k;
+    if (cudaMalloc((void **)&s->d_tab, k * EACH_KEY_DOUBLES * sizeof(double)) != cudaSuccess ||
+        cudaMalloc((void **)&s->d_keys, k * (32 + 4 + 1)) != cudaSuccess) {
+        (void)cudaGetLastError();
+        ctx->last_error = "cudaMalloc failed for the verifying-key set";
+        return fail(DALEK_E_NOMEM);
+    }
+    s->d_slots = s->d_keys + 8 * k;
+    s->d_kstat = (uint8_t *)(s->d_slots + k);
+    for (size_t i = 0; i < k; i++) slots[i] = (uint32_t)i;
+    cudaStream_t st = ctx->stream;
+    ge_p3_raw *pw = (ge_p3_raw *)ctx->ws[WS_EACH_POW].p;
+    bool cuda_ok = cudaEventRecord(ctx->ev_a, st) == cudaSuccess &&
+                   cudaMemcpyAsync(s->d_keys, pubkeys, k * 32, cudaMemcpyHostToDevice, st) == cudaSuccess &&
+                   cudaMemcpyAsync(s->d_slots, slots, k * 4, cudaMemcpyHostToDevice, st) == cudaSuccess;
+    for (size_t o = 0; cuda_ok && o < k; o += group) {             // uniq = slots 0..m-1 over the keys from o
+        const size_t m = std::min(group, k - o);
+        k_each_key_pow16<<<cdiv(m, 64), 64, 0, st>>>(s->d_keys + 8 * o, s->d_slots, m, pw, s->d_kstat + o);
+        k_each_key_rows<<<cdiv(m * 512, 128), 128, 0, st>>>(pw, m, s->d_tab + o * EACH_KEY_DOUBLES);
+        ctx->launches += 2;
+        cuda_ok = cudaGetLastError() == cudaSuccess;
+    }
+    cuda_ok = cuda_ok && cudaEventRecord(ctx->ev_b, st) == cudaSuccess &&
+              cudaMemcpyAsync(kstat, s->d_kstat, k, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+              cudaStreamSynchronize(st) == cudaSuccess;
+    if (!cuda_ok) {
+        ctx->last_error = std::string("verifying-key set build: ") + cudaGetErrorString(cudaGetLastError());
+        return fail(DALEK_E_CUDA);
+    }
+    float ms = 0.f;
+    if ((ms = elapsed_ms(ctx->ev_a, ctx->ev_b)) >= 0.f) ctx->last_kernel_ms = ms;
+    ctx->last_kernel_launches = (int)(2 * ((k + group - 1) / group));
+    bool all_ok = true;
+    for (size_t i = 0; i < k; i++) {
+        const bool good = !(kstat[i] & 1);
+        all_ok &= good;
+        if (ok) ok[i] = good;
+        if (weak) weak[i] = good && (kstat[i] & 2);                // VerifyingKey::is_weak (verifying.rs:192-194)
+    }
+    if (!all_ok) { ctx->last_error = "a verifying key does not decode"; return fail(ED25519_ERR_POINT_DECOMPRESSION); }
+    delete[] slots; delete[] kstat;
+    *out = s;
+    return DALEK_OK;
+}
+
+size_t ed25519_b200_key_set_len(const ed25519_b200_key_set *s) { return s ? s->k : 0; }
+
+void ed25519_b200_key_set_destroy(ed25519_b200_key_set *s)
+{
+    if (!s) return;
+    cudaSetDevice(s->device);
+    key_set_free(s);
+}
+
+int ed25519_b200_key_set_verify_flat(dalek_b200_ctx *ctx, const ed25519_b200_key_set *s, const uint8_t *msgs_flat,
+                                     const uint64_t *msg_offsets, const uint8_t *sigs, const uint32_t *key_idx, size_t n,
+                                     int strict, uint8_t *results)
+{
+    int rc;
+    if ((rc = key_set_check(ctx, s))) return rc;
+    if ((n && (!sigs || !results)) || !flat_messages_ok(msgs_flat, msg_offsets, n)) return DALEK_E_INVALID_ARG;
+    if (!key_indices_ok(ctx, s, key_idx, n)) return DALEK_E_INVALID_ARG;
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    if (!n) return DALEK_OK;
+    CallTimer timer(ctx);
+    KeySetFront f;
+    if ((rc = key_set_prepare(ctx))) return rc;
+    if ((rc = key_set_front_reserve(ctx, n, f))) return rc;
+    const ge_niels_packed *base = (const ge_niels_packed *)ctx->ws[WS_BASE_TABLE].p;
+    // independent per signature: pieces alternate between two streams (copy-in -> front + comb -> copy-out)
+    rc = run_pieces(ctx, msgs_flat, msg_offsets, sigs, 64, (const uint8_t *)key_idx, key_idx ? 4 : 0, results, 1, nullptr, 0, n,
+                    [&](const uint8_t *d_msgs, const uint64_t *d_offs, const uint8_t *d_sigs, const uint8_t *d_idx, size_t m,
+                        uint8_t *d_out, uint8_t *, cudaStream_t st, size_t lo) {
+                        key_set_launch(s, d_msgs, d_offs, nullptr, (const uint32_t *)d_sigs, key_idx ? (const uint32_t *)d_idx : nullptr,
+                                       m, strict, f, lo, base, d_out, st);
+                        ctx->launches++;                           // run_pieces counts one launch per piece
+                        return 0;
+                    });
+    return rc ? rc : verify_each_summary(results, n);
+}
+
+int ed25519_b200_key_set_verify_flat_dev(dalek_b200_ctx *ctx, const ed25519_b200_key_set *s, const void *d_msgs_flat,
+                                         const void *d_msg_offsets, const void *d_sigs, const void *d_key_idx, size_t n, int strict,
+                                         uint8_t *results)
+{
+    int rc;
+    if ((rc = key_set_check(ctx, s))) return rc;
+    if (n && (!d_msg_offsets || !d_sigs || !results)) return DALEK_E_INVALID_ARG;
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    if (!n) return DALEK_OK;
+    CallTimer timer(ctx);
+    return key_set_resident(ctx, s, (const uint8_t *)d_msgs_flat, (const uint64_t *)d_msg_offsets, nullptr, (const uint32_t *)d_sigs,
+                            (const uint32_t *)d_key_idx, n, strict, results);
+}
+
+// the three inputs have fixed widths, so they cross PCIe whole, as in verify_prehashed_each
+int ed25519_b200_key_set_verify_prehashed(dalek_b200_ctx *ctx, const ed25519_b200_key_set *s, const uint8_t *prehashes,
+                                          const uint8_t *context, size_t context_len, const uint8_t *sigs, const uint32_t *key_idx,
+                                          size_t n, int strict, uint8_t *results)
+{
+    int rc;
+    if ((rc = key_set_check(ctx, s))) return rc;
+    if ((n && (!prehashes || !sigs || !results)) || (context_len && !context) || context_len > 255) return DALEK_E_INVALID_ARG;
+    if (!key_indices_ok(ctx, s, key_idx, n)) return DALEK_E_INVALID_ARG;
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    if (!n) return DALEK_OK;
+    CallTimer timer(ctx);
+    Sha512Prefix dom;
+    ed25519ph_dom2(dom, context, context_len);
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_MSGS], n * 64))) return rc;
+    if ((rc = ws_reserve(ctx, ctx->ws[WS_STAGING_IN], n * 68))) return rc;
+    uint8_t *d_ph = (uint8_t *)ctx->ws[WS_STAGING_MSGS].p, *d_sigs = (uint8_t *)ctx->ws[WS_STAGING_IN].p, *d_idx = d_sigs + n * 64;
+    cudaStream_t st = ctx->stream;
+    CUDA_TRY(ctx, cudaMemcpyAsync(d_ph, prehashes, n * 64, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(d_sigs, sigs, n * 64, cudaMemcpyHostToDevice, st));
+    if (key_idx) CUDA_TRY(ctx, cudaMemcpyAsync(d_idx, key_idx, n * 4, cudaMemcpyHostToDevice, st));
+    return key_set_resident(ctx, s, d_ph, nullptr, &dom, (const uint32_t *)d_sigs, key_idx ? (const uint32_t *)d_idx : nullptr, n,
+                            strict, results);
 }
 
 }  // extern "C"

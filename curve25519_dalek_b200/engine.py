@@ -109,6 +109,14 @@ def load_library():
     lib.ed25519_b200_sign_flat.argtypes = [vp, vp, sz, vp, vp, sz, vp]
     lib.ed25519_b200_sign_prehashed.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp]
     lib.ed25519_b200_verify_prehashed_each.argtypes = [vp, vp, vp, sz, vp, vp, sz, C.c_int, vp]
+    lib.ed25519_b200_key_set_new.argtypes = [vp, vp, sz, vp, vp, C.POINTER(vp)]
+    lib.ed25519_b200_key_set_len.argtypes = [vp]
+    lib.ed25519_b200_key_set_len.restype = sz
+    lib.ed25519_b200_key_set_destroy.argtypes = [vp]
+    lib.ed25519_b200_key_set_destroy.restype = None
+    lib.ed25519_b200_key_set_verify_flat.argtypes = [vp, vp, vp, vp, vp, vp, sz, C.c_int, vp]
+    lib.ed25519_b200_key_set_verify_flat_dev.argtypes = [vp, vp, vp, vp, vp, vp, sz, C.c_int, vp]
+    lib.ed25519_b200_key_set_verify_prehashed.argtypes = [vp, vp, vp, vp, sz, vp, vp, sz, C.c_int, vp]
     lib.dalek_b200_edwards_to_montgomery_batch.argtypes = [vp, vp, sz, vp]
     lib.dalek_b200_x25519_batch.argtypes = [vp, vp, vp, sz, vp, vp]
     lib.dalek_b200_x25519_batch_dev.argtypes = [vp, vp, vp, sz, vp, vp]
@@ -826,6 +834,40 @@ class Engine:
         rc = self._check(self.lib.ed25519_b200_verify_prehashed_each(self.h, _ptr(prehashes), _ptr(ctx) if ctx else None, len(ctx),
                                                                      _ptr(sigs), _ptr(pubkeys), n, 1 if strict else 0,
                                                                      C.addressof(res)))
+        return rc, list(res)[:n]
+
+    # ---- resident verifying-key sets ----
+    def key_set_new(self, pubkeys, k):
+        """ed25519_b200_key_set_new for k 32-byte keys: (rc, handle or None, ok, weak); rc 4 (PointDecompression) when a
+        key does not decode (its ok byte is 0, and no handle is made)."""
+        h = C.c_void_p()
+        ok, weak = (C.c_uint8 * max(k, 1))(), (C.c_uint8 * max(k, 1))()
+        rc = self._check(self.lib.ed25519_b200_key_set_new(self.h, _ptr(pubkeys), k, C.addressof(ok), C.addressof(weak), C.byref(h)))
+        return rc, (h if h.value else None), bytes(ok)[:k], bytes(weak)[:k]
+
+    def key_set_len(self, handle):
+        return int(self.lib.ed25519_b200_key_set_len(handle))
+
+    def key_set_destroy(self, handle):
+        self.lib.ed25519_b200_key_set_destroy(handle)
+
+    def key_set_verify_flat(self, handle, msgs_flat, offsets, sigs, indices, n, strict=False, device_ptrs=False):
+        """verify (or verify_strict) of signature i under key indices[i] of the set (n uint32, or None for key 0):
+        (rc, results) as in verify_each_flat.  With device_ptrs every input is a device buffer."""
+        res = (C.c_uint8 * max(n, 1))()
+        fn = self.lib.ed25519_b200_key_set_verify_flat_dev if device_ptrs else self.lib.ed25519_b200_key_set_verify_flat
+        rc = self._check(fn(self.h, handle, _ptr(msgs_flat), _ptr(offsets), _ptr(sigs), _ptr(indices), n, 1 if strict else 0,
+                            C.addressof(res)))
+        return rc, list(res)[:n]
+
+    def key_set_verify_prehashed(self, handle, prehashes, sigs, indices, n, context=None, strict=False):
+        """verify_prehashed (or verify_prehashed_strict) of signature i under key indices[i] of the set: (rc, results) as
+        in verify_prehashed_each."""
+        res = (C.c_uint8 * max(n, 1))()
+        ctx = bytes(context) if context is not None else b""
+        rc = self._check(self.lib.ed25519_b200_key_set_verify_prehashed(self.h, handle, _ptr(prehashes), _ptr(ctx) if ctx else None,
+                                                                        len(ctx), _ptr(sigs), _ptr(indices), n,
+                                                                        1 if strict else 0, C.addressof(res)))
         return rc, list(res)[:n]
 
     def sign_batch_flat(self, seeds, msgs_flat, offsets, n):
@@ -1755,6 +1797,84 @@ class EdwardsBasepointTable(_BasepointTable):
 class RistrettoBasepointTable(_BasepointTable):
     """RistrettoBasepointTable (ristretto.rs:1080-1115): CompressedRistretto in and out."""
     _FMT = POINTS_RISTRETTO
+
+
+class VerifyingKeySet:
+    """k VerifyingKeys (VerifyingKey::from_bytes, verifying.rs:167-175) resident on the GPU: each key is decompressed and
+    tabulated once, and every later call sends messages, signatures and key indices only."""
+
+    def __init__(self, verifying_keys, engine=None):
+        """verifying_keys = iterable of 32-byte encodings, kept as given (the challenge hashes them).  A key that does not
+        decode raises SignatureError (PointDecompression) naming the first one."""
+        self.h = None
+        self.eng = engine or default_engine()
+        _, keys = _items(list(verifying_keys), 32, "verifying keys")
+        if not keys:
+            raise ValueError("a verifying-key set needs at least one key")
+        rc, h, ok, weak = self.eng.key_set_new(b"".join(keys), len(keys))
+        if rc:
+            err = SignatureError(rc)
+            err.args = ("%s: verifying key %d does not decode" % (err.kind, ok.index(0)),)
+            raise err
+        self.h, self.k, self._weak = h, len(keys), weak
+
+    def __len__(self):
+        return self.k
+
+    def is_weak(self, i=0):
+        """VerifyingKey::is_weak (verifying.rs:192-194) of key i: a key of small order."""
+        if not 0 <= i < self.k:
+            raise IndexError("key index out of range")
+        return bool(self._weak[i])
+
+    def _indices(self, indices, n):
+        if indices is None:
+            return None
+        import array
+        idx = array.array("I", indices)
+        if len(idx) != n:
+            raise ValueError("one key index per signature")
+        if n and max(idx) >= self.k:
+            raise ValueError("a key index is not below len()")
+        return idx.tobytes()
+
+    def verify_each(self, messages, signatures, indices=None, strict=False):
+        """VerifyingKey::verify / verify_strict (verifying.rs:203-219, :359-382) of signature i over message i under key
+        indices[i] (None: key 0): the list of result codes (0 Ok, 1 Verify, 3 ScalarFormat), or one code for a single
+        message."""
+        single = isinstance(messages, (bytes, bytearray))
+        msgs = [bytes(messages)] if single else [bytes(m) for m in messages]
+        _, sigs = _items([signatures] if single else signatures, 64, "signatures")
+        if len(sigs) != len(msgs):
+            raise ValueError("messages and signatures must have the same length")
+        idx = self._indices([indices] if single and indices is not None else indices, len(msgs))
+        flat, offs, n = _flat_messages(msgs)
+        _, res = self.eng.key_set_verify_flat(self.h, flat, offs, b"".join(sigs), idx, n, strict)
+        return res[0] if single else res
+
+    def verify_prehashed_each(self, prehashed, signatures, indices=None, context=None, strict=False):
+        """VerifyingKey::verify_prehashed / verify_prehashed_strict (verifying.rs:230-257, :424-459) of each signature
+        under key indices[i], as ed25519_verify_prehashed.  A context longer than 255 bytes raises ValueError."""
+        single, phs = _prehash_items(prehashed)
+        _, sigs = _items([signatures] if single else signatures, 64, "signatures")
+        if len(sigs) != len(phs):
+            raise ValueError("prehashes and signatures must have the same length")
+        if context is not None and len(bytes(context)) > 255:
+            raise ValueError("an Ed25519ph context is at most 255 bytes")
+        idx = self._indices([indices] if single and indices is not None else indices, len(phs))
+        _, res = self.eng.key_set_verify_prehashed(self.h, b"".join(phs), b"".join(sigs), idx, len(phs), context, strict)
+        return res[0] if single else res
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.eng.key_set_destroy(self.h)                   # does not use the engine's context: safe after its close()
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class RistrettoPoint(_GroupOps):

@@ -93,7 +93,8 @@ int dalek_b200_last_stage_ms(const dalek_b200_ctx *ctx, const char *stage, float
  * precomputed-MSM / X25519 / to_montgomery_batch / hash-to-group / Lizard / map_to_curve / map_to_curve_inverse / mul_batch
  * / vartime_double_base_batch / MontgomeryPoint / mul_base_ct_batch / scalar_binary_batch / scalar_unary_batch /
  * scalar_from_bytes_batch / scalar_hash_from_bytes_batch / scalar_fold_batch call, or of the last ed25519_b200_verifying_keys /
- * sign_flat / sign_prehashed / verify_prehashed_each call, and after the last work it enqueued (all of the call's streams
+ * sign_flat / sign_prehashed / verify_prehashed_each / key_set_new / key_set_verify_flat / key_set_verify_flat_dev /
+ * key_set_verify_prehashed call, and after the last work it enqueued (all of the call's streams
  * joined): the device time of that call, copies of host-buffer calls included. */
 int dalek_b200_last_call_ms(const dalek_b200_ctx *ctx, float *ms);
 
@@ -723,6 +724,53 @@ int ed25519_b200_sign_prehashed(dalek_b200_ctx *ctx, const uint8_t *seeds, size_
 int ed25519_b200_verify_prehashed_each(dalek_b200_ctx *ctx, const uint8_t *prehashes, const uint8_t *context,
                                        size_t context_len, const uint8_t *sigs, const uint8_t *pubkeys, size_t n,
                                        int strict, uint8_t *results);
+
+/* -------- resident verifying-key sets -----------------------------------------------------------------------------------
+ * A VerifyingKey is decompressed once by VerifyingKey::from_bytes (E/verifying.rs:167-175) and then verifies any number of
+ * messages.  A set holds k keys in device memory: the 32 bytes of each key exactly as given (the challenge k = SHA-512(R ||
+ * A || M) hashes VerifyingKey.compressed, E/verifying.rs:515-523, so a non-canonical encoding is hashed as the caller
+ * wrote it), the 64 x 8 multiples (j+1) 16^i A of each key as FP64 affine Niels (64 KiB per key, the per-key comb tables
+ * of ed25519_b200_verify_each_flat), a status byte and a 4-byte slot index per key.  new allocates that memory and
+ * destroy frees it; the set is not a context workspace and serves only the context that made it (another context is
+ * DALEK_E_INVALID_ARG).
+ *
+ * new is VerifyingKey::from_bytes once per key, for k >= 1 keys (k = 0 is DALEK_E_INVALID_ARG).  If a key does not
+ * decode, ok[i] = 0 for it (ok: k bytes, nullable; 1 for every other key), *out stays NULL, nothing stays allocated and
+ * the call returns ED25519_ERR_POINT_DECOMPRESSION.  weak[i] (k bytes, nullable) is VerifyingKey::is_weak
+ * (E/verifying.rs:192-194), i.e. EdwardsPoint::is_small_order (C/edwards.rs:1405-1407) of the decoded key, and 0 for a
+ * key that does not decode.  A failed allocation returns DALEK_E_NOMEM with last_error set and no set. */
+typedef struct ed25519_b200_key_set ed25519_b200_key_set;
+int ed25519_b200_key_set_new(dalek_b200_ctx *ctx, const uint8_t *pubkeys /* k x 32 B */, size_t k,
+                             uint8_t *ok /* k, nullable */, uint8_t *weak /* k, nullable */, ed25519_b200_key_set **out);
+size_t ed25519_b200_key_set_len(const ed25519_b200_key_set *s);
+/* destroy waits for the device and frees the set; it does not use the context, so a set may be destroyed before or
+ * after its context.  NULL is a no-op. */
+void ed25519_b200_key_set_destroy(ed25519_b200_key_set *s);
+/* verify (strict = 0, E/verifying.rs:203-219) or verify_strict (strict = 1, E/verifying.rs:359-382) of signature i
+ * under key key_idx[i] of the set (key_idx NULL: key 0 for every signature).  results and return value are exactly those
+ * of ed25519_b200_verify_each_flat on the same inputs with the key bytes inlined, with the same error precedence: 0 Ok,
+ * 1 Verify, 3 ScalarFormat (PointDecompression cannot occur: every key of a set decodes).  verify_strict rejects every
+ * signature under a weak key.  The set's tables always serve the call (option "each_comb" does not apply); each signature
+ * costs 128 mixed additions and no doubling, with no per-call table build, key de-duplication or host synchronisation.
+ * n = 0 is a successful no-op; a NULL sigs or results with n > 0 is DALEK_E_INVALID_ARG; flat messages as in the
+ * hash-to-group block.  Host buffers: an index >= k is DALEK_E_INVALID_ARG before any device work, and the batch is
+ * streamed in pieces. */
+int ed25519_b200_key_set_verify_flat(dalek_b200_ctx *ctx, const ed25519_b200_key_set *s, const uint8_t *msgs_flat,
+                                     const uint64_t *msg_offsets, const uint8_t *sigs, const uint32_t *key_idx /* n, or NULL */,
+                                     size_t n, int strict, uint8_t *results /* n */);
+/* same with messages, offsets, signatures and indices in device memory; results in host memory; blocks until done.  An
+ * index >= k is never used as an address (key 0 is read in its place) and is reported after the batch ran: the call
+ * returns DALEK_E_INVALID_ARG and the results are unspecified. */
+int ed25519_b200_key_set_verify_flat_dev(dalek_b200_ctx *ctx, const ed25519_b200_key_set *s, const void *d_msgs_flat,
+                                         const void *d_msg_offsets, const void *d_sigs, const void *d_key_idx, size_t n,
+                                         int strict, uint8_t *results /* host */);
+/* verify_prehashed (strict = 0) / verify_prehashed_strict (strict = 1) (E/verifying.rs:230-257, :424-459) of signature i
+ * under key key_idx[i]: results and return value as ed25519_b200_verify_prehashed_each on the same inputs with the key
+ * bytes inlined.  prehashes: n x 64 B; one context of context_len <= 255 bytes (NULL only with context_len = 0), a longer
+ * one is DALEK_E_INVALID_ARG.  Other rules as ed25519_b200_key_set_verify_flat. */
+int ed25519_b200_key_set_verify_prehashed(dalek_b200_ctx *ctx, const ed25519_b200_key_set *s, const uint8_t *prehashes,
+                                          const uint8_t *context, size_t context_len, const uint8_t *sigs,
+                                          const uint32_t *key_idx /* n, or NULL */, size_t n, int strict, uint8_t *results);
 
 /* -------- input synthesis (benchmarks / tests): fixed-base multiples and keys + signatures ---- */
 /* out[i] = scalars[i] * B as extended limbs (EdwardsPoint::mul_base, C/edwards.rs:918-928).  Public scalars only:
