@@ -41,17 +41,24 @@ touches the CPU checker used by the tests.  Names follow the reference:
       s * P_{t_i} per item
   VerifyingKeySet .verify_each / verify_prehashed_each / is_weak (ed25519-dalek/src/verifying.rs:167-257, :359-459): k
       VerifyingKeys decompressed and tabulated once on the GPU, each signature verified under its key index
+  SigningKeySet .from_seeds / from_keypair_bytes / from_expanded / sign / sign_prehashed / verifying_keys
+      (ed25519-dalek/src/signing.rs:106, :140-150, :566-571, :312; hazmat.rs:84-99): k signing keys derived once on the
+      GPU, each message signed under its key index
+  ed25519_expanded_verifying_keys / ed25519_raw_sign / ed25519_raw_sign_prehashed (ed25519-dalek/src/hazmat.rs:84-99,
+      :137, :182; verifying.rs:97-102): signing from ExpandedSecretKey bytes
 """
 from .engine import (Engine, MultiEngine, EngineError, EdwardsPoint, RistrettoPoint, MontgomeryPoint, Scalar, SignatureError, verify_batch, default_engine,
                      library_path, load_library, POINTS_COMPRESSED, POINTS_EXTENDED, POINTS_RISTRETTO, POINTS_MONTGOMERY,
                      VartimeEdwardsPrecomputation, VartimeRistrettoPrecomputation, x25519, x25519_public_keys,
                      X25519_BASEPOINT_BYTES, ed25519_verifying_keys, ed25519_sign, ed25519_sign_prehashed,
                      ed25519_verify_prehashed, ed25519_to_montgomery, EdwardsBasepointTable, RistrettoBasepointTable,
-                     VerifyingKeySet)
+                     VerifyingKeySet, SigningKeySet, ed25519_expanded_verifying_keys, ed25519_raw_sign,
+                     ed25519_raw_sign_prehashed)
 
 __all__ = ["Engine", "MultiEngine", "EngineError", "EdwardsPoint", "RistrettoPoint", "MontgomeryPoint", "Scalar", "SignatureError", "verify_batch", "default_engine",
            "library_path", "load_library", "POINTS_COMPRESSED", "POINTS_EXTENDED", "POINTS_RISTRETTO", "POINTS_MONTGOMERY",
            "VartimeEdwardsPrecomputation", "VartimeRistrettoPrecomputation", "x25519", "x25519_public_keys",
            "X25519_BASEPOINT_BYTES", "ed25519_verifying_keys", "ed25519_sign", "ed25519_sign_prehashed",
            "ed25519_verify_prehashed", "ed25519_to_montgomery", "EdwardsBasepointTable", "RistrettoBasepointTable",
-           "VerifyingKeySet"]
+           "VerifyingKeySet", "SigningKeySet", "ed25519_expanded_verifying_keys", "ed25519_raw_sign",
+           "ed25519_raw_sign_prehashed"]

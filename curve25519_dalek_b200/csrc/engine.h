@@ -31,7 +31,7 @@ enum WsRole {
     WS_SCALARS,
     // pieces.h, api.cu, base.cu, batch.cu, lizard.cu, point_ops.cu, precomp.cu, scalars.cu, sign.cu, single.cu, straus.cu,
     // varmul.cu [call] fixed-width inputs staged from the host: MSM input points, signatures and keys, the inputs of
-    // run_pieces, the points of a segmented sum
+    // run_pieces, the points of a segmented sum, the secret keys a signing-key set is built from
     WS_STAGING_IN,
     // pieces.h, api.cu, batch.cu, lizard.cu, point_ops.cu, precomp.cu, scalars.cu, straus.cu, varmul.cu [call] outputs of
     // run_pieces and the prepared Niels points of an MSM (verify's MSM points)
@@ -42,8 +42,9 @@ enum WsRole {
     WS_STAGING_MSGS,
     // pieces.h, batch.cu, single.cu [call] the n + 1 message offsets of WS_STAGING_MSGS
     WS_MSG_OFFSETS,
-    // double_base.cu, lizard.cu, montgomery.cu, point_ops.cu, scalars.cu, straus.cu, varmul.cu [call] small per-call
-    // scratch: status words, broadcast operands and tables, the G/H tables of the Ristretto double-base batch
+    // double_base.cu, lizard.cu, montgomery.cu, point_ops.cu, scalars.cu, sign.cu, straus.cu, varmul.cu [call] small
+    // per-call scratch: status words (the bad-index word of a signing-key set call), broadcast operands and tables, the
+    // G/H tables of the Ristretto double-base batch
     WS_CALL_SCRATCH,
     // ---- tables built once per context ----
     // base.cu, double_base.cu, single.cu [context] 64 x 8 affine Niels entries (j+1) 16^i B (base_table_ensure)
@@ -113,10 +114,11 @@ enum WsRole {
     // msm.cu [call] the first stage of the reduction's plain sums
     WS_MSM_SUM_PART,
     // ---- verification (batch.cu) and the per-signature verifier (single.cu) ----
-    // batch.cu, sign.cu [call] SHA-512(R || A || M), 64 B per signature; in a sign call the signer's expanded keys
+    // batch.cu, sign.cu [call] SHA-512(R || A || M), 64 B per signature; in a sign call the signer's expanded keys (a
+    // hazmat call: the caller's ExpandedSecretKey bytes)
     WS_VERIFY_HRAM,
     // batch.cu, sign.cu [call] h_i (z_i h_i once merged), 32 B per signature, read by single.cu after verify_each_front;
-    // in a sign call the signer's verifying keys
+    // in a sign call the signer's verifying keys (a hazmat call: the caller's)
     WS_VERIFY_H,
     // batch.cu [call] z_i s_i
     WS_VERIFY_ZS_PROD,

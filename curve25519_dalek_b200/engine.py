@@ -117,6 +117,18 @@ def load_library():
     lib.ed25519_b200_key_set_verify_flat.argtypes = [vp, vp, vp, vp, vp, vp, sz, C.c_int, vp]
     lib.ed25519_b200_key_set_verify_flat_dev.argtypes = [vp, vp, vp, vp, vp, vp, sz, C.c_int, vp]
     lib.ed25519_b200_key_set_verify_prehashed.argtypes = [vp, vp, vp, vp, sz, vp, vp, sz, C.c_int, vp]
+    lib.ed25519_b200_expanded_verifying_keys.argtypes = [vp, vp, sz, vp]
+    lib.ed25519_b200_raw_sign_flat.argtypes = [vp, vp, vp, sz, vp, vp, sz, vp]
+    lib.ed25519_b200_raw_sign_prehashed.argtypes = [vp, vp, vp, sz, vp, sz, vp, sz, vp]
+    lib.ed25519_b200_signing_key_set_new.argtypes = [vp, vp, sz, C.c_int, vp, C.POINTER(vp)]
+    lib.ed25519_b200_signing_key_set_len.argtypes = [vp]
+    lib.ed25519_b200_signing_key_set_len.restype = sz
+    lib.ed25519_b200_signing_key_set_verifying_keys.argtypes = [vp, vp]
+    lib.ed25519_b200_signing_key_set_destroy.argtypes = [vp]
+    lib.ed25519_b200_signing_key_set_destroy.restype = None
+    lib.ed25519_b200_signing_key_set_sign_flat.argtypes = [vp, vp, vp, vp, vp, sz, vp]
+    lib.ed25519_b200_signing_key_set_sign_flat_dev.argtypes = [vp, vp, vp, vp, vp, sz, vp]
+    lib.ed25519_b200_signing_key_set_sign_prehashed.argtypes = [vp, vp, vp, vp, sz, vp, sz, vp]
     lib.dalek_b200_edwards_to_montgomery_batch.argtypes = [vp, vp, sz, vp]
     lib.dalek_b200_x25519_batch.argtypes = [vp, vp, vp, sz, vp, vp]
     lib.dalek_b200_x25519_batch_dev.argtypes = [vp, vp, vp, sz, vp, vp]
@@ -158,8 +170,9 @@ class EngineError(RuntimeError):
 
 class SignatureError(Exception):
     """ed25519_dalek::SignatureError (ed25519-dalek/src/errors.rs:23-53): `.kind` is one of
-    'Verify', 'ArrayLength', 'ScalarFormat', 'PointDecompression', 'PrehashedContextLength'."""
-    KINDS = {1: "Verify", 2: "ArrayLength", 3: "ScalarFormat", 4: "PointDecompression", 5: "PrehashedContextLength"}
+    'Verify', 'ArrayLength', 'ScalarFormat', 'PointDecompression', 'PrehashedContextLength', 'MismatchedKeypair'."""
+    KINDS = {1: "Verify", 2: "ArrayLength", 3: "ScalarFormat", 4: "PointDecompression", 5: "PrehashedContextLength",
+             6: "MismatchedKeypair"}
 
     def __init__(self, code):
         self.code = code
@@ -869,6 +882,73 @@ class Engine:
                                                                         len(ctx), _ptr(sigs), _ptr(indices), n,
                                                                         1 if strict else 0, C.addressof(res)))
         return rc, list(res)[:n]
+
+    # ---- hazmat signing from ExpandedSecretKey bytes ----
+    def expanded_verifying_keys(self, esks, n):
+        """VerifyingKey::from(&ExpandedSecretKey::from_bytes(esk)) for n 64-byte esks -> n x 32 B."""
+        out = (C.c_uint8 * (32 * max(n, 1)))()
+        self._check(self.lib.ed25519_b200_expanded_verifying_keys(self.h, _ptr(esks), n, C.addressof(out)))
+        return bytes(out)[:32 * n]
+
+    def raw_sign_flat(self, esks, vks, n_keys, msgs_flat, offsets, n):
+        """hazmat::raw_sign for n flat messages with n_keys = n or 1 (esk, verifying key) pairs -> n x 64 B."""
+        out = (C.c_uint8 * (64 * max(n, 1)))()
+        self._check(self.lib.ed25519_b200_raw_sign_flat(self.h, _ptr(esks), _ptr(vks), n_keys, _ptr(msgs_flat), _ptr(offsets), n,
+                                                        C.addressof(out)))
+        return bytes(out)[:64 * n]
+
+    def raw_sign_prehashed(self, esks, vks, n_keys, prehashes, n, context=None):
+        """hazmat::raw_sign_prehashed (Ed25519ph) for n 64-byte prehashes and one context: (rc, n x 64 B); rc 5 is
+        PrehashedContextLength."""
+        out = (C.c_uint8 * (64 * max(n, 1)))()
+        ctx = bytes(context) if context is not None else b""
+        rc = self._check(self.lib.ed25519_b200_raw_sign_prehashed(self.h, _ptr(esks), _ptr(vks), n_keys, _ptr(prehashes), n,
+                                                                  _ptr(ctx) if ctx else None, len(ctx), C.addressof(out)))
+        return rc, bytes(out)[:64 * n]
+
+    # ---- resident signing-key sets ----
+    def signing_key_set_new(self, keys, k, form):
+        """ed25519_b200_signing_key_set_new for k keys of form SIGNING_KEY_SEED / _KEYPAIR / _EXPANDED: (rc, handle or None,
+        status); rc 4 (PointDecompression) or 6 (MismatchedKeypair) is the status of the first failing keypair, and no
+        handle is made."""
+        h = C.c_void_p()
+        status = (C.c_uint8 * max(k, 1))()
+        rc = self._check(self.lib.ed25519_b200_signing_key_set_new(self.h, _ptr(keys), k, form, C.addressof(status), C.byref(h)))
+        return rc, (h if h.value else None), bytes(status)[:k]
+
+    def signing_key_set_len(self, handle):
+        return int(self.lib.ed25519_b200_signing_key_set_len(handle))
+
+    def signing_key_set_verifying_keys(self, handle):
+        k = self.signing_key_set_len(handle)
+        out = (C.c_uint8 * (32 * max(k, 1)))()
+        self._check(self.lib.ed25519_b200_signing_key_set_verifying_keys(handle, C.addressof(out)))
+        return bytes(out)[:32 * k]
+
+    def signing_key_set_destroy(self, handle):
+        self.lib.ed25519_b200_signing_key_set_destroy(handle)
+
+    def signing_key_set_sign_flat(self, handle, msgs_flat, offsets, indices, n, device_ptrs=False, out=None):
+        """Signer::try_sign of message i under key indices[i] of the set (n uint32, or None for key 0) -> n x 64 B.  With
+        device_ptrs every buffer, `out` included, is a device pointer and the call returns None."""
+        if device_ptrs:
+            self._check(self.lib.ed25519_b200_signing_key_set_sign_flat_dev(self.h, handle, _ptr(msgs_flat), _ptr(offsets),
+                                                                            _ptr(indices), n, _ptr(out)))
+            return None
+        res = (C.c_uint8 * (64 * max(n, 1)))()
+        self._check(self.lib.ed25519_b200_signing_key_set_sign_flat(self.h, handle, _ptr(msgs_flat), _ptr(offsets), _ptr(indices),
+                                                                    n, C.addressof(res)))
+        return bytes(res)[:64 * n]
+
+    def signing_key_set_sign_prehashed(self, handle, prehashes, indices, n, context=None):
+        """SigningKey::sign_prehashed of prehash i under key indices[i] of the set: (rc, n x 64 B); rc 5 is
+        PrehashedContextLength."""
+        res = (C.c_uint8 * (64 * max(n, 1)))()
+        ctx = bytes(context) if context is not None else b""
+        rc = self._check(self.lib.ed25519_b200_signing_key_set_sign_prehashed(self.h, handle, _ptr(prehashes),
+                                                                              _ptr(ctx) if ctx else None, len(ctx), _ptr(indices),
+                                                                              n, C.addressof(res)))
+        return rc, bytes(res)[:64 * n]
 
     def sign_batch_flat(self, seeds, msgs_flat, offsets, n):
         pks = (C.c_uint8 * (32 * max(n, 1)))()
@@ -1615,6 +1695,54 @@ def ed25519_sign_prehashed(seeds, prehashed, context=None, engine=None):
     return outs[0] if single else outs
 
 
+def _raw_sign_args(esks, vks, n):
+    single_e, es = _items(esks, 64, "ExpandedSecretKey bytes")
+    single_v, vs = _items(vks, 32, "verifying keys")
+    if len(es) != len(vs) or single_e != single_v:
+        raise ValueError("one verifying key per ExpandedSecretKey")
+    if not single_e and len(es) not in (1, n):
+        raise ValueError("one key, or one key per message")
+    return es, vs
+
+
+def ed25519_expanded_verifying_keys(esks, engine=None):
+    """VerifyingKey::from(&ExpandedSecretKey::from_bytes(esk)) (hazmat.rs:84-99, verifying.rs:97-102) for each 64-byte
+    ExpandedSecretKey (scalar bytes, then hash_prefix): one gives its 32-byte VerifyingKey, a list gives the list."""
+    single, es = _items(esks, 64, "ExpandedSecretKey bytes")
+    eng = engine or default_engine()
+    raw = eng.expanded_verifying_keys(b"".join(es), len(es))
+    outs = [raw[32 * i:32 * i + 32] for i in range(len(es))]
+    return outs[0] if single else outs
+
+
+def ed25519_raw_sign(esks, messages, verifying_keys, engine=None):
+    """hazmat::raw_sign::<Sha512> (hazmat.rs:137) on the GPU.  `messages` is one message or a list; `esks` is one 64-byte
+    ExpandedSecretKey, which signs every message, or one per message, and `verifying_keys` matches it.  The verifying keys
+    are hashed as given and not decoded: the caller makes sure they decode, as the reference's VerifyingKey type does."""
+    single = isinstance(messages, (bytes, bytearray))
+    msgs = [bytes(messages)] if single else [bytes(m) for m in messages]
+    es, vs = _raw_sign_args(esks, verifying_keys, len(msgs))
+    eng = engine or default_engine()
+    flat, offs, n = _flat_messages(msgs)
+    raw = eng.raw_sign_flat(b"".join(es), b"".join(vs), len(es), flat, offs, n) if n else b""
+    outs = [raw[64 * i:64 * i + 64] for i in range(n)]
+    return outs[0] if single else outs
+
+
+def ed25519_raw_sign_prehashed(esks, prehashed, verifying_keys, context=None, engine=None):
+    """hazmat::raw_sign_prehashed::<Sha512, Sha512> (hazmat.rs:182, Ed25519ph) on the GPU; `prehashed` as in
+    ed25519_sign_prehashed, keys as in ed25519_raw_sign.  Raises SignatureError(5) for a context longer than 255 bytes."""
+    single, phs = _prehash_items(prehashed)
+    es, vs = _raw_sign_args(esks, verifying_keys, len(phs))
+    eng = engine or default_engine()
+    n = len(phs)
+    rc, raw = eng.raw_sign_prehashed(b"".join(es), b"".join(vs), len(es) if n else 0, b"".join(phs), n, context)
+    if rc:
+        raise SignatureError(rc)
+    outs = [raw[64 * i:64 * i + 64] for i in range(n)]
+    return outs[0] if single else outs
+
+
 def ed25519_verify_prehashed(prehashed, signatures, verifying_keys, context=None, strict=False, engine=None):
     """VerifyingKey::verify_prehashed / verify_prehashed_strict (verifying.rs:230-257, :424-459) of each signature: the
     list of result codes (0 Ok, 1 Verify, 3 ScalarFormat, 4 PointDecompression), or one code for a single item.  A
@@ -1868,6 +1996,108 @@ class VerifyingKeySet:
     def close(self):
         if getattr(self, "h", None):
             self.eng.key_set_destroy(self.h)                   # does not use the engine's context: safe after its close()
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+SIGNING_KEY_SEED, SIGNING_KEY_KEYPAIR, SIGNING_KEY_EXPANDED = 0, 1, 2        # DALEK_SIGNING_KEY_*
+
+
+class SigningKeySet:
+    """k Ed25519 signing keys resident on the GPU: each key is derived once (its clamped scalar, hash_prefix and
+    verifying key stay in device memory until close(), which clears them), and every later call sends messages and key
+    indices only.  Make one with from_seeds, from_keypair_bytes or from_expanded."""
+
+    def __init__(self, keys, form, engine=None):
+        self.h = None
+        self.eng = engine or default_engine()
+        size = 32 if form == SIGNING_KEY_SEED else 64
+        _, ks = _items(list(keys), size, "keys of this form")
+        if not ks:
+            raise ValueError("a signing-key set needs at least one key")
+        rc, h, status = self.eng.signing_key_set_new(b"".join(ks), len(ks), form)
+        if rc:
+            err = SignatureError(rc)
+            err.args = ("%s: key %d" % (err.kind, next(i for i, c in enumerate(status) if c)),)
+            raise err
+        self.h, self.k, self._pks = h, len(ks), None
+
+    @classmethod
+    def from_seeds(cls, seeds, engine=None):
+        """SigningKey::from_bytes (signing.rs:106) for each 32-byte seed."""
+        return cls(seeds, SIGNING_KEY_SEED, engine)
+
+    @classmethod
+    def from_keypair_bytes(cls, keypairs, engine=None):
+        """SigningKey::from_keypair_bytes (signing.rs:140-150) for each 64-byte seed || verifying key.  Raises
+        SignatureError naming the first key whose public half does not decode (PointDecompression) or is not the key
+        derived from the seed, byte for byte (MismatchedKeypair)."""
+        return cls(keypairs, SIGNING_KEY_KEYPAIR, engine)
+
+    @classmethod
+    def from_expanded(cls, esks, engine=None):
+        """ExpandedSecretKey::from_bytes (hazmat.rs:84-99) for each 64 bytes (scalar bytes, then hash_prefix), with the
+        verifying key derived from it."""
+        return cls(esks, SIGNING_KEY_EXPANDED, engine)
+
+    def __len__(self):
+        return self.k
+
+    def verifying_keys(self):
+        """The 32-byte VerifyingKey of every key, in order."""
+        if self._pks is None:
+            raw = self.eng.signing_key_set_verifying_keys(self.h)
+            self._pks = [raw[32 * i:32 * i + 32] for i in range(self.k)]
+        return list(self._pks)
+
+    def verifying_key(self, i=0):
+        """SigningKey::verifying_key (signing.rs:171) of key i."""
+        if not 0 <= i < self.k:
+            raise IndexError("key index out of range")
+        return self.verifying_keys()[i]
+
+    def _indices(self, indices, n):
+        if indices is None:
+            return None
+        import array
+        idx = array.array("I", indices)
+        if len(idx) != n:
+            raise ValueError("one key index per message")
+        if n and max(idx) >= self.k:
+            raise ValueError("a key index is not below len()")
+        return idx.tobytes()
+
+    def sign(self, messages, indices=None):
+        """Signer::sign (signing.rs:566-571) of message i under key indices[i] (None: key 0).  One message (bytes) and
+        one index give one 64-byte signature; lists give the list."""
+        single = isinstance(messages, (bytes, bytearray))
+        msgs = [bytes(messages)] if single else [bytes(m) for m in messages]
+        idx = self._indices([indices] if single and indices is not None else indices, len(msgs))
+        flat, offs, n = _flat_messages(msgs)
+        raw = self.eng.signing_key_set_sign_flat(self.h, flat, offs, idx, n) if n else b""
+        outs = [raw[64 * i:64 * i + 64] for i in range(n)]
+        return outs[0] if single else outs
+
+    def sign_prehashed(self, prehashed, indices=None, context=None):
+        """SigningKey::sign_prehashed (signing.rs:312, Ed25519ph) of each prehash under key indices[i], as
+        ed25519_sign_prehashed.  Raises SignatureError(5) for a context longer than 255 bytes."""
+        single, phs = _prehash_items(prehashed)
+        idx = self._indices([indices] if single and indices is not None else indices, len(phs))
+        n = len(phs)
+        rc, raw = self.eng.signing_key_set_sign_prehashed(self.h, b"".join(phs), idx, n, context)
+        if rc:
+            raise SignatureError(rc)
+        outs = [raw[64 * i:64 * i + 64] for i in range(n)]
+        return outs[0] if single else outs
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.eng.signing_key_set_destroy(self.h)           # does not use the engine's context: safe after its close()
             self.h = None
 
     def __del__(self):

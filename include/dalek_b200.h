@@ -43,6 +43,7 @@ typedef struct dalek_b200_ctx dalek_b200_ctx;
 #define ED25519_ERR_SCALAR_FORMAT 3       /* InternalError::ScalarFormat       (E/errors.rs:27) */
 #define ED25519_ERR_POINT_DECOMPRESSION 4 /* InternalError::PointDecompression (E/errors.rs:26) */
 #define ED25519_ERR_PREHASHED_CONTEXT_LENGTH 5 /* InternalError::PrehashedContextLength (E/errors.rs:50) */
+#define ED25519_ERR_MISMATCHED_KEYPAIR 6  /* InternalError::MismatchedKeypair  (E/errors.rs:52) */
 /* engine errors */
 #define DALEK_E_INVALID_ARG (-1)
 #define DALEK_E_NO_DEVICE (-2)
@@ -94,7 +95,8 @@ int dalek_b200_last_stage_ms(const dalek_b200_ctx *ctx, const char *stage, float
  * / vartime_double_base_batch / MontgomeryPoint / mul_base_ct_batch / scalar_binary_batch / scalar_unary_batch /
  * scalar_from_bytes_batch / scalar_hash_from_bytes_batch / scalar_fold_batch call, or of the last ed25519_b200_verifying_keys /
  * sign_flat / sign_prehashed / verify_prehashed_each / key_set_new / key_set_verify_flat / key_set_verify_flat_dev /
- * key_set_verify_prehashed call, and after the last work it enqueued (all of the call's streams
+ * key_set_verify_prehashed / expanded_verifying_keys / raw_sign_flat / raw_sign_prehashed / signing_key_set_new /
+ * signing_key_set_sign_flat / signing_key_set_sign_flat_dev / signing_key_set_sign_prehashed call, and after the last work it enqueued (all of the call's streams
  * joined): the device time of that call, copies of host-buffer calls included. */
 int dalek_b200_last_call_ms(const dalek_b200_ctx *ctx, float *ms);
 
@@ -771,6 +773,87 @@ int ed25519_b200_key_set_verify_flat_dev(dalek_b200_ctx *ctx, const ed25519_b200
 int ed25519_b200_key_set_verify_prehashed(dalek_b200_ctx *ctx, const ed25519_b200_key_set *s, const uint8_t *prehashes,
                                           const uint8_t *context, size_t context_len, const uint8_t *sigs,
                                           const uint32_t *key_idx /* n, or NULL */, size_t n, int strict, uint8_t *results);
+
+/* -------- hazmat signing from expanded secret keys (secret-key operations) ---------------------------------------------
+ * ed25519_dalek::hazmat signs from an ExpandedSecretKey: keys that have no seed, such as hierarchically derived children,
+ * blinded keys or scalars from a threshold protocol.  esks holds 64-byte ExpandedSecretKey bytes: the low 32 bytes are
+ * the scalar bytes, the high 32 bytes hash_prefix.  ExpandedSecretKey::from_bytes (E/hazmat.rs:84-99) clamps the scalar
+ * bytes and reduces them mod l; any 64 bytes are accepted.  Secret: the esks and everything derived from them but the
+ * verifying keys and the signatures; constant time in them as the signer above, and their device copies are cleared
+ * before a call returns, failed calls included.  Host buffers, streamed in pieces; n = 0 is a successful no-op, a NULL
+ * buffer with n > 0 is DALEK_E_INVALID_ARG; flat messages as in the hash-to-group block.  No option affects these calls.
+ *
+ * VerifyingKey::from(&ExpandedSecretKey::from_bytes(esk)) (E/verifying.rs:97-102): n x 64 B esks -> n x 32 B
+ * compress([clamp(lo) mod l]B), which is compress([clamp(lo)]B). */
+int ed25519_b200_expanded_verifying_keys(dalek_b200_ctx *ctx, const uint8_t *esks, size_t n, uint8_t *pubkeys_out);
+/* hazmat::raw_sign::<Sha512> (E/hazmat.rs:137, E/signing.rs:854-904): sigs_out n x 64 B, signature i over message i under
+ * esk i and verifying key i (n_keys = n) or under esks[0] / vks[0] for every message (n_keys = 1; any other value is
+ * DALEK_E_INVALID_ARG).  vks (n_keys x 32 B) is hashed into the challenge exactly as given: a key that does not match
+ * the secret gives the reference's bytes for that key, not an error.  The call does not decode vks: in the reference the
+ * VerifyingKey type guarantees that the bytes decode, here the caller must.  With one key per message this costs one
+ * comb per signature, as A is supplied. */
+int ed25519_b200_raw_sign_flat(dalek_b200_ctx *ctx, const uint8_t *esks, const uint8_t *vks, size_t n_keys, const uint8_t *msgs_flat,
+                               const uint64_t *msg_offsets, size_t n, uint8_t *sigs_out);
+/* hazmat::raw_sign_prehashed::<Sha512, Sha512> (Ed25519ph, E/hazmat.rs:182, E/signing.rs:917-976): prehashes n x 64 B,
+ * one context for the batch as in ed25519_b200_sign_prehashed (context_len > 255 returns
+ * ED25519_ERR_PREHASHED_CONTEXT_LENGTH and writes nothing).  esks, vks and n_keys as in ed25519_b200_raw_sign_flat. */
+int ed25519_b200_raw_sign_prehashed(dalek_b200_ctx *ctx, const uint8_t *esks, const uint8_t *vks, size_t n_keys,
+                                    const uint8_t *prehashes, size_t n, const uint8_t *context, size_t context_len,
+                                    uint8_t *sigs_out);
+
+/* -------- resident signing-key sets (secret-key operations) ------------------------------------------------------------
+ * A service that signs at volume holds a fixed set of keys and signs each message under one of them.  A set derives its
+ * k keys once and keeps them in device memory: per key the clamped scalar and hash_prefix (64 B, secret) and the
+ * verifying key (32 B), plus a host copy of the verifying keys.  new allocates that memory and destroy clears the secret
+ * part and frees it; the set is not a context workspace and serves only the context that made it (another context is
+ * DALEK_E_INVALID_ARG).  Each signature costs one comb and no key derivation.  Constant time as the signer above; the
+ * key indices are public (which key signs a message is not secret in the reference either).
+ *
+ * new takes k >= 1 keys (k = 0 is DALEK_E_INVALID_ARG) in one form:
+ *   DALEK_SIGNING_KEY_SEED      32 B SecretKey each: SigningKey::from_bytes (E/signing.rs:106).
+ *   DALEK_SIGNING_KEY_KEYPAIR   64 B seed || public half each: SigningKey::from_keypair_bytes (E/signing.rs:140-150).
+ *       status[i] = ED25519_ERR_POINT_DECOMPRESSION when the public half does not decode (checked first, as
+ *       VerifyingKey::try_from runs first in the reference), else ED25519_ERR_MISMATCHED_KEYPAIR when it is not
+ *       byte-equal to the derived verifying key (equality is on bytes, E/verifying.rs:91-95, so a non-canonical
+ *       encoding of the right point is a mismatch).
+ *   DALEK_SIGNING_KEY_EXPANDED  64 B ExpandedSecretKey bytes each: ExpandedSecretKey::from_bytes (E/hazmat.rs:84-99),
+ *       the verifying key derived as in ed25519_b200_expanded_verifying_keys.
+ * Any other form is DALEK_E_INVALID_ARG.  status (k bytes, nullable) is 0 for every key that is fine.  Any nonzero status
+ * leaves *out NULL and nothing allocated, and the call returns the status of the first failing key.  A failed allocation
+ * returns DALEK_E_NOMEM with last_error set and no set.  The staged secret bytes are cleared before the call returns. */
+#define DALEK_SIGNING_KEY_SEED 0
+#define DALEK_SIGNING_KEY_KEYPAIR 1
+#define DALEK_SIGNING_KEY_EXPANDED 2
+typedef struct ed25519_b200_signing_key_set ed25519_b200_signing_key_set;
+int ed25519_b200_signing_key_set_new(dalek_b200_ctx *ctx, const uint8_t *keys /* k x 32 or 64 B */, size_t k, int form,
+                                     uint8_t *status /* k, nullable */, ed25519_b200_signing_key_set **out);
+size_t ed25519_b200_signing_key_set_len(const ed25519_b200_signing_key_set *s);
+/* the k x 32 B verifying keys (SigningKey::verifying_key, E/signing.rs:171), from the host copy: no device access.
+ * Returns 0, or DALEK_E_INVALID_ARG for a NULL argument. */
+int ed25519_b200_signing_key_set_verifying_keys(const ed25519_b200_signing_key_set *s, uint8_t *pubkeys_out);
+/* destroy clears the secret device memory, waits for the device and frees the set; it does not use the context, so a
+ * set may be destroyed before or after its context.  NULL is a no-op. */
+void ed25519_b200_signing_key_set_destroy(ed25519_b200_signing_key_set *s);
+/* Signer::try_sign (E/signing.rs:566-571) of message i under key key_idx[i] of the set (key_idx NULL: key 0 for every
+ * message): sigs_out n x 64 B, the bytes ed25519_b200_sign_flat gives with that key's seed (or raw_sign with that
+ * ExpandedSecretKey and its derived verifying key).  n = 0 is a successful no-op; a NULL sigs_out with n > 0 is
+ * DALEK_E_INVALID_ARG; flat messages as in the hash-to-group block.  An index >= k is DALEK_E_INVALID_ARG before any
+ * device work.  The batch is streamed in pieces. */
+int ed25519_b200_signing_key_set_sign_flat(dalek_b200_ctx *ctx, const ed25519_b200_signing_key_set *s, const uint8_t *msgs_flat,
+                                           const uint64_t *msg_offsets, const uint32_t *key_idx /* n, or NULL */, size_t n,
+                                           uint8_t *sigs_out);
+/* same with messages, offsets, indices and signatures in device memory; blocks until done.  An index >= k is never used
+ * as an address: that message's signature is 64 zero bytes (never a signature under another key, which a caller that
+ * ignores the return code could not tell from a good one), every other message is signed, and the call returns
+ * DALEK_E_INVALID_ARG after the batch ran. */
+int ed25519_b200_signing_key_set_sign_flat_dev(dalek_b200_ctx *ctx, const ed25519_b200_signing_key_set *s, const void *d_msgs_flat,
+                                               const void *d_msg_offsets, const void *d_key_idx, size_t n, void *d_sigs_out);
+/* SigningKey::sign_prehashed (Ed25519ph, E/signing.rs:312, :917-976) of prehash i (n x 64 B) under key key_idx[i], one
+ * context for the batch as in ed25519_b200_sign_prehashed: context_len > 255 returns ED25519_ERR_PREHASHED_CONTEXT_LENGTH
+ * and writes nothing.  Other rules as ed25519_b200_signing_key_set_sign_flat. */
+int ed25519_b200_signing_key_set_sign_prehashed(dalek_b200_ctx *ctx, const ed25519_b200_signing_key_set *s, const uint8_t *prehashes,
+                                                const uint8_t *context, size_t context_len, const uint32_t *key_idx /* n, or NULL */,
+                                                size_t n, uint8_t *sigs_out);
 
 /* -------- input synthesis (benchmarks / tests): fixed-base multiples and keys + signatures ---- */
 /* out[i] = scalars[i] * B as extended limbs (EdwardsPoint::mul_base, C/edwards.rs:918-928).  Public scalars only:
